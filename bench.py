@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the VisualCLA hot path on B200 (contract: see the task's section (4) and DESIGN.md "Measurement").
+"""Benchmark of the VisualCLA hot path on H100 (see DESIGN.md "Measurement").
 
 A "step" = one pass of the whole path over one batch of synthetic requests:
     B images (224x224) + 64-token prompts -> ViT-L/14 -> Resampler -> projector -> LLaMA-7B prefill (S = 128)
@@ -9,6 +9,7 @@ metric = images+256-token generations per second (whole job, all GPUs).
   python bench.py --gpus 1 --steps 5 --warmup 3            # this repo's CUDA path
   python bench.py --impl reference ...                      # reference algorithm on the host cores (CPU oracle port)
   torchrun --nproc-per-node N bench.py --gpus N ...         # data parallel, one rank per GPU, weak scaling
+  python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs bench_outputs   # + the last timed step's outputs as .npy
 """
 import argparse
 import json
@@ -43,6 +44,8 @@ def parse():
                     help="weak: --batch-per-gpu requests on every GPU; strong: a fixed global batch of 64 (SURVEY 8d config 4: B_local = 64/N)")
     ap.add_argument("--no-extras", action="store_true", help="skip the configs[2] / configs[4] / strong-scaling / HF-CUDA blocks of the default line")
     ap.add_argument("--pdl", type=int, default=int(os.environ.get("VCLA_PDL", "1")))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (rank 0's generated token ids) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -51,7 +54,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sus=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, source="fallback")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sus=989.0, source="H100 SXM data-sheet")
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -295,7 +298,7 @@ def run_config(args, world, rank, Bl, T, n_new, steps, warmup, with_e2e, with_tr
     eng.kernel_launches(reset=True)
     with ClockSampler(int(os.environ.get("LOCAL_RANK", "0"))) as clocks:
         ms, out = timed(step_device, steps)
-    res = {"B_local": Bl, "B": B, "T": T, "S": S, "n_new": n_new, "ms": ms, "steps": steps, "value": B * steps / (ms / 1000.0),
+    res = {"B_local": Bl, "B": B, "T": T, "S": S, "n_new": n_new, "ms": ms, "steps": steps, "value": B * steps / (ms / 1000.0), "outputs": {"tokens": out},
            "launches": eng.kernel_launches(reset=True), "clocks": clocks.summary()}
     pre_ms = [a.elapsed_time(b) for a, b in zip(ev.get("start", []), ev.get("prefill_done", []))]
     dec_ms = [a.elapsed_time(b) for a, b in zip(ev.get("prefill_done", []), ev.get("done", []))]
@@ -366,6 +369,18 @@ def hf_cuda_sample(B, T, n_new, dtype="float16", steps=2):
     return run_hf_cuda(ns, emit=False)
 
 
+def dump_outputs(path, outputs):
+    """Write each output of the timed path's last step as <path>/<name>.npy (float64: token ids are exact; 64 MB at most)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    total = 0
+    for name, t in outputs.items():
+        a = t.detach().cpu().double().numpy()
+        total += a.nbytes
+        assert total <= 64 << 20, f"outputs exceed 64 MB ({total} bytes)"
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def run_native(args):
     import torch
     import torch.distributed as dist
@@ -387,6 +402,8 @@ def run_native(args):
     Bl, n_new, T = args.batch_per_gpu, args.new_tokens, args.prompt_tokens
     B, S = Bl * world, T + NQ
     main = run_config(args, world, rank, Bl, T, n_new, args.steps, args.warmup, with_e2e=True, with_trace=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, main["outputs"])
     pk = peaks()
     cfg_name = {(8, 64, 256): "1", (32, 128, 256): "2", (16, 1024, 512): "4"}.get((Bl, T, n_new), "*")
     line = {"metric": METRIC, "value": main["value"], "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -394,18 +411,18 @@ def run_native(args):
             "data": "synthetic (randn 224x224 pixels, uniform random token ids, hash-normal weights of the VisualCLA-7B architecture)",
             "config": {"workload": f"configs[{cfg_name}]: batch {Bl} per GPU x {world} GPU, 224x224 images, {T}-token prompts (S={S} with 64 image tokens), "
                                    f"{n_new}-token greedy decode, EOS disabled", "global_batch": B, "parallelism": f"dp{world}",
-                       "l2": "inputs larger than L2: every decode step streams 13.4 GB of weights (>> 126 MB L2)", "pdl": bool(args.pdl),
+                       "l2": "inputs larger than L2: every decode step streams 13.4 GB of weights (>> 50 MB L2)", "pdl": bool(args.pdl),
                        "token_exchange": "none (1 GPU)" if world == 1 else "NCCL all-gather of the chosen tokens inside the decode CUDA graphs (vcla_nccl_init)"},
             "e2e": main["e2e"], "gpu_launches": int(main["launches"]), "clocks": main["clocks"]}
     if "phases" in main:
         line["phases"] = main["phases"]
     if "sampling" in main:
         line["sampling"] = main["sampling"]
-    line["config"]["schedule"] = ("prefill: 5 kernels/layer (deferred RMSNorm + RoPE/KV-append + SwiGLU + residual epilogues in the tcgen05 GEMM, CTA-pair 256x256 "
-                                  "tiles, tcgen05 flash attention); decode: 5 kernels/layer (cluster split-K GEMMs with DSMEM reduce and fused consumers), "
+    line["config"]["schedule"] = ("prefill: 5 kernels/layer (deferred RMSNorm + RoPE/KV-append + SwiGLU + residual epilogues in the wgmma GEMM, "
+                                  "wgmma flash attention); decode: 5 kernels/layer (cluster split-K GEMMs with DSMEM reduce and fused consumers), "
                                   "CUDA graphs of 16 steps")
     if rank == 0:
-        # ---- roofline of the dominant kernel, IN SITU: the fused gate/up swap-AB tcgen05 GEMM (180.4 MB of weights per launch, the
+        # ---- roofline of the dominant kernel, IN SITU: the fused gate/up decode GEMM (180.4 MB of weights per launch, the
         #      largest share of a decode step), timed inside a graph-replayed decode step; the isolated micro-benchmark (32 launches
         #      back to back, PDL weight prefetch overlapping neighbours) is reported beside it, not as the headline.
         traffic = None
@@ -415,7 +432,7 @@ def run_native(args):
         iso = main.get("isolated", {})
         ins = main.get("insitu_us", {})
         rf = {"bound": "hbm", "peak": pk["hbm"], "unit": "GB/s", "traffic": traffic,
-              "kernel": "gemm_tc_kernel<BN,5,swap-AB> fused gate/up projection (22016x4096 bf16 weights, 180.4 MB algorithmic bytes per launch)",
+              "kernel": "gemm_csk_kernel fused gate/up projection (22016x4096 bf16 weights, 180.4 MB algorithmic bytes per launch)",
               "of": pk["source"] + " copy bandwidth"}
         if "gate_up" in ins:
             us = ins["gate_up"]
@@ -484,7 +501,7 @@ def run_native(args):
 # ----------------------------------------------------------------------------------------------------------------
 # informational arm: the reference's CUDA path = HF CLIPVisionModel + the Resampler arithmetic in torch + HF
 # LlamaForCausalLM.generate(inputs_embeds=...) on the same GPU, same shapes, random weights (north star's 8x denominator).
-# /root/reference is not on the GPU box, so the composite module is re-assembled from the very HF classes it calls
+# The reference itself is not needed: the composite module is re-assembled from the very HF classes it calls
 # (modeling_visualcla.py:346-391) and the oracle's torch restatement of the in-repo Resampler, run on the device.
 # ----------------------------------------------------------------------------------------------------------------
 def run_hf_cuda(args, emit=True):

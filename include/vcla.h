@@ -1,5 +1,5 @@
 /*
- * vcla.h -- C ABI of the B200-native VisualCLA multimodal forward path (libvcla.so).
+ * vcla.h -- C ABI of the H100-native VisualCLA multimodal forward path (libvcla.so).
  *
  * This is the drop-in boundary for ONE hot path of airaria/Visual-Chinese-LLaMA-Alpaca:
  *   image + prompt -> CLIP-ViT-L/14 -> post_layernorm -> 6-layer Resampler -> projector
@@ -209,7 +209,7 @@ int64_t vcla_kernel_launches(vcla_ctx* ctx, int reset);
 int vcla_read_stage(vcla_ctx* ctx, const char* stage, int B, float* dst_host, vcla_stream stream);
 
 /* ---- operator-level entry points (kernel parity tests, micro-benchmarks) ---------------------- */
-/* D = A[M,K] * W[N,K]^T on the tcgen05 path.  mode: 0 store bf16 (act: 0 none, 1 quick_gelu, 2 gelu),
+/* D = A[M,K] * W[N,K]^T on the wgmma path.  mode: 0 store bf16 (act: 0 none, 1 quick_gelu, 2 gelu),
  * 1 fp32 (accumulate flag), 2 SwiGLU (W rows interleaved [32 gate|32 up]), 3 swap-AB split-K partials
  * (out f32 [splits][M_b][N] with A = weights).  use_reference != 0 runs the naive CUDA-core kernel instead. */
 int vcla_op_gemm(const void* A_dev_bf16, const void* W_dev_bf16, int M, int N, int K, int mode, int act, int accumulate,
@@ -226,10 +226,8 @@ int vcla_op_gemm_csk_clusters(int B, int splits);
 /* tuning hooks: read / override the CTAs-per-cluster of the five decode GEMM shapes {qkv, o, gate_up, down, lm_head} at batch B */
 int vcla_debug_set_csk_splits(vcla_ctx* ctx, int B, int qkv, int o, int gate_up, int down, int lm_head);
 int vcla_debug_get_csk_splits(vcla_ctx* ctx, int B, int* out5);
-/* CTA-pair (tcgen05 cta_group::2, 256 x 256) tiles for the 256-wide prefill GEMMs: on by default; 0 selects the single-CTA 128 x 256 tile */
-void vcla_set_gemm_two_cta(int on);
-/* prefill attention kernel: 0 = the mma.sync kernel everywhere, 1 (default) = tcgen05 flash attention (QK^T / PV as UMMA, S and O in TMEM,
- * TMA operands) at head dim 128 (LLaMA prefill) and mma.sync at head dim 64 (ViT / Resampler), 2 = tcgen05 everywhere */
+/* prefill attention kernel: 0 = the mma.sync kernel everywhere, 1 (default) = wgmma flash attention (QK^T / PV on the warpgroup tensor
+ * cores, S and O in registers, TMA operands) at head dim 128 (LLaMA prefill) and mma.sync at head dim 64 (ViT / Resampler), 2 = wgmma everywhere */
 void vcla_set_attention_tc(int mode);
 int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v0, int kv0_stride, int n0, const void* k1,
                       const void* v1, int kv1_stride, int n1, void* out, int o_stride, int B, int H, int Sq, int HD, float scale,

@@ -8,7 +8,7 @@ What it restates
   (models/visualcla/modeling_utils.py:130 builds it, :150/:152/:187/:189 call it); in the reference's pinned
   transformers (4.x) that is the PIL/numpy pipeline of HF:models/clip/image_processing_clip.py:22-33
       convert RGB -> resize(shortest_edge=224, BICUBIC) -> center_crop(224,224) -> rescale(1/255) -> normalize(mean,std)
-  whose only non-trivial arithmetic lives in a third-party dependency that is not vendored in /root/reference:
+  whose only non-trivial arithmetic lives in a third-party dependency that is not vendored in the reference:
   Pillow's `ImagingResample` (src/libImaging/Resample.c; behaviour unchanged across Pillow 7 … 12).  Its published
   algorithm for 8-bit images is restated below in integer numpy: separable, antialiased (filter support scaled by the
   down-scaling factor), coefficients quantised to 22 fractional bits, a rounding shift and an 8-bit clip after EACH pass,

@@ -1,7 +1,6 @@
-"""Import shim that lets the UNMODIFIED reference package (`/root/reference/models/visualcla`)
-import and run under the installed transformers 5.5.0.  TEST INFRASTRUCTURE ONLY
-(used by oracle/gen_golden.py in the authoring container; /root/reference does not exist
-on the GPU box, nothing at run time there imports this).
+"""Import shim that lets the UNMODIFIED reference package (`<reference checkout>/models/visualcla`, located by
+$VCLA_REFERENCE_MODELS = `<reference checkout>/models`) import and run under transformers 5.5.0.  TEST INFRASTRUCTURE ONLY
+(used by oracle/gen_golden.py to produce tests/golden; no test and nothing at run time imports this).
 
 Why each patch is needed (SURVEY.md section 8c):
   * transformers.pytorch_utils.find_pruneable_heads_and_indices   removed in 5.x
@@ -16,7 +15,7 @@ Why each patch is needed (SURVEY.md section 8c):
 import os
 import sys
 
-REFERENCE_MODELS = os.environ.get("VCLA_REFERENCE_MODELS", "/root/reference/models")
+REFERENCE_MODELS = os.environ.get("VCLA_REFERENCE_MODELS", "")
 
 
 def import_reference():

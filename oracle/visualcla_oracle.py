@@ -13,14 +13,14 @@ Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline /
 Pinning status: the reference repo has no tests / golden vectors of its own
 (SURVEY.md section 4, 8c).  This oracle is pinned against *outputs of the reference
 itself* run in the authoring container: `oracle/gen_golden.py` imports the
-unmodified reference (`/root/reference/models/visualcla`, behind the import shim
+unmodified reference (`models/visualcla` of a reference checkout, behind the import shim
 in `oracle/ref_shim.py`) plus HF transformers 5.5.0 CLIP/LLaMA, runs
 `VisualCLAModel.forward/.generate` on seeded weights and writes
 `tests/golden/*.npz`; `tests/test_oracle_golden.py` checks this restatement
 against those files.
 
 Every function cites the reference lines it restates.  `ref:` paths are relative
-to /root/reference, `HF:` paths to site-packages/transformers (5.5.0).
+to the reference repository's root, `HF:` paths to site-packages/transformers (5.5.0).
 """
 from __future__ import annotations
 

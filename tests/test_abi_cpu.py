@@ -94,7 +94,7 @@ def test_config_struct_matches_header():
 
 
 def test_version_and_error_strings(lib):
-    assert b"sm_100a" in lib.vcla_version()
+    assert b"sm_90a" in lib.vcla_version()
     assert isinstance(lib.vcla_last_error(), bytes)
 
 

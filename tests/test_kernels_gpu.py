@@ -83,7 +83,7 @@ def test_gemm_f32_residual(lib, M, N, K, accumulate):
 
 
 def test_gemm_matches_naive_kernel(lib):
-    """tcgen05 path vs the CUDA-core reference kernel inside the library (same epilogue semantics)."""
+    """wgmma path vs the CUDA-core reference kernel inside the library (same epilogue semantics)."""
     M, N, K = 200, 320, 448
     A, W = _rand((M, K), 1.0, 7), _rand((N, K), 1.0 / math.sqrt(K), 8)
     o1 = torch.zeros((M, N), device="cuda")
@@ -135,10 +135,11 @@ def _attn_ref(q, k, v, scale, causal):
     return (torch.softmax(s, -1) @ vf).transpose(1, 2)
 
 
+# The ids are stable test names: "tcgen05" labels VCLA_ATTN_TC mode 2, the tensor-core kernel of csrc/attention_tc.cu (wgmma on sm_90a).
 @pytest.fixture(params=[0, 2], ids=["mma_sync", "tcgen05"])
 def attn_impl(request, lib):
-    """Both prefill attention kernels behind the same entry point: the mma.sync one (csrc/attention.cu) and the tcgen05 one
-    (csrc/attention_tc.cu: QK^T and PV as UMMA, S / O in TMEM, TMA operands)."""
+    """Both prefill attention kernels behind the same entry point: the mma.sync one (csrc/attention.cu) and the wgmma one
+    (csrc/attention_tc.cu: QK^T and PV on the warpgroup tensor cores, S / O in registers, TMA operands)."""
     lib.vcla_set_attention_tc(request.param)
     yield request.param
     lib.vcla_set_attention_tc(int(__import__("os").environ.get("VCLA_ATTN_TC", "1")))
@@ -258,24 +259,3 @@ def test_csk_swiglu(lib, F, K, B, S):
     rstd = torch.rsqrt(ssq.sum(1) / K + 1e-6)[:, None]
     ref = torch.nn.functional.silu((X.float() @ g.float().t()) * rstd) * ((X.float() @ u.float().t()) * rstd)
     assert (h.float() - ref).abs().max().item() <= 1.5e-2 * max(1.0, ref.abs().max().item())
-
-
-def test_two_cta_tiles_match_single_cta(lib):
-    """cta_group::2 (CTA pair, 256 x 256 tiles) vs the single-CTA 128 x 256 tile: same inputs, same epilogues, bit-identical outputs
-    (the K order of the accumulation is the same), odd tile counts and ragged edges included."""
-    for M, N, K in [(1024, 12288, 4096), (2056, 4096, 1024), (300, 1003, 640), (129, 512, 64)]:
-        A, W = _rand((M, K), 1.0, 21), _rand((N, K), 1.0 / math.sqrt(K), 22)
-        bias = torch.randn(N, device="cuda")
-        outs = []
-        for two in (1, 0):
-            lib.vcla_set_gemm_two_cta(two)
-            out = torch.full((M, N), float("nan"), dtype=torch.bfloat16, device="cuda")
-            _gemm(lib, A, W, 0, bias=bias, out=out, ldo=N, tile_n=256)
-            base = torch.randn(M, N, generator=torch.Generator().manual_seed(3)).cuda()
-            acc = base.clone()
-            _gemm(lib, A, W, 1, accumulate=1, bias=bias, out=acc, ldo=N, tile_n=256)
-            outs.append((out, acc))
-        lib.vcla_set_gemm_two_cta(1)
-        ref = A.float() @ W.float().t() + bias
-        assert (outs[0][0].float() - ref).abs().max().item() <= 2e-2 * max(1.0, ref.abs().max().item())
-        assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1]), (M, N, K)

@@ -18,11 +18,10 @@ import visualcla_oracle as O
 
 pytestmark = pytest.mark.gpu
 
-# Gates = ~1.5x the error measured on B200 (profiles/r2_parity_measured.json; every run appends its measured values to
-# $VCLA_PARITY_LOG when set).  north_star's "1e-3" is below what ANY bf16 path reaches against an fp32 oracle -- see
+# Gates = ~1.5x the measured error (every run appends its measured values to $VCLA_PARITY_LOG when set).  north_star's "1e-3" is below what ANY bf16 path reaches against an fp32 oracle -- see
 # test_7b_error_not_worse_than_hf_bf16, which measures HF's own bf16 path on the same GPU, weights and inputs.
-STAGE_TOL = {"vit_out": 6e-3, "post_ln": 6e-3, "resampler_out": 1.7e-2, "projector_out": 1.5e-2}   # relative to the stage's max |value|; measured 3.7e-3 / 4.0e-3 / 1.12e-2 / 9.4e-3
-LOGIT_TOL = 1.5e-2    # relative to max |logit| (measured: 4.9e-3 .. 7.9e-3 on the mid / 7B configs)
+STAGE_TOL = {"vit_out": 6e-3, "post_ln": 6e-3, "resampler_out": 1.7e-2, "projector_out": 1.5e-2}   # relative to the stage's max |value|
+LOGIT_TOL = 1.5e-2    # relative to max |logit|
 LOGIT_TOL_TINY = 3.0e-2   # the 2-layer tiny reference goldens measure 1.3e-2 .. 2.05e-2 depending on the attention kernel (few, narrow layers:
                           # a max-abs metric over little averaging of the bf16 roundings)
 LOSS_TOL = 3e-2       # absolute, cross-entropy in nats (measured 1.3e-2 on the tiny goldens: ~1 % logit error at |logit| ~ 17)
@@ -335,6 +334,7 @@ def test_lora_fold_at_load(tmp_path):
     assert _rel_err(got, ref) <= LOGIT_TOL
 
 
+# "tcgen05" is the stable id of VCLA_ATTN_TC mode 2, the tensor-core kernel of csrc/attention_tc.cu (wgmma on sm_90a)
 @pytest.mark.parametrize("impl", [0, 2], ids=["mma_sync", "tcgen05"])
 def test_prefill_attention_kernels_end_to_end(golden_dir, impl):
     """Both prefill attention kernels through the whole path: ViT (257 tokens, hd 64), Resampler (two KV segments), LLaMA causal

@@ -3,7 +3,7 @@ oracle/clip_preprocess_oracle.py: integer work, so the bar is bit-exact (float32
 round-to-nearest cast of it).
 
 The per-thread code of both kernels is also replayed on the host bit for bit by tests/test_preprocess_core_cpu.py; these tests
-ran green on a B200 in round 1 (7 passed as XPASS), so they are ordinary tests now: a mismatch fails the suite."""
+are ordinary tests: a mismatch fails the suite."""
 import hashlib
 import os
 

@@ -1,4 +1,4 @@
-"""Tuning sweep of the cluster split-K decode GEMMs (csrc/gemm_decode.cu) on a B200: for every decode GEMM shape and every cluster size S,
+"""Tuning sweep of the cluster split-K decode GEMMs (csrc/gemm_decode.cu) on one GPU: for every decode GEMM shape and every cluster size S,
 the kernel timed alone over 32 layers' distinct weights (vcla_bench_decode_gemm), then whole decode steps for a few S combinations.
     python tools/csk_sweep.py <batch> [out.json]
 """

@@ -1,4 +1,4 @@
-"""Tile-shape sweep of the prefill tcgen05 GEMM on the path's shapes (TFLOP/s per tile N)."""
+"""Tile-shape sweep of the prefill wgmma GEMM on the path's shapes (TFLOP/s per tile N)."""
 import ctypes as C
 import os
 import sys

@@ -1,6 +1,6 @@
-"""Measure the device image pre-processing (csrc/preprocess.cu) on a B200 with the reference's CPU path timed beside it.
+"""Measure the device image pre-processing (csrc/preprocess.cu) on one GPU with the reference's CPU path timed beside it.
 
-    python tools/preprocess_bench.py [--sizes 480x640,1080x1920,3000x4000] [--reps 200] > profiles/rN_preprocess.jsonl
+    python tools/preprocess_bench.py [--sizes 480x640,1080x1920,3000x4000] [--reps 200]
 
 Per picture size one JSON line:
   device_us        both kernels + the tap-table upload, CUDA events on the launching stream, picture already in HBM
@@ -33,7 +33,7 @@ def hbm_peak_gbps():
                 return float(v["burst"] if isinstance(v, dict) and "burst" in v else v), "MEASURED_PEAKS.json"
     except Exception:
         pass
-    return 6500.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data-sheet"
 
 
 def algorithmic_bytes(proc, h, w, side=224):

@@ -1,6 +1,6 @@
 """Targets for ncu: runs only the kernel of interest so `ncu -k regex:... -s N -c 3` lands on it.
   python tools/profile_gemm.py decode [which] [B]   -> decode swap-AB weight-streaming GEMM over the 32 layers' weights
-  python tools/profile_gemm.py prefill              -> prefill tcgen05 GEMM  (1024 x 12288 x 4096, tile 128x256)
+  python tools/profile_gemm.py prefill              -> prefill wgmma GEMM  (1024 x 12288 x 4096, tile 64x256)
   python tools/profile_gemm.py step [B]             -> one full prefill + 4 decode steps (launch list)"""
 import ctypes as C
 import os

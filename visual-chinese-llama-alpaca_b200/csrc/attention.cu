@@ -4,7 +4,7 @@
 //                      (64 queries over [64 query-rows ; 257 image rows] = two KV segments, hd 64) and LLaMA prefill
 //                      (causal, hd 128).  Attention is <3 % of the path's FLOPs (SURVEY section 8a), so this uses the
 //                      register-fragment tensor path (mma.sync m16n8k16) with fp32 online softmax; the dense
-//                      contractions that dominate run on tcgen05 (gemm.cu).
+//                      contractions that dominate run on wgmma (gemm.cu).
 //  attention_decode  : one new token per sequence against the paged KV cache.  HBM-bound.  Fuses: split-K
 //                      reduction of the QKV projection partials, RoPE, KV-cache append, split-KV attention and the
 //                      final cross-split combine (last-arriving CTA, fixed order => deterministic).
@@ -194,14 +194,13 @@ __global__ void __launch_bounds__(128) attn_prefill_kernel(const AttnCall c) {
   }
 }
 
-// 0 = mma.sync kernel for everything, 1 (default) = tcgen05 kernel where it is the faster one on B200 (head dim 128: LLaMA prefill),
-// 2 = tcgen05 kernel for everything it can describe (tests).  Measured under ncu (profiles/r2_ncu_kernels.json, attn reports): the
-// ViT's 257 tokens at head dim 64 waste a third of the 128-row UMMA tiles and stay on mma.sync (25.8 vs 42 us per launch at batch 8).
+// 0 = mma.sync kernel for everything, 1 (default) = wgmma kernel at head dim 128 (LLaMA prefill), mma.sync at head dim 64 (ViT,
+// Resampler: short sequences, few KV tiles per CTA), 2 = wgmma kernel for everything it can describe (tests).
 static int g_attn_tc = -1;
 void attention_set_tc(int mode) { g_attn_tc = mode < 0 ? 0 : (mode > 2 ? 2 : mode); }
 int attention_prefill(const AttnCall& c, cudaStream_t st) {
   if (g_attn_tc < 0) { const char* e = getenv("VCLA_ATTN_TC"); g_attn_tc = (e != nullptr) ? atoi(e) : 1; if (g_attn_tc < 0 || g_attn_tc > 2) g_attn_tc = 1; }
-  // the tcgen05 kernel needs TMA-describable operands (16 B aligned, 16 B-multiple pitches) and one KV segment when causal
+  // the wgmma kernel needs TMA-describable operands (16 B aligned, 16 B-multiple pitches) and one KV segment when causal
   const bool tma_ok = (c.q_stride % 8) == 0 && (c.kv0_stride % 8) == 0 && (c.n1 == 0 || (c.kv1_stride % 8) == 0) && (c.o_stride % 8) == 0 &&
                       !(c.causal && c.n1 > 0);
   const bool want_tc = g_attn_tc == 2 || (g_attn_tc == 1 && c.HD == 128);

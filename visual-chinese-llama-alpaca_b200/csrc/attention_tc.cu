@@ -1,20 +1,17 @@
-// tcgen05 flash attention for the prefill side of the path (sm_100a): LLaMA's causal prefill (hd 128) by default; it also covers
+// wgmma flash attention for the prefill side of the path (sm_90a): LLaMA's causal prefill (hd 128) by default; it also covers
 // ViT self-attention (257 tokens, hd 64) and the Resampler's 64 queries over [their own 64 rows ; 257 image rows] (two KV segments,
-// hd 64), which the default dispatch leaves on the mma.sync kernel because the 128-row tile wastes a third of its work there
-// (attention.cu: attention_prefill; VCLA_ATTN_TC=2 forces this kernel everywhere, and the tests run it on every shape).
+// hd 64), which the default dispatch leaves on the mma.sync kernel (attention.cu: attention_prefill; VCLA_ATTN_TC=2 forces this
+// kernel everywhere, and the tests run it on every shape).
 //
-// One CTA per (128 query rows, head, sequence).  Both contractions run on the 5th-generation tensor cores:
-//   S = Q K^T   UMMA 128 x 128 x HD   A = Q tile, B = K tile, both K-major [rows][64-element k-blocks] staged by TMA (128 B swizzle);
-//               fp32 scores in TMEM
-//   O += P V    UMMA 128 x HD x 128   A = P (bf16 probabilities written by the softmax warps into shared memory in the same K-major
-//               swizzled layout), B = V tile exactly as TMA delivers it ([kv rows][64 head dims] = an MN-major operand: the
-//               instruction descriptor's b_major bit + a matrix descriptor with SBO = 8 rows, LBO = the next 64 head dims)
-// O accumulates in TMEM; the online-softmax rescale (O *= exp2(m_old - m_new)) is a tcgen05.ld / multiply / tcgen05.st of the row
-// by the thread that owns it, between the PV MMAs of consecutive tiles.
-//
-// Warps: 0 = TMA producer (Q once, then the K/V tiles), 1 = MMA issuer + TMEM owner, 2..5 = softmax / rescale /
-// epilogue (thread t owns query row t = TMEM lane t).  Masks: keys past a segment's end, causal (key <= query + Sk - Sq), left padding
-// (kv_start).  Fully masked rows produce zeros, like the mma.sync kernel (csrc/attention.cu).
+// One CTA per (64 query rows, head, sequence); one warpgroup computes, one warp loads.  Both contractions run on wgmma:
+//   S = Q K^T   m64n64k16 x HD/16   A = Q tile, B = K tile, both K-major [64-element k-blocks][64 rows][128 B] staged by TMA
+//               (128 B swizzle); fp32 scores in registers
+//   O += P V    m64nHDk16 x 4       A = P from registers (the score fragment rounded to bf16 IS the A fragment layout), B = V tile
+//               exactly as TMA delivers it ([head-dim block][kv rows][64 head dims] = an MN-major operand: transpose bit + a
+//               descriptor with SBO = 8 kv rows, LBO = the next 64 head dims)
+// O accumulates in registers; the online-softmax rescale (O *= exp2(m_old - m_new)) is a multiply of the thread's fragment rows.
+// K/V tiles are double buffered, two CTAs share an SM.  Masks: keys past a segment's end, causal (key <= query + Sk - Sq), left
+// padding (kv_start).  Fully masked rows produce zeros, like the mma.sync kernel (csrc/attention.cu).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -24,8 +21,9 @@
 
 namespace vcla {
 
-constexpr int kAtThreads = 192;
-constexpr int kAtBQ = 128, kAtBKV = 128;
+constexpr int kAtThreads = 160;                 // warps 0..3 = the wgmma warpgroup, warp 4 = TMA producer
+constexpr int kAtBQ = 64, kAtBKV = 64;
+constexpr int kAtStages = 2;
 
 struct AttnTcParams {
   int Sq, n0, n1, H;
@@ -38,38 +36,13 @@ struct AttnTcParams {
 template <int HD>
 struct AttnTcCfg {
   static constexpr int KB = HD / 64;                         // 64-element k-blocks of the head dimension
-  static constexpr int Q_BYTES = KB * kAtBQ * 128;           // [KB][128 rows][128 B]
+  static constexpr int Q_BYTES = KB * kAtBQ * 128;           // [KB][64 rows][128 B]
   static constexpr int K_BYTES = KB * kAtBKV * 128;
-  static constexpr int V_BYTES = KB * kAtBKV * 128;          // [KB (head-dim halves)][128 kv rows][128 B]
-  static constexpr int P_BYTES = 2 * kAtBQ * 128;            // [2 kv k-blocks][128 rows][128 B]
-  // TWO CTAs per SM overlap each other's phases (one CTA's softmax runs while the other's MMAs and TMA loads do): 1 K/V stage,
-  // 1 score buffer, 256 TMEM columns each.  (Measured under ncu: one CTA per SM with 2 stages / 2 score buffers left the tensor pipe
-  // 6-12 % active.)  hd 128: P (32 KB) is written over the K tile of the same iteration -- K is dead once S = Q K^T has completed
-  // (the softmax waits for exactly that), and the next K is loaded only after P V has completed (the commit that frees the stage) --
-  // which brings the CTA to 96 KB.  hd 64: K is only 16 KB, P keeps its own buffer (80 KB).
-  static constexpr int NSTAGE = 1;
-  static constexpr int NSBUF = 1;
-  static constexpr int CTAS_PER_SM = 2;
+  static constexpr int V_BYTES = KB * kAtBKV * 128;          // [KB (head-dim blocks)][64 kv rows][128 B]
   static constexpr int KV_OFF = Q_BYTES;
-  static constexpr bool P_ALIASES_K = (K_BYTES >= P_BYTES);
-  static constexpr int P_OFF = P_ALIASES_K ? KV_OFF : KV_OFF + NSTAGE * (K_BYTES + V_BYTES);
-  static constexpr int BAR_OFF = P_ALIASES_K ? KV_OFF + NSTAGE * (K_BYTES + V_BYTES) : P_OFF + P_BYTES;
+  static constexpr int BAR_OFF = KV_OFF + kAtStages * (K_BYTES + V_BYTES);
   static constexpr int SMEM_BYTES = BAR_OFF + 256 + 1024;
-  static constexpr int TMEM_COLS = 256;                      // S: 128 columns, then O: HD columns
-  static constexpr uint32_t O_COL = NSBUF * 128;
 };
-
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]),
-        "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // MN-major operand, 128 B swizzle: rows (the contraction index) of 128 B = 64 contiguous MN elements, 8-row atoms 1024 B apart
 // (stride byte offset), the next 64 MN elements `lbo_bytes` away (leading byte offset)
@@ -78,28 +51,27 @@ __device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint3
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-constexpr uint32_t kIdescBMajorMN = 1u << 16;
 
 template <int HD>
-__global__ void __launch_bounds__(kAtThreads, AttnTcCfg<HD>::CTAS_PER_SM)
+__device__ __forceinline__ void wgmma_pv(float (&o)[HD / 2], const uint32_t (&a)[4], uint64_t bdesc) {
+  if constexpr (HD == 64) wgmma_bf16_rs_tb_n64(o, a, bdesc, 1);
+  else wgmma_bf16_rs_tb_n128(o, a, bdesc, 1);
+}
+
+template <int HD>
+__global__ void __launch_bounds__(kAtThreads, 2)
 attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0, const __grid_constant__ CUtensorMap tmV0,
                        const __grid_constant__ CUtensorMap tmK1, const __grid_constant__ CUtensorMap tmV1, const AttnTcParams p) {
   using C = AttnTcCfg<HD>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
   const uint32_t bar0 = base + C::BAR_OFF;
   const uint32_t q_full = bar0;
   auto kv_full = [&](int s) { return bar0 + 8u * (1 + s); };
-  auto kv_empty = [&](int s) { return bar0 + 8u * (3 + s); };
-  auto s_full = [&](int b) { return bar0 + 8u * (5 + b); };
-  const uint32_t p_ready = bar0 + 8u * 7, o_done = bar0 + 8u * 8;
-  const uint32_t tmem_slot = bar0 + 8u * 9;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + C::BAR_OFF + 8 * 9);
+  auto kv_empty = [&](int s) { return bar0 + 8u * (1 + kAtStages + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * kAtBQ, h = blockIdx.y, b = blockIdx.z;
@@ -117,30 +89,23 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 1); mbar_init(s_full(s), 1); }
-    mbar_init(p_ready, 4);
-    mbar_init(o_done, 1);
+    for (int s = 0; s < kAtStages; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 1); }
     fence_barrier_init();
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
     if (p.n1 > 0) { tma_prefetch_desc(&tmK1); tma_prefetch_desc(&tmV1); }
   }
-  if (warp == 1) tmem_alloc(tmem_slot, C::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0 && n_tiles > 0) {
       // ===================== TMA producer =====================
       pdl_wait();                                             // q / k / v come from the previous kernel
-      trace.dep();
       mbar_arrive_expect_tx(q_full, C::Q_BYTES);
       for (int kb = 0; kb < C::KB; ++kb) tma_load_2d(base + kb * kAtBQ * 128, &tmQ, h * HD + kb * 64, b * p.Sq + q0, q_full, kEvictNormal);
       for (int i = 0; i < n_tiles; ++i) {
-        const int j = jt0 + i, stage = i % C::NSTAGE;
-        mbar_wait(kv_empty(stage), (((uint32_t)(i / C::NSTAGE)) & 1u) ^ 1u);
+        const int j = jt0 + i, stage = i % kAtStages;
+        mbar_wait_mma(kv_empty(stage), (((uint32_t)(i / kAtStages)) & 1u) ^ 1u);
         mbar_arrive_expect_tx(kv_full(stage), C::K_BYTES + C::V_BYTES);
         const uint32_t sk = base + C::KV_OFF + stage * (C::K_BYTES + C::V_BYTES), sv = sk + C::K_BYTES;
         const bool seg1 = j >= nt0;
@@ -154,161 +119,100 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0 && n_tiles > 0) {
-      // ===================== MMA issuer =====================
-      constexpr uint32_t idesc_s = make_idesc_bf16(kAtBQ, kAtBKV);
-      constexpr uint32_t idesc_o = make_idesc_bf16(kAtBQ, HD) | kIdescBMajorMN;
-      auto issue_s = [&](int i) {                              // S[i % NSBUF] = Q K_i^T
-        const int stage = i % C::NSTAGE, sbuf = i % C::NSBUF;
-        mbar_wait(kv_full(stage), ((uint32_t)(i / C::NSTAGE)) & 1u);
-        tc_fence_after();
-        const uint32_t sk = base + C::KV_OFF + stage * (C::K_BYTES + C::V_BYTES);
-        const uint32_t d_tmem = tmem_base + (uint32_t)(sbuf * kAtBKV);
-#pragma unroll
-        for (int kb = 0; kb < C::KB; ++kb) {
-          const uint64_t adesc = make_desc_sw128(base + kb * kAtBQ * 128), bdesc = make_desc_sw128(sk + kb * kAtBKV * 128);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16(d_tmem, adesc + 2u * k, bdesc + 2u * k, idesc_s, (kb > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(s_full(sbuf));
-      };
-      mbar_wait(q_full, 0);
-      issue_s(0);
-      for (int i = 0; i < n_tiles; ++i) {
-        if (C::NSBUF == 2 && i + 1 < n_tiles) issue_s(i + 1);  // two score buffers: overlaps the softmax of tile i
-        mbar_wait(p_ready, (uint32_t)i & 1u);
-        tc_fence_after();
-        const int stage = i % C::NSTAGE;
-        const uint32_t sv = base + C::KV_OFF + stage * (C::K_BYTES + C::V_BYTES) + C::K_BYTES;
-        const uint32_t sp = base + C::P_OFF;
-        const uint32_t o_tmem = tmem_base + C::O_COL;
-#pragma unroll
-        for (int ks = 0; ks < kAtBKV / 16; ++ks) {             // 16 kv rows per MMA: P k-block ks / 4 (+32 B per step), V rows +16 * 128 B
-          const uint64_t adesc = make_desc_sw128(sp + (ks >> 2) * kAtBQ * 128) + 2u * (ks & 3);
-          const uint64_t bdesc = make_desc_mn_sw128(sv + ks * 16 * 128, (uint32_t)(kAtBKV * 128));
-          umma_bf16(o_tmem, adesc, bdesc, idesc_o, (i > 0 || ks > 0) ? 1u : 0u);
-        }
-        umma_commit(kv_empty(stage));                          // K/V stage (and P) reusable
-        umma_commit(o_done);
-        // one score buffer / one K/V stage: the next tile's K arrives only after this commit frees the stage; the scores of
-        // tile i were consumed before p_ready(i).  (The other CTA on the SM keeps the tensor core busy meanwhile.)
-        if (C::NSBUF == 1 && i + 1 < n_tiles) issue_s(i + 1);
-      }
-    }
-    __syncwarp();
   } else {
-    // ===================== softmax / rescale / epilogue: thread = query row =====================
-    const int q = warp & 3;
-    const int r = q * 32 + lane;                               // row inside the tile = TMEM lane
-    const int qi = q0 + r;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    float m_run = -INFINITY, l_run = 0.f;
-    uint8_t* p_row = base_ptr + C::P_OFF + (size_t)r * 128;     // + kv k-block * 16 KB; 16 B chunk c sits at (c ^ (r & 7)) * 16
+    // ===================== wgmma warpgroup: S = Q K^T, online softmax, O += P V, epilogue =====================
+    // Thread (warp w, lane l) holds query rows 16 w + l / 4 (+ 8) and columns 8 j + 2 (l % 4) (+ 1) of S and O; the 4 lanes of a
+    // quad share a row.  l_run is this thread's partial row sum (alpha is uniform over the quad), reduced over the quad at the end.
+    const int fr = warp * 16 + (lane >> 2), fc = 2 * (lane & 3);
+    pdl_wait();
+    trace.dep();                                               // (the trace slot belongs to thread 0, a thread of this warpgroup)
+    float o[HD / 2];
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    if (n_tiles > 0) mbar_wait_mma(q_full, 0);
     for (int i = 0; i < n_tiles; ++i) {
-      const int j = jt0 + i, buf = i % C::NSBUF;
+      const int j = jt0 + i, stage = i % kAtStages;
       const bool seg1 = j >= nt0;
       const int kbase = seg1 ? p.n0 + (j - nt0) * kAtBKV : j * kAtBKV;       // global key index of the tile's first row
       const int kvalid = seg1 ? p.n1 - (j - nt0) * kAtBKV : p.n0 - j * kAtBKV; // keys of this tile that exist in the segment
-      int hi = min(kvalid, kAtBKV);
-      if (p.causal) hi = min(hi, qi + off - kbase + 1);
       const int lo = max(kv0 - kbase, 0);
-      mbar_wait(s_full(buf), ((uint32_t)(i / C::NSBUF)) & 1u);
-      tc_fence_after();
-      const uint32_t s_addr = lane_addr + (uint32_t)(buf * kAtBKV);
-      // pass 1: row maximum of the visible scores
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(s_addr + c * 32, v);
-        tmem_ld_wait();
+      const uint32_t sk = base + C::KV_OFF + stage * (C::K_BYTES + C::V_BYTES), sv = sk + C::K_BYTES;
+      mbar_wait_mma(kv_full(stage), ((uint32_t)(i / kAtStages)) & 1u);
+      float s[kAtBKV / 2];
+      wgmma_fence();
 #pragma unroll
-        for (int e = 0; e < 32; ++e) { const int jj = c * 32 + e; if (jj >= lo && jj < hi) mx = fmaxf(mx, __uint_as_float(v[e]) * p.sl2); }
+      for (int kb = 0; kb < C::KB; ++kb) {
+        const uint64_t adesc = make_desc_sw128(base + kb * kAtBQ * 128), bdesc = make_desc_sw128(sk + kb * kAtBKV * 128);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_bf16<kAtBKV>(s, adesc + 2u * k, bdesc + 2u * k, (kb > 0 || k > 0) ? 1 : 0);
       }
-      const float m_new = fmaxf(m_run, mx);
-      const float m_safe = (m_new == -INFINITY) ? 0.f : m_new;
-      const float alpha = exp2f(m_run - m_safe);               // 0 when nothing was visible before
-      m_run = m_new;
-      // the previous tile's P V must have completed: O is rescaled in TMEM and the P buffer is rewritten
-      if (i > 0) {
-        mbar_wait(o_done, (uint32_t)(i - 1) & 1u);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < HD / 32; ++c) {
-          uint32_t v[32];
-          tmem_ld_32x32(lane_addr + C::O_COL + c * 32, v);
-          tmem_ld_wait();
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+      uint32_t pa[kAtBKV / 16][4];                             // P as the A fragments of the 4 k-steps of P V
 #pragma unroll
-          for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * alpha);
-          tmem_st_32x32(lane_addr + C::O_COL + c * 32, v);
-        }
-        tmem_st_wait();
-      }
-      // pass 2: probabilities -> bf16 -> shared memory (K-major, 128 B swizzle: what the PV MMA reads as its A operand)
-      float ls = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(s_addr + c * 32, v);
-        tmem_ld_wait();
-        uint32_t pk[16];
+      for (int h2 = 0; h2 < 2; ++h2) {
+        const int qi = q0 + fr + 8 * h2;
+        int hi = min(kvalid, kAtBKV);
+        if (p.causal) hi = min(hi, qi + off - kbase + 1);
+        float mx = -INFINITY;
 #pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int j0 = c * 32 + 2 * e;
-          float p0 = (j0 >= lo && j0 < hi) ? exp2f(__uint_as_float(v[2 * e]) * p.sl2 - m_safe) : 0.f;
-          float p1 = (j0 + 1 >= lo && j0 + 1 < hi) ? exp2f(__uint_as_float(v[2 * e + 1]) * p.sl2 - m_safe) : 0.f;
+        for (int jj = 0; jj < kAtBKV / 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * jj + fc + e;
+            if (col >= lo && col < hi) mx = fmaxf(mx, s[4 * jj + 2 * h2 + e] * p.sl2);
+          }
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float m_new = fmaxf(m_run[h2], mx);
+        const float m_safe = (m_new == -INFINITY) ? 0.f : m_new;
+        const float alpha = exp2f(m_run[h2] - m_safe);         // 0 when nothing was visible before
+        m_run[h2] = m_new;
+        float ls = 0.f;
+#pragma unroll
+        for (int jj = 0; jj < kAtBKV / 8; ++jj) {
+          const int col = 8 * jj + fc;
+          const float p0 = (col >= lo && col < hi) ? exp2f(s[4 * jj + 2 * h2] * p.sl2 - m_safe) : 0.f;
+          const float p1 = (col + 1 >= lo && col + 1 < hi) ? exp2f(s[4 * jj + 2 * h2 + 1] * p.sl2 - m_safe) : 0.f;
           const __nv_bfloat162 pb = __floats2bfloat162_rn(p0, p1);
-          ls += __bfloat162float(pb.x) + __bfloat162float(pb.y);       // the sum of what the tensor core will actually multiply
-          pk[e] = *reinterpret_cast<const uint32_t*>(&pb);
+          ls += __bfloat162float(pb.x) + __bfloat162float(pb.y);   // the sum of what the tensor core will actually multiply
+          // k-step jj / 2: registers {row, cols 0-7 | row + 8, cols 0-7 | row, cols 8-15 | row + 8, cols 8-15}
+          pa[jj >> 1][(jj & 1) * 2 + h2] = *reinterpret_cast<const uint32_t*>(&pb);
         }
-        // 32 values = 64 B = 16 B chunks (c & 1) * 4 .. + 3 of kv k-block c >> 1
-        uint8_t* dst = p_row + (size_t)(c >> 1) * (kAtBQ * 128);
+        l_run[h2] = l_run[h2] * alpha + ls;
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int chunk = (c & 1) * 4 + g;
-          *reinterpret_cast<uint4*>(dst + ((chunk ^ (r & 7)) << 4)) = make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-        }
+        for (int jj = 0; jj < HD / 8; ++jj) { o[4 * jj + 2 * h2] *= alpha; o[4 * jj + 2 * h2 + 1] *= alpha; }
       }
-      l_run = l_run * alpha + ls;
-      fence_proxy_async();                                     // generic-proxy writes of P -> visible to the tensor core (async proxy)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < kAtBKV / 16; ++ks)                 // 16 kv rows per MMA: V rows +16 * 128 B
+        wgmma_pv<HD>(o, pa[ks], make_desc_mn_sw128(sv + ks * 16 * 128, (uint32_t)(kAtBKV * 128)));
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(o);
+      if (threadIdx.x == 0) mbar_arrive(kv_empty(stage));     // K/V stage reusable
     }
     // ---- epilogue: O / l -> bf16
-    if (n_tiles > 0) {
-      mbar_wait(o_done, (uint32_t)(n_tiles - 1) & 1u);
-      tc_fence_after();
-    } else {
-      pdl_wait();
-    }
-    const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
-    bf16* orow = p.out + (size_t)(b * p.Sq + (qi < p.Sq ? qi : 0)) * p.o_stride + h * HD;
-#pragma unroll 1
-    for (int c = 0; c < HD / 32; ++c) {
-      uint32_t v[32];
-      if (n_tiles > 0) { tmem_ld_32x32(lane_addr + C::O_COL + c * 32, v); tmem_ld_wait(); }
-      else {
 #pragma unroll
-        for (int e = 0; e < 32; ++e) v[e] = 0u;
-      }
+    for (int h2 = 0; h2 < 2; ++h2) {
+      float l = l_run[h2];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      const float inv = l > 0.f ? 1.f / l : 0.f;
+      const int qi = q0 + fr + 8 * h2;
       if (qi < p.Sq) {
-        uint4* dst = reinterpret_cast<uint4*>(orow + c * 32);
+        bf16* orow = p.out + (size_t)(b * p.Sq + qi) * p.o_stride + h * HD;
 #pragma unroll
-        for (int g = 0; g < 4; ++g)
-          dst[g] = make_uint4(pack_bf16x2(__uint_as_float(v[8 * g]) * inv, __uint_as_float(v[8 * g + 1]) * inv),
-                              pack_bf16x2(__uint_as_float(v[8 * g + 2]) * inv, __uint_as_float(v[8 * g + 3]) * inv),
-                              pack_bf16x2(__uint_as_float(v[8 * g + 4]) * inv, __uint_as_float(v[8 * g + 5]) * inv),
-                              pack_bf16x2(__uint_as_float(v[8 * g + 6]) * inv, __uint_as_float(v[8 * g + 7]) * inv));
+        for (int jj = 0; jj < HD / 8; ++jj)
+          *reinterpret_cast<uint32_t*>(orow + 8 * jj + fc) = pack_bf16x2(o[4 * jj + 2 * h2] * inv, o[4 * jj + 2 * h2 + 1] * inv);
       }
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   trace.done();
-  if (warp == 1) tmem_dealloc(tmem_base, C::TMEM_COLS);
 }
 
 VCLA_DEFINE_TRACE_SETTER(trace_set_attention_tc)
@@ -338,12 +242,12 @@ static int attn_tc_init() {
   return g_at_rc;
 }
 
-// rows x cols bf16 view with a row pitch of `ld` elements; boxes of 128 rows x 64 columns (128 B), 128 B swizzle
+// rows x cols bf16 view with a row pitch of `ld` elements; boxes of 64 rows x 64 columns (128 B), 128 B swizzle
 static int attn_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld) {
   if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ld * 2) % 16 != 0) { set_error("attention_tc: operands must be 16 B aligned with a 16 B-multiple pitch"); return -1; }
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {ld * 2};
-  cuuint32_t box[2] = {64, 128};
+  cuuint32_t box[2] = {64, (cuuint32_t)kAtBQ};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = g_at_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

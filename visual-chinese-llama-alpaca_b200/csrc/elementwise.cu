@@ -677,7 +677,7 @@ __global__ void fill_hash_normal_kernel(bf16* dst_bf16, float* dst_f32, int64_t 
 }
 int fill_hash_normal(bf16* dst_bf16, float* dst_f32, int64_t n, uint32_t seed, float mul, float offset, cudaStream_t st) {
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
   fill_hash_normal_kernel<<<(int)blocks, 256, 0, st>>>(dst_bf16, dst_f32, n, seed, mul, offset);
   VCLA_CUDA_OK(cudaGetLastError());
   return 0;
@@ -694,7 +694,7 @@ __global__ void convert_kernel(const T* src, int64_t n, O* dst) {
 template <typename O>
 static int convert_any(const void* src, int dtype, int64_t n, O* dst, cudaStream_t st) {
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
   if (blocks == 0) return 0;
   if (dtype == 0) convert_kernel<float, O><<<(int)blocks, 256, 0, st>>>((const float*)src, n, dst);
   else if (dtype == 1) convert_kernel<__half, O><<<(int)blocks, 256, 0, st>>>((const __half*)src, n, dst);

@@ -132,12 +132,11 @@ struct vcla_ctx {
   int decode_schedule = 2;
   int csk_qkv = 0, csk_o = 0, csk_gu = 0, csk_d = 0, csk_lm = 0;   // CTAs per cluster (= K splits), chosen per batch on first use
   int csk_batch = 0;
-  int fused_decode = 0;   // VCLA_FUSED_DECODE=1: 5-kernel/layer schedule with in-GEMM split-K fixup. Correct (parity-tested) but measured slower
-                          // on B200 (3.96 vs 3.32 ms/token at B=8): the fence->atomic->reload chain per tile outlasts a kernel boundary.   // tokens of every step since the last prefill, appended by the argmax kernel
+  int fused_decode = 0;   // VCLA_FUSED_DECODE=1: 5-kernel/layer schedule with in-GEMM split-K fixup (parity-tested; the fence->atomic->reload
+                          // chain per tile is serial latency, so the cluster split-K schedule is the default)
   int sp_qkv = 1, sp_o = 1, sp_gu = 1, sp_d = 1, sp_lm = 1, kv_splits = 1;
   int l2_prefetch_kb = 0;    // decode GEMMs: weight k-blocks per CTA prefetched into L2 during the dependency wait (VCLA_L2_PREFETCH_KB).
-                             // Measured harmful on B200 (0/8/16/24/48 -> 3142/3226/3349/3390/3437 us per step: the prefetch traffic delays
-                             // the latency-critical consumer kernel in front of the GEMM), so it is off by default.
+                             // Off by default: the prefetch traffic can delay the latency-critical consumer kernel in front of the GEMM.
   // graphs
   std::map<GraphKey, cudaGraphExec_t> graphs;
   std::map<GraphKey, int64_t> graph_launches;
@@ -341,9 +340,9 @@ void layout_activations(vcla_ctx* c) {
   c->finished = a_alloc<int32_t>(c, Bp);
 }
 
-// Split-K factor of a decode GEMM (row tiles of 128 x `splits` work units on 2 persistent CTAs per SM).  Measured on B200
-// (profiles/r1_decode_step_trace_*.json): a thin last wave is latency-bound (one lone CTA streams ~80 GB/s), and a single
-// wave of one-tile CTAs loses the epilogue/load overlap -> prefer >= ~2 waves with a last wave that is >= 60 % full.
+// Split-K factor of a decode GEMM (row tiles of 128 x `splits` work units on 2 persistent CTAs per SM).  A thin last wave is
+// latency-bound (one lone CTA streams a small fraction of HBM bandwidth), and a single wave of one-tile CTAs loses the
+// epilogue/load overlap -> prefer >= ~2 waves with a last wave that is >= 60 % full.
 int pick_splits(int n_out, int K) {
   const int tiles = (n_out + 127) / 128;
   const int kb = (K + 63) / 64;
@@ -413,7 +412,7 @@ static int nccl_api() {
 extern "C" {
 
 const char* vcla_last_error(void) { return get_error(); }
-const char* vcla_version(void) { return "vcla-b200 0.1 (sm_100a, tcgen05/TMA)"; }
+const char* vcla_version(void) { return "vcla-h100 0.1 (sm_90a, wgmma/TMA)"; }
 void vcla_set_pdl(int on) { set_pdl(on != 0); }
 
 int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
@@ -1372,7 +1371,6 @@ int vcla_debug_get_csk_splits(vcla_ctx* c, int B, int* out5) {
   return 0;
 }
 int vcla_op_gemm_csk_clusters(int B, int splits) { return gemm_csk_clusters(B, splits); }
-void vcla_set_gemm_two_cta(int on) { gemm_set_two_cta(on); }
 void vcla_set_attention_tc(int on) { attention_set_tc(on); }
 int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v0, int kv0_stride, int n0, const void* k1, const void* v1,
                       int kv1_stride, int n1, void* out, int o_stride, int B, int H, int Sq, int HD, float scale, int causal, vcla_stream stream) {

@@ -1,18 +1,18 @@
-// tcgen05 GEMM for sm_100a:  D[M,N] = A[M,K] * B[N,K]^T, bf16 operands, fp32 accumulation in TMEM.
+// wgmma GEMM for sm_90a:  D[M,N] = A[M,K] * B[N,K]^T, bf16 operands, fp32 accumulation in registers.
 //
 // One kernel template serves the whole path:
-//   * prefill / ViT / Resampler / projector: A = activations (tokens are the 128-row UMMA M dimension),
+//   * prefill / ViT / Resampler / projector: A = activations (tokens are the wgmma M dimension),
 //     B = nn.Linear weight [N_out, K]; fused epilogues: bias, quick_gelu / erf-gelu, fp32 residual add
-//     with output-row remap (+ position-embedding table), SwiGLU.
+//     with output-row remap (+ position-embedding table), SwiGLU, deferred RMSNorm, RoPE + KV-cache append.
 //   * decode ("swap-AB"): A = weight [N_out, K] (streamed once from HBM through TMA), B = the few
 //     activation rows [batch_pad, K]; split-K partials are written to an fp32 workspace that the
 //     next (fused consumer) kernel reduces in a fixed order, so results are deterministic.
 //
-// Structure (per CTA, 192 threads): warp 0 lane 0 = TMA producer, warp 1 lane 0 = MMA issuer (+ TMEM
-// alloc/dealloc by the whole warp), warps 2..5 = epilogue (TMEM lane quadrant = warp_idx % 4).
-// smem ring of STAGES x {A 128x64, B BNx64} tiles in the 128B-swizzled K-major layout that both TMA
-// and the UMMA shared-memory descriptors understand; two TMEM accumulator stages so the epilogue of
-// tile i overlaps the MMAs of tile i+1.  Persistent: each CTA walks tiles blockIdx.x, +gridDim.x, ...
+// Structure (per CTA, 160 threads): warp 4 lane 0 = TMA producer, warps 0..3 = one wgmma warpgroup that issues the
+// MMAs (BM / 64 blocks of m64nBNk16 per 16-wide k step) and then runs the epilogue straight from its accumulator registers.
+// smem ring of STAGES x {A BMx64, B BNx64} tiles in the 128B-swizzled K-major layout that both TMA and the wgmma
+// shared-memory descriptors understand; the producer keeps filling the ring for the next tile while the epilogue runs.
+// Persistent: each CTA walks tiles blockIdx.x, +gridDim.x, ...
 #include "common.cuh"
 #include "kernels.h"
 
@@ -41,7 +41,7 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -71,22 +71,23 @@ struct GemmParams {
   GemmRope rope;
 };
 
-constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
-constexpr int kGemmThreads = 192;
+constexpr int kGemmThreads = 160;   // warps 0..3 = the wgmma warpgroup (MMA + epilogue), warp 4 = TMA producer
+constexpr int kSwapBlockM = 128;    // swap-AB tiles: 128 weight rows (the split-K fixup's tile counters count these)
 
-template <int BN, int STAGES, int CTAS = 1>
+// BM x BN tile, BM / 64 wgmma row blocks; the accumulators take BM * BN / 128 fp32 registers per thread (<= 128)
+template <int BM, int BN, int STAGES>
 struct GemmCfg {
-  static constexpr int A_BYTES = kBlockM * kBlockK * 2;
-  static constexpr int B_BYTES = (BN / CTAS) * kBlockK * 2;            // a CTA pair splits the B tile's N rows
+  static constexpr int MH = BM / 64;
+  static constexpr int A_BYTES = BM * kBlockK * 2;
+  static constexpr int B_BYTES = BN * kBlockK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
   static constexpr int FIX_OFF = BAR_OFF + 256;             // [4 warps][64] fp32 cross-warp scratch + 1 flag of the split-K fixup
-  static constexpr int SMEM_BYTES = FIX_OFF + 1088 + 1024;  // barriers + tmem slot + fixup scratch, + slack for 1024 B alignment
-  static constexpr int TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  static constexpr int CH = BN < 32 ? BN : 32;  // epilogue column chunk
+  static constexpr int SMEM_BYTES = FIX_OFF + 1088 + 1024;  // barriers + fixup scratch, + slack for 1024 B alignment
   static_assert(STAGE_BYTES % 1024 == 0, "stage must keep 1024 B alignment for SWIZZLE_128B");
-  static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "UMMA N constraint for M=128");
+  static_assert(BM == 64 || BM == 128, "tile rows");
+  static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256 && BM * BN <= 64 * 256, "wgmma N constraint / accumulator registers");
 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {
@@ -95,28 +96,18 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   return x;
 }
 
-// CTAS = 2: a CTA PAIR (cluster (2,1,1), two SMs of one TPC) computes a 256 x BN tile with tcgen05.mma.cta_group::2: each CTA stages
-// its own 128 A rows and HALF of the B tile, the leader (cluster rank 0) issues the MMAs for both, each CTA's TMEM receives its 128
-// rows.  Per SM and k-block this halves the B bytes written to and read from shared memory, which is what bounds the 128 x 256
-// single-CTA tile (A 4 KB + B 8 KB per 128-cycle MMA against a 128 B/cycle crossbar that also takes the TMA writes).
-template <int BN, int STAGES, bool SWAP, int CTAS = 1>
+template <int BM, int BN, int STAGES, bool SWAP>
 __global__ void __launch_bounds__(kGemmThreads, SWAP ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  using C = GemmCfg<BN, STAGES, CTAS>;
-  static_assert(CTAS == 1 || (!SWAP && BN == 256), "the CTA-pair variant is the 256 x 256 prefill tile");
-  constexpr bool TWO = CTAS == 2;
-  const int crank = TWO ? (int)cluster_rank() : 0;
-  const bool leader = crank == 0;
+  using C = GemmCfg<BM, BN, STAGES>;
+  constexpr int MH = C::MH;
+  static_assert(!SWAP || BM == kSwapBlockM, "swap-AB tiles are 128 weight rows");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
   const uint32_t bar0 = base + C::BAR_OFF;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar0 + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar0 + 8u * (2 * STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar0 + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + C::BAR_OFF + 8 * (2 * STAGES + 4));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -127,35 +118,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 1);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 4 * CTAS);      // the leader's MMA warp waits for the epilogue warps of BOTH CTAs
-    }
     fence_barrier_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 1) { if constexpr (TWO) tmem_alloc_2cta(tmem_slot, C::TMEM_COLS); else tmem_alloc(tmem_slot, C::TMEM_COLS); }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (TWO) cluster_barrier();        // the peer's barriers exist before TMA / commits / arrives target them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   // PDL: let the next kernel's CTAs become resident as soon as ours are (they only prefetch read-only weights and
   // then block in griddepcontrol.wait until this grid has completed), see the producer below.
   pdl_launch_dependents();
-  const int tile0 = TWO ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;          // a pair walks the pair-tiles together
-  const int tile_step = TWO ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
   auto tile_coords = [&](int t, int& m_blk, int& n_blk, int& kb0, int& kb1, int& ks) {
-    if constexpr (TWO) {
-      const int m_pairs = (p.m_tiles + 1) >> 1;
-      m_blk = (t % m_pairs) * 2 + crank;       // this CTA's 128 rows of the pair's 256
-      n_blk = t / m_pairs;
-      ks = 0; kb0 = 0; kb1 = p.kb_total;
-      return;
-    }
     m_blk = t % p.m_tiles;
     int r = t / p.m_tiles;
     n_blk = r % p.n_tiles;
@@ -164,7 +137,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     kb1 = min(p.kb_total, kb0 + p.kb_per_split);
   };
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       // ===================== TMA producer =====================
       // The weight operand (A when swap-AB, else B) never depends on the previous kernel, so its tiles for the first
@@ -180,36 +153,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const uint64_t act_policy = SWAP ? p.policy_b : p.policy_a;
       auto flush_pending = [&]() {
         pdl_wait();
-        trace.dep();
-        for (int i = 0; i < npend; ++i) {
-          if constexpr (TWO) tma_load_2d_2cta(pend_dst[i], act_map, pend_c0[i], pend_c1[i], pend_bar[i], act_policy);
-          else tma_load_2d(pend_dst[i], act_map, pend_c0[i], pend_c1[i], pend_bar[i], act_policy);
-        }
+        for (int i = 0; i < npend; ++i) tma_load_2d(pend_dst[i], act_map, pend_c0[i], pend_c1[i], pend_bar[i], act_policy);
         npend = 0;
         dep_ready = true;
       };
-      for (int t = tile0; t < p.total_tiles; t += tile_step) {
+      for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
         int m_blk, n_blk, kb0, kb1, ks;
         tile_coords(t, m_blk, n_blk, kb0, kb1, ks);
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
+          mbar_wait_mma(empty_bar(stage), phase ^ 1u);
           const uint32_t sa = base + stage * C::STAGE_BYTES;
-          if constexpr (TWO) {
-            // both CTAs' bytes are counted on the LEADER's full barrier (the only one the MMA thread waits on)
-            if (leader) mbar_arrive_expect_tx(full_bar(stage), 2 * C::STAGE_BYTES);
-            tma_load_2d_2cta(sa + C::A_BYTES, &tmB, kb * kBlockK, n_blk * BN + crank * (BN / 2), full_bar(stage), p.policy_b);   // weights (half)
-            if (dep_ready) {
-              tma_load_2d_2cta(sa, &tmA, kb * kBlockK, m_blk * kBlockM, full_bar(stage), p.policy_a);
-            } else {
-              pend_dst[npend] = sa; pend_bar[npend] = full_bar(stage); pend_c0[npend] = kb * kBlockK; pend_c1[npend] = m_blk * kBlockM; ++npend;
-            }
-            if (!dep_ready && npend == STAGES) flush_pending();
-            if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-            continue;
-          }
           mbar_arrive_expect_tx(full_bar(stage), C::STAGE_BYTES);
           if constexpr (SWAP) {
-            tma_load_2d(sa, &tmA, kb * kBlockK, m_blk * kBlockM, full_bar(stage), p.policy_a);           // weights
+            tma_load_2d(sa, &tmA, kb * kBlockK, m_blk * BM, full_bar(stage), p.policy_a);           // weights
             if (dep_ready) {
               tma_load_2d(sa + C::A_BYTES, &tmB, kb * kBlockK, n_blk * BN, full_bar(stage), p.policy_b);
             } else {
@@ -218,14 +174,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           } else {
             tma_load_2d(sa + C::A_BYTES, &tmB, kb * kBlockK, n_blk * BN, full_bar(stage), p.policy_b);   // weights
             if (dep_ready) {
-              tma_load_2d(sa, &tmA, kb * kBlockK, m_blk * kBlockM, full_bar(stage), p.policy_a);
+              tma_load_2d(sa, &tmA, kb * kBlockK, m_blk * BM, full_bar(stage), p.policy_a);
             } else {
-              pend_dst[npend] = sa; pend_bar[npend] = full_bar(stage); pend_c0[npend] = kb * kBlockK; pend_c1[npend] = m_blk * kBlockM; ++npend;
+              pend_dst[npend] = sa; pend_bar[npend] = full_bar(stage); pend_c0[npend] = kb * kBlockK; pend_c1[npend] = m_blk * BM; ++npend;
             }
           }
           if (!dep_ready && npend == STAGES) {
             // The smem ring is full and the dependency is (probably) still unresolved: HBM would idle while the small
-            // consumer kernel in front of us runs.  Pull this CTA's NEXT weight tiles into the 126 MB L2 so the main loop
+            // consumer kernel in front of us runs.  Pull this CTA's NEXT weight tiles into L2 so the main loop
             // streams them from L2 afterwards.
             if (p.l2_prefetch_kb > 0) {
               int budget = p.l2_prefetch_kb;
@@ -234,7 +190,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 int m2, n2, k0, k1, s2;
                 tile_coords(t2, m2, n2, k0, k1, s2);
                 for (int kk = (t2 == t ? kbn : k0); kk < k1 && budget > 0; ++kk, --budget) {
-                  if constexpr (SWAP) tma_prefetch_l2_2d(&tmA, kk * kBlockK, m2 * kBlockM);
+                  if constexpr (SWAP) tma_prefetch_l2_2d(&tmA, kk * kBlockK, m2 * BM);
                   else tma_prefetch_l2_2d(&tmB, kk * kBlockK, n2 * BN);
                 }
               }
@@ -247,88 +203,74 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if (!dep_ready) flush_pending();
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0 && leader) {
-      // ===================== MMA issuer (CTA pair: the leader only) =====================
-      constexpr uint32_t idesc = make_idesc_bf16(kBlockM * CTAS, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t accphase = 0;
-      for (int t = tile0; t < p.total_tiles; t += tile_step) {
-        int m_blk, n_blk, kb0, kb1, ks;
-        tile_coords(t, m_blk, n_blk, kb0, kb1, ks);
-        mbar_wait(tempty_bar(acc), accphase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sa = base + stage * C::STAGE_BYTES;
-          const uint64_t adesc = make_desc_sw128(sa);
-          const uint64_t bdesc = make_desc_sw128(sa + C::A_BYTES);
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) {
-            // advance 16 elements (32 B) along K inside the 128 B swizzle atom: +2 in the 16 B-unit address field
-            if constexpr (TWO) umma_bf16_2cta(d_tmem, adesc + 2u * k, bdesc + 2u * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            else umma_bf16(d_tmem, adesc + 2u * k, bdesc + 2u * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          // smem slot reusable once these MMAs have read it (pair: the slot of BOTH CTAs)
-          if constexpr (TWO) umma_commit_2cta(empty_bar(stage), 3); else umma_commit(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        // accumulator complete -> epilogue (pair: each CTA's epilogue reads its own TMEM)
-        if constexpr (TWO) umma_commit_2cta(tfull_bar(acc), 3); else umma_commit(tfull_bar(acc));
-        acc ^= 1;
-        if (acc == 0) accphase ^= 1u;
-      }
-    }
-    __syncwarp();
   } else {
-    // ===================== epilogue warps =====================
-    const int q = warp & 3;                // TMEM lane quadrant this warp may access
-    const int row_in_tile = q * 32 + lane;
+    // ===================== wgmma warpgroup: MMAs, then the epilogue from the register accumulators =====================
+    // Thread (warp w, lane l) holds rows 16 w + l / 4 (+ 8) of every 64-row block and columns 8 j + 2 (l % 4) (+ 1).
+    const int fr = warp * 16 + (lane >> 2);
+    const int fc = 2 * (lane & 3);
     pdl_wait();                            // outputs / residual reads are ordered after the previous grid
-    int acc = 0;
-    uint32_t accphase = 0;
-    for (int t = tile0; t < p.total_tiles; t += tile_step) {
+    trace.dep();                           // (the trace slot belongs to thread 0, a thread of this warpgroup)
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[MH][BN / 2];
+    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
       int m_blk, n_blk, kb0, kb1, ks;
       tile_coords(t, m_blk, n_blk, kb0, kb1, ks);
-      mbar_wait(tfull_bar(acc), accphase);
-      tc_fence_after();
-      const int row = m_blk * kBlockM + row_in_tile;
-      const bool row_ok = row < p.M;
-      const uint32_t taddr0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN);
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait_mma(full_bar(stage), phase);
+        const uint32_t sa = base + stage * C::STAGE_BYTES;
+        const uint64_t bdesc = make_desc_sw128(sa + C::A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {
+#pragma unroll
+          for (int h = 0; h < MH; ++h)
+            wgmma_bf16<BN>(acc[h], make_desc_sw128(sa + h * 64 * 128) + 2u * k, bdesc + 2u * k, (kb > kb0 || k > 0) ? 1 : 0);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                   // the previous k-block's MMAs are done reading their stage
+        if (prev >= 0 && threadIdx.x == 0) mbar_arrive(empty_bar(prev));
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
+      if (prev >= 0 && threadIdx.x == 0) mbar_arrive(empty_bar(prev));
 
       if constexpr (SWAP) {
-        // rows = weight rows (output features), columns = batch.  Coalesced across lanes.
+        // rows = weight rows (output features), columns = batch
         float* ws = reinterpret_cast<float*>(p.out);
 #pragma unroll
-        for (int c = 0; c < BN / C::CH; ++c) {
-          uint32_t v[C::CH];
-          if constexpr (C::CH == 32) tmem_ld_32x32(taddr0 + c * C::CH, v);
-          else tmem_ld_32x16(taddr0 + c * C::CH, reinterpret_cast<uint32_t(&)[16]>(v));
-          tmem_ld_wait();
-          if (row_ok) {
+        for (int h = 0; h < MH; ++h) {
 #pragma unroll
-            for (int i = 0; i < C::CH; ++i) {
-              const int b = c * C::CH + i;
-              if (b < p.ws_rows) ws[((size_t)ks * p.ws_rows + b) * (size_t)p.ldo + row] = __uint_as_float(v[i]);
+          for (int h2 = 0; h2 < 2; ++h2) {
+            const int row = m_blk * BM + h * 64 + fr + 8 * h2;
+            if (row < p.M) {
+#pragma unroll
+              for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int b = 8 * j + fc + e;
+                  if (b < p.ws_rows) ws[((size_t)ks * p.ws_rows + b) * (size_t)p.ldo + row] = acc[h][4 * j + 2 * h2 + e];
+                }
+              }
             }
           }
         }
         if (p.fix.mode != FIX_NONE) {
-          // hand the accumulator stage back first: the MMA warp runs ahead on the next tile while we fix this one up
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(acc));
           // ---- split-K fixup: the CTA whose partial completes the tile reduces all partials (fixed order) and applies
-          //      the fused consumer.  Classic last-block pattern: fence, count, fence.
+          //      the fused consumer.  Classic last-block pattern: fence, count, fence.  Thread t owns tile row t here.
+          const int q = warp;
+          const int row_in_tile = q * 32 + lane;
+          const int row = m_blk * BM + row_in_tile;
+          const bool row_ok = row < p.M;
           volatile int* s_flag = reinterpret_cast<volatile int*>(base_ptr + C::FIX_OFF + 1024);
           float* s_red = reinterpret_cast<float*>(base_ptr + C::FIX_OFF);          // [4][64]
           __threadfence();
           asm volatile("bar.sync 1, 128;" ::: "memory");
-          if (warp == 2 && lane == 0) {
+          if (warp == 0 && lane == 0) {
             const int old = atomicAdd(p.fix.tile_counters + m_blk, 1);
             *s_flag = (old == p.splits - 1) ? 1 : 0;
           }
@@ -373,12 +315,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
               }
               asm volatile("bar.sync 1, 128;" ::: "memory");
-              const int t = (warp - 2) * 32 + lane;     // 0..127
+              const int t = row_in_tile;                // 0..127
               if (t < nb) p.fix.ssq[(size_t)t * p.m_tiles + m_blk] = s_red[t] + s_red[64 + t] + s_red[128 + t] + s_red[192 + t];
               // second level: the CTA that finishes the last tile turns the per-tile sums into the per-row scale
               __threadfence();
               asm volatile("bar.sync 1, 128;" ::: "memory");
-              if (warp == 2 && lane == 0) {
+              if (warp == 0 && lane == 0) {
                 const int old = atomicAdd(p.fix.tile_counters + p.m_tiles, 1);
                 *s_flag = (old == p.m_tiles - 1) ? 2 : 1;
               }
@@ -396,12 +338,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                   }
                   p.fix.rstd_out[t] = rsqrtf(ss * p.fix.inv_dim + p.fix.eps);
                 }
-                if (warp == 2 && lane == 0) p.fix.tile_counters[p.m_tiles] = 0;
+                if (warp == 0 && lane == 0) p.fix.tile_counters[p.m_tiles] = 0;
               }
             } else {  // FIX_SWIGLU: tile rows = [32 gate | 32 up | 32 gate | 32 up]
               const int blk = row_in_tile >> 6, within = row_in_tile & 63;
               const int gi = within & 31;                       // pair index inside the 64-row block
-              const int grow = m_blk * kBlockM + blk * 64 + gi; // gate row ; up row = grow + 32
+              const int grow = m_blk * BM + blk * 64 + gi;      // gate row ; up row = grow + 32
               const int jout = m_blk * 64 + blk * 32 + gi;      // output feature
               const bool pair_ok = (grow + 32) < p.M;
               const int half = (nb + 1) >> 1;
@@ -431,229 +373,158 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               }
             }
             __syncwarp();
-            if (warp == 2 && lane == 0) p.fix.tile_counters[m_blk] = 0;   // ready for the next launch / graph replay
+            if (warp == 0 && lane == 0) p.fix.tile_counters[m_blk] = 0;   // ready for the next launch / graph replay
           }
-          acc ^= 1;
-          if (acc == 0) accphase ^= 1u;
-          continue;
         }
+        continue;
       } else {
-        int orow = row;
-        if (p.rows_per_group > 0) orow = (row / p.rows_per_group) * p.group_stride + (row % p.rows_per_group) + p.row_offset;
         const int col_tile = n_blk * BN;
-        // deferred RMSNorm: the operand rows were not normalised; their scale commutes with the GEMM and lands here
-        float rs = 1.f;
-        if (p.rowscale.ssq != nullptr && row_ok) {
-          const float* sp = p.rowscale.ssq + (size_t)row * p.rowscale.slots;
-          float ss = 0.f;
-          for (int i = 0; i < p.rowscale.slots; ++i) ss += __ldg(sp + i);       // fixed order: deterministic
-          rs = rsqrtf(ss * p.rowscale.inv_dim + p.rowscale.eps);
-        }
-        if (p.rope.cos != nullptr) {
-          // ---- fused QKV epilogue: RoPE on q / k heads, store q|k|v rows, append k / v to the paged cache (BN = 256 = 2 heads)
-          if constexpr (BN == 256) {
-            const GemmRope& R = p.rope;
-            const int bq = row_ok ? row / R.S : 0, sq = row_ok ? row % R.S : 0;
-            const int pad = (R.left_pad != nullptr && row_ok) ? __ldg(R.left_pad + bq) : 0;
-            const int cpos = sq - pad;                               // index inside the (compact) KV cache
-            const bool cached = row_ok && cpos >= 0;                 // padding rows are neither rotated nor cached
-            const int pos = R.pos_from_mask ? (cpos > 0 ? cpos : 0) : sq;
-            int page = 0, slot = 0;
-            if (cached) { page = __ldg(R.page_table + (size_t)bq * R.pages_per_seq + cpos / R.page_tokens); slot = cpos % R.page_tokens; }
-            const float* ct = R.cos + (size_t)pos * 64;
-            const float* stb = R.sin + (size_t)pos * 64;
-            bf16* orow_ptr = reinterpret_cast<bf16*>(p.out) + (size_t)orow * p.ldo;
-#pragma unroll 1
-            for (int hh = 0; hh < 2; ++hh) {
-              const int hcol = col_tile + hh * 128;                  // first column of this head inside [q | k | v]
-              if (hcol >= p.N) break;
-              const int region = hcol / R.T, head = (hcol % R.T) / 128;
-#pragma unroll 1
-              for (int half = 0; half < 2; ++half) {                 // dims [32 half, 32 half + 32) pair with [64 + 32 half, ...)
-                uint32_t lo[32], hi[32];
-                tmem_ld_32x32(taddr0 + hh * 128 + half * 32, lo);
-                tmem_ld_32x32(taddr0 + hh * 128 + 64 + half * 32, hi);
-                tmem_ld_wait();
-                if (!row_ok) continue;
-                uint32_t plo[16], phi[16];
-                if (region < 2 && cached) {
 #pragma unroll
-                  for (int i = 0; i < 8; ++i) {
-                    const float4 c4 = __ldg(reinterpret_cast<const float4*>(ct + half * 32) + i);
-                    const float4 s4 = __ldg(reinterpret_cast<const float4*>(stb + half * 32) + i);
-                    const float cc[4] = {c4.x, c4.y, c4.z, c4.w}, sn[4] = {s4.x, s4.y, s4.z, s4.w};
-                    float ol[4], oh[4];
+        for (int h = 0; h < MH; ++h) {
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                      const float a = __uint_as_float(lo[4 * i + j]) * rs, b2 = __uint_as_float(hi[4 * i + j]) * rs;
-                      ol[j] = a * cc[j] - b2 * sn[j];
-                      oh[j] = b2 * cc[j] + a * sn[j];
+          for (int h2 = 0; h2 < 2; ++h2) {
+#define ACC(j, e) acc[h][4 * (j) + 2 * h2 + (e)]
+            const int row = m_blk * BM + h * 64 + fr + 8 * h2;
+            const bool row_ok = row < p.M;
+            int orow = row;
+            if (p.rows_per_group > 0) orow = (row / p.rows_per_group) * p.group_stride + (row % p.rows_per_group) + p.row_offset;
+            // deferred RMSNorm: the operand rows were not normalised; their scale commutes with the GEMM and lands here
+            float rs = 1.f;
+            if (p.rowscale.ssq != nullptr && row_ok) {
+              const float* sp = p.rowscale.ssq + (size_t)row * p.rowscale.slots;
+              float ss = 0.f;
+              for (int i = 0; i < p.rowscale.slots; ++i) ss += __ldg(sp + i);       // fixed order: deterministic
+              rs = rsqrtf(ss * p.rowscale.inv_dim + p.rowscale.eps);
+            }
+            if (p.rope.cos != nullptr) {
+              // ---- fused QKV epilogue: RoPE on q / k heads, store q|k|v rows, append k / v to the paged cache (whole heads per tile)
+              if constexpr (BN % 128 == 0) {
+                const GemmRope& R = p.rope;
+                if (row_ok) {
+                  const int bq = row / R.S, sq = row % R.S;
+                  const int pad = (R.left_pad != nullptr) ? __ldg(R.left_pad + bq) : 0;
+                  const int cpos = sq - pad;                               // index inside the (compact) KV cache
+                  const bool cached = cpos >= 0;                           // padding rows are neither rotated nor cached
+                  const int pos = R.pos_from_mask ? (cpos > 0 ? cpos : 0) : sq;
+                  int page = 0, slot = 0;
+                  if (cached) { page = __ldg(R.page_table + (size_t)bq * R.pages_per_seq + cpos / R.page_tokens); slot = cpos % R.page_tokens; }
+                  const float* ct = R.cos + (size_t)pos * 64;
+                  const float* stb = R.sin + (size_t)pos * 64;
+                  bf16* orow_ptr = reinterpret_cast<bf16*>(p.out) + (size_t)orow * p.ldo;
+#pragma unroll
+                  for (int hh = 0; hh < BN / 128; ++hh) {
+                    const int hcol = col_tile + hh * 128;                  // first column of this head inside [q | k | v]
+                    if (hcol < p.N) {
+                      const int region = hcol / R.T, head = (hcol % R.T) / 128;
+                      bf16* cdst = (region >= 1 && cached) ? R.kv_pages + ((((size_t)page * 2 + (region - 1)) * R.H + head) * R.page_tokens + slot) * 128 : nullptr;
+#pragma unroll
+                      for (int jj = 0; jj < 8; ++jj) {                     // dims d = 8 jj + fc (+1) pair with d + 64 (HF rotate_half)
+                        const int d = 8 * jj + fc;
+                        float lo0 = ACC(hh * 16 + jj, 0) * rs, lo1 = ACC(hh * 16 + jj, 1) * rs;
+                        float hi0 = ACC(hh * 16 + jj + 8, 0) * rs, hi1 = ACC(hh * 16 + jj + 8, 1) * rs;
+                        if (region < 2 && cached) {
+                          const float2 c2 = __ldg(reinterpret_cast<const float2*>(ct + d));
+                          const float2 s2 = __ldg(reinterpret_cast<const float2*>(stb + d));
+                          const float a0 = lo0, b0 = hi0, a1 = lo1, b1 = hi1;
+                          lo0 = a0 * c2.x - b0 * s2.x; hi0 = b0 * c2.x + a0 * s2.x;
+                          lo1 = a1 * c2.y - b1 * s2.y; hi1 = b1 * c2.y + a1 * s2.y;
+                        }
+                        const uint32_t plo = pack_bf16x2(lo0, lo1), phi = pack_bf16x2(hi0, hi1);
+                        *reinterpret_cast<uint32_t*>(orow_ptr + hcol + d) = plo;
+                        *reinterpret_cast<uint32_t*>(orow_ptr + hcol + 64 + d) = phi;
+                        if (cdst != nullptr) {
+                          *reinterpret_cast<uint32_t*>(cdst + d) = plo;
+                          *reinterpret_cast<uint32_t*>(cdst + 64 + d) = phi;
+                        }
+                      }
                     }
-                    plo[2 * i] = pack_bf16x2(ol[0], ol[1]); plo[2 * i + 1] = pack_bf16x2(ol[2], ol[3]);
-                    phi[2 * i] = pack_bf16x2(oh[0], oh[1]); phi[2 * i + 1] = pack_bf16x2(oh[2], oh[3]);
-                  }
-                } else {
-#pragma unroll
-                  for (int i = 0; i < 16; ++i) {
-                    plo[i] = pack_bf16x2(__uint_as_float(lo[2 * i]) * rs, __uint_as_float(lo[2 * i + 1]) * rs);
-                    phi[i] = pack_bf16x2(__uint_as_float(hi[2 * i]) * rs, __uint_as_float(hi[2 * i + 1]) * rs);
-                  }
-                }
-                uint4* d0 = reinterpret_cast<uint4*>(orow_ptr + hcol + half * 32);
-                uint4* d1 = reinterpret_cast<uint4*>(orow_ptr + hcol + 64 + half * 32);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  d0[i] = make_uint4(plo[4 * i], plo[4 * i + 1], plo[4 * i + 2], plo[4 * i + 3]);
-                  d1[i] = make_uint4(phi[4 * i], phi[4 * i + 1], phi[4 * i + 2], phi[4 * i + 3]);
-                }
-                if (region >= 1 && cached) {
-                  bf16* cdst = R.kv_pages + ((((size_t)page * 2 + (region - 1)) * R.H + head) * R.page_tokens + slot) * 128;
-                  uint4* c0 = reinterpret_cast<uint4*>(cdst + half * 32);
-                  uint4* c1 = reinterpret_cast<uint4*>(cdst + 64 + half * 32);
-#pragma unroll
-                  for (int i = 0; i < 4; ++i) {
-                    c0[i] = make_uint4(plo[4 * i], plo[4 * i + 1], plo[4 * i + 2], plo[4 * i + 3]);
-                    c1[i] = make_uint4(phi[4 * i], phi[4 * i + 1], phi[4 * i + 2], phi[4 * i + 3]);
                   }
                 }
               }
-            }
-          }
-        } else if (p.mode == GEMM_SWIGLU_BF16) {
-          if constexpr (BN % 64 == 0) {
-            bf16* out = reinterpret_cast<bf16*>(p.out);
-#pragma unroll 1
-            for (int c = 0; c < BN / 64; ++c) {
-              uint32_t g[32], u[32];
-              tmem_ld_32x32(taddr0 + c * 64, g);
-              tmem_ld_32x32(taddr0 + c * 64 + 32, u);
-              tmem_ld_wait();
-              const int col0 = col_tile + c * 64;            // first gate column of this pair (in interleaved space)
-              if (row_ok && col0 < p.N) {
-                uint32_t pk[16];
+            } else if (p.mode == GEMM_SWIGLU_BF16) {
+              // columns interleaved [32 gate | 32 up]: gate column 8 jj + fc of a 64-block pairs with up column 8 (jj + 4) + fc
+              if constexpr (BN % 64 == 0) {
+                bf16* out = reinterpret_cast<bf16*>(p.out);
+                if (row_ok) {
 #pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                  float g0 = __uint_as_float(g[2 * i]) * rs, g1 = __uint_as_float(g[2 * i + 1]) * rs;
-                  float u0 = __uint_as_float(u[2 * i]) * rs, u1 = __uint_as_float(u[2 * i + 1]) * rs;
-                  float h0 = g0 / (1.f + __expf(-g0)) * u0;
-                  float h1 = g1 / (1.f + __expf(-g1)) * u1;
-                  pk[i] = pack_bf16x2(h0, h1);
-                }
-                uint4* dst = reinterpret_cast<uint4*>(out + (size_t)orow * p.ldo + col0 / 2);
+                  for (int c = 0; c < BN / 64; ++c) {
+                    const int col0 = col_tile + c * 64;            // first gate column of this pair (in interleaved space)
+                    if (col0 < p.N) {
 #pragma unroll
-                for (int i = 0; i < 4; ++i) dst[i] = make_uint4(pk[4 * i], pk[4 * i + 1], pk[4 * i + 2], pk[4 * i + 3]);
-              }
-            }
-          }
-        } else {
-          float ssq_acc = 0.f;     // GemmEmitNorm: this tile's share of the row's sum of squares
-#pragma unroll 1
-          for (int c = 0; c < BN / C::CH; ++c) {
-            uint32_t v[C::CH];
-            if constexpr (C::CH == 32) tmem_ld_32x32(taddr0 + c * C::CH, v);
-            else tmem_ld_32x16(taddr0 + c * C::CH, reinterpret_cast<uint32_t(&)[16]>(v));
-            tmem_ld_wait();
-            const int col0 = col_tile + c * C::CH;
-            if (!row_ok || col0 >= p.N) continue;
-            const bool full = (col0 + C::CH <= p.N);
-            float x[C::CH];
-#pragma unroll
-            for (int i = 0; i < C::CH; ++i) x[i] = __uint_as_float(v[i]) * rs;
-            if (p.bias != nullptr) {
-              if (full) {
-                const float4* bp = reinterpret_cast<const float4*>(p.bias + col0);
-#pragma unroll
-                for (int i = 0; i < C::CH / 4; ++i) {
-                  float4 b4 = __ldg(bp + i);
-                  x[4 * i] += b4.x; x[4 * i + 1] += b4.y; x[4 * i + 2] += b4.z; x[4 * i + 3] += b4.w;
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < C::CH; ++i) if (col0 + i < p.N) x[i] += __ldg(p.bias + col0 + i);
-              }
-            }
-            if (p.mode == GEMM_STORE_BF16) {
-              if (p.act != ACT_NONE) {
-#pragma unroll
-                for (int i = 0; i < C::CH; ++i) x[i] = apply_act(x[i], p.act);
-              }
-              bf16* out = reinterpret_cast<bf16*>(p.out) + (size_t)orow * p.ldo + col0;
-              if (full && (p.ldo & 7) == 0) {
-                uint4* dst = reinterpret_cast<uint4*>(out);
-#pragma unroll
-                for (int i = 0; i < C::CH / 8; ++i)
-                  dst[i] = make_uint4(pack_bf16x2(x[8 * i], x[8 * i + 1]), pack_bf16x2(x[8 * i + 2], x[8 * i + 3]),
-                                      pack_bf16x2(x[8 * i + 4], x[8 * i + 5]), pack_bf16x2(x[8 * i + 6], x[8 * i + 7]));
-              } else {
-#pragma unroll
-                for (int i = 0; i < C::CH; ++i) if (col0 + i < p.N) out[i] = __float2bfloat16(x[i]);
-              }
-            } else {  // GEMM_ADD_F32
-              float* out = reinterpret_cast<float*>(p.out) + (size_t)orow * p.ldo + col0;
-              const float* rt = p.rowtab ? p.rowtab + (size_t)(row % p.rowtab_period) * p.N + col0 : nullptr;
-              if (full && (p.ldo & 3) == 0 && (p.N & 3) == 0) {
-                // all loads first, then the arithmetic, then all stores: with the loads interleaved between stores to a second
-                // (possibly aliasing) output the compiler has to serialise one L2 round trip per float4
-                float4* __restrict__ dst = reinterpret_cast<float4*>(out);
-                float4 oldv[C::CH / 4];
-                if (p.accumulate) {
-#pragma unroll
-                  for (int i = 0; i < C::CH / 4; ++i) oldv[i] = dst[i];
-                }
-#pragma unroll
-                for (int i = 0; i < C::CH / 4; ++i) {
-                  if (rt) {
-                    const float4 r4 = __ldg(reinterpret_cast<const float4*>(rt) + i);
-                    x[4 * i] += r4.x; x[4 * i + 1] += r4.y; x[4 * i + 2] += r4.z; x[4 * i + 3] += r4.w;
-                  }
-                  if (p.accumulate) { x[4 * i] += oldv[i].x; x[4 * i + 1] += oldv[i].y; x[4 * i + 2] += oldv[i].z; x[4 * i + 3] += oldv[i].w; }
-                }
-#pragma unroll
-                for (int i = 0; i < C::CH / 4; ++i) dst[i] = make_float4(x[4 * i], x[4 * i + 1], x[4 * i + 2], x[4 * i + 3]);
-                if (p.emit.xw != nullptr) {
-                  uint2* __restrict__ xd = reinterpret_cast<uint2*>(p.emit.xw + (size_t)orow * p.emit.ldxw + col0);
-                  const float4* __restrict__ wp = reinterpret_cast<const float4*>(p.emit.norm_w + col0);
-#pragma unroll
-                  for (int i = 0; i < C::CH / 4; ++i) {
-                    const float4 w4 = __ldg(wp + i);
-                    ssq_acc += x[4 * i] * x[4 * i] + x[4 * i + 1] * x[4 * i + 1] + x[4 * i + 2] * x[4 * i + 2] + x[4 * i + 3] * x[4 * i + 3];
-                    xd[i] = make_uint2(pack_bf16x2(x[4 * i] * w4.x, x[4 * i + 1] * w4.y), pack_bf16x2(x[4 * i + 2] * w4.z, x[4 * i + 3] * w4.w));
+                      for (int jj = 0; jj < 4; ++jj) {
+                        const float g0 = ACC(8 * c + jj, 0) * rs, g1 = ACC(8 * c + jj, 1) * rs;
+                        const float u0 = ACC(8 * c + jj + 4, 0) * rs, u1 = ACC(8 * c + jj + 4, 1) * rs;
+                        const float h0 = g0 / (1.f + __expf(-g0)) * u0;
+                        const float h1 = g1 / (1.f + __expf(-g1)) * u1;
+                        bf16* dst = out + (size_t)orow * p.ldo + col0 / 2 + 8 * jj + fc;
+                        if ((p.ldo & 1) == 0) *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(h0, h1);
+                        else { dst[0] = __float2bfloat16(h0); dst[1] = __float2bfloat16(h1); }
+                      }
+                    }
                   }
                 }
-              } else {
+              }
+            } else {
+              float ssq_acc = 0.f;     // GemmEmitNorm: this thread's share of the row's sum of squares over the tile
+              if (row_ok) {
 #pragma unroll
-                for (int i = 0; i < C::CH; ++i) {
-                  if (col0 + i < p.N) {
-                    float o = x[i];
-                    if (rt) o += __ldg(rt + i);
-                    if (p.accumulate) o += out[i];
-                    out[i] = o;
+                for (int j = 0; j < BN / 8; ++j) {
+                  const int col = col_tile + 8 * j + fc;
+                  if (col >= p.N) continue;
+                  const bool two = col + 1 < p.N;
+                  float x0 = ACC(j, 0) * rs, x1 = ACC(j, 1) * rs;
+                  if (p.bias != nullptr) { x0 += __ldg(p.bias + col); if (two) x1 += __ldg(p.bias + col + 1); }
+                  if (p.mode == GEMM_STORE_BF16) {
+                    if (p.act != ACT_NONE) { x0 = apply_act(x0, p.act); x1 = apply_act(x1, p.act); }
+                    bf16* out = reinterpret_cast<bf16*>(p.out) + (size_t)orow * p.ldo + col;
+                    if (two && (p.ldo & 1) == 0) *reinterpret_cast<uint32_t*>(out) = pack_bf16x2(x0, x1);
+                    else { out[0] = __float2bfloat16(x0); if (two) out[1] = __float2bfloat16(x1); }
+                  } else {  // GEMM_ADD_F32
+                    float* out = reinterpret_cast<float*>(p.out) + (size_t)orow * p.ldo + col;
+                    if (p.rowtab) {
+                      const float* rt = p.rowtab + (size_t)(row % p.rowtab_period) * p.N + col;
+                      x0 += __ldg(rt); if (two) x1 += __ldg(rt + 1);
+                    }
+                    if (two && (p.ldo & 1) == 0) {
+                      float2* o2 = reinterpret_cast<float2*>(out);
+                      if (p.accumulate) { const float2 old = *o2; x0 += old.x; x1 += old.y; }
+                      *o2 = make_float2(x0, x1);
+                    } else {
+                      if (p.accumulate) { x0 += out[0]; if (two) x1 += out[1]; }
+                      out[0] = x0; if (two) out[1] = x1;
+                    }
                     if (p.emit.xw != nullptr) {
-                      ssq_acc += o * o;
-                      p.emit.xw[(size_t)orow * p.emit.ldxw + col0 + i] = __float2bfloat16(o * __ldg(p.emit.norm_w + col0 + i));
+                      bf16* xd = p.emit.xw + (size_t)orow * p.emit.ldxw + col;
+                      const float y0 = x0 * __ldg(p.emit.norm_w + col);
+                      ssq_acc += x0 * x0;
+                      if (two) {
+                        const float y1 = x1 * __ldg(p.emit.norm_w + col + 1);
+                        ssq_acc += x1 * x1;
+                        if ((p.emit.ldxw & 1) == 0) *reinterpret_cast<uint32_t*>(xd) = pack_bf16x2(y0, y1);
+                        else { xd[0] = __float2bfloat16(y0); xd[1] = __float2bfloat16(y1); }
+                      } else {
+                        xd[0] = __float2bfloat16(y0);
+                      }
                     }
                   }
                 }
               }
+              if (p.emit.ssq_out != nullptr) {
+                // the 4 lanes of a quad hold one row
+                ssq_acc += __shfl_xor_sync(0xffffffffu, ssq_acc, 1);
+                ssq_acc += __shfl_xor_sync(0xffffffffu, ssq_acc, 2);
+                if (row_ok && (lane & 3) == 0) p.emit.ssq_out[(size_t)orow * p.n_tiles + n_blk] = ssq_acc;
+              }
             }
+#undef ACC
           }
-          if (p.emit.ssq_out != nullptr && row_ok) p.emit.ssq_out[(size_t)orow * p.n_tiles + n_blk] = ssq_acc;
         }
       }
-      // release this accumulator stage back to the MMA warp (pair: the leader's)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) { if (TWO && !leader) mbar_arrive_cluster(tempty_bar(acc), 0); else mbar_arrive(tempty_bar(acc)); }
-      acc ^= 1;
-      if (acc == 0) accphase ^= 1u;
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if constexpr (TWO) cluster_barrier();        // the peer may still address this CTA's barriers / shared memory / TMEM
   trace.done();
-  if (warp == 1) { if constexpr (TWO) tmem_dealloc_2cta(tmem_base, C::TMEM_COLS); else tmem_dealloc(tmem_base, C::TMEM_COLS); }
 }
 
 VCLA_DEFINE_TRACE_SETTER(trace_set_gemm)
@@ -668,14 +539,15 @@ static PFN_encodeTiled g_encode = nullptr;
 static std::once_flag g_gemm_once;
 static int g_gemm_init_rc = 0;
 
-template <int BN, int STAGES, bool SWAP, int CTAS = 1>
+template <int BM, int BN, int STAGES, bool SWAP>
 static int set_attr() {
-  using C = GemmCfg<BN, STAGES, CTAS>;
-  VCLA_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, SWAP, CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+  using C = GemmCfg<BM, BN, STAGES>;
+  VCLA_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BM, BN, STAGES, SWAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
   return 0;
 }
 
-// tile configurations (BN, STAGES): prefill 256x4 / 128x6 / 64x8 ; decode swap-AB 16x5 / 32x5 / 64x4 (two CTAs per SM)
+// tile configurations (BM x BN, STAGES): prefill 64x256x5 / 128x128x6 / 128x64x8 ; decode swap-AB 128 x {16x5, 32x5, 64x4}
+// (two CTAs per SM).  Every configuration keeps <= 128 accumulator registers per thread of the single wgmma warpgroup.
 static int gemm_init_impl() {
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
@@ -685,13 +557,12 @@ static int gemm_init_impl() {
     return -1;
   }
   g_encode = reinterpret_cast<PFN_encodeTiled>(fn);
-  if (set_attr<256, 4, false>()) return -1;
-  if (set_attr<256, 6, false, 2>()) return -1;
-  if (set_attr<128, 6, false>()) return -1;
-  if (set_attr<64, 8, false>()) return -1;
-  if (set_attr<16, 5, true>()) return -1;
-  if (set_attr<32, 5, true>()) return -1;
-  if (set_attr<64, 4, true>()) return -1;
+  if (set_attr<64, 256, 5, false>()) return -1;
+  if (set_attr<128, 128, 6, false>()) return -1;
+  if (set_attr<128, 64, 8, false>()) return -1;
+  if (set_attr<128, 16, 5, true>()) return -1;
+  if (set_attr<128, 32, 5, true>()) return -1;
+  if (set_attr<128, 64, 4, true>()) return -1;
   return 0;
 }
 int gemm_init() {
@@ -719,29 +590,25 @@ static int make_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t co
   return 0;
 }
 
-template <int BN, int STAGES, bool SWAP, int CTAS = 1>
+template <int BM, int BN, int STAGES, bool SWAP>
 static int launch(const GemmCall& c, GemmParams p, cudaStream_t st) {
-  using C = GemmCfg<BN, STAGES, CTAS>;
+  using C = GemmCfg<BM, BN, STAGES>;
   CUtensorMap ta, tb;
-  if (make_tmap(&ta, c.A, c.M, c.K, c.lda, kBlockM)) return -1;
-  if (make_tmap(&tb, c.B, c.N, c.K, c.ldb, BN / CTAS)) return -1;
+  if (make_tmap(&ta, c.A, c.M, c.K, c.lda, BM)) return -1;
+  if (make_tmap(&tb, c.B, c.N, c.K, c.ldb, BN)) return -1;
+  p.m_tiles = (c.M + BM - 1) / BM;
   p.n_tiles = (c.N + BN - 1) / BN;
-  p.total_tiles = (CTAS == 2 ? (p.m_tiles + 1) / 2 : p.m_tiles) * p.n_tiles * p.splits;     // pair-tiles of 256 rows
-  const int slots = CTAS == 2 ? num_sms() / 2 : num_sms() * (SWAP ? 2 : 1);
-  const int grid = (p.total_tiles < slots ? p.total_tiles : slots) * CTAS;
+  p.total_tiles = p.m_tiles * p.n_tiles * p.splits;
+  const int slots = num_sms() * (SWAP ? 2 : 1);
+  const int grid = p.total_tiles < slots ? p.total_tiles : slots;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(kGemmThreads);
   cfg.dynamicSmemBytes = C::SMEM_BYTES;
   cfg.stream = st;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   int nattr = 0;
-  if (CTAS == 2) {
-    attr[nattr].id = cudaLaunchAttributeClusterDimension;
-    attr[nattr].val.clusterDim.x = 2; attr[nattr].val.clusterDim.y = 1; attr[nattr].val.clusterDim.z = 1;
-    ++nattr;
-  }
   if (pdl_enabled()) {
     attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[nattr].val.programmaticStreamSerializationAllowed = 1;
@@ -754,25 +621,17 @@ static int launch(const GemmCall& c, GemmParams p, cudaStream_t st) {
     if (!once) {
       once = true;
       int per_sm = -1;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_tc_kernel<BN, STAGES, SWAP, CTAS>, kGemmThreads, C::SMEM_BYTES);
-      fprintf(stderr, "[vcla] gemm_tc<%d,%d,%d,%d>: smem %d, occupancy query %d blocks/SM, grid %d\n", BN, STAGES, (int)SWAP, CTAS, C::SMEM_BYTES, per_sm, grid);
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_tc_kernel<BM, BN, STAGES, SWAP>, kGemmThreads, C::SMEM_BYTES);
+      fprintf(stderr, "[vcla] gemm_tc<%d,%d,%d,%d>: smem %d, occupancy query %d blocks/SM, grid %d\n", BM, BN, STAGES, (int)SWAP, C::SMEM_BYTES, per_sm, grid);
     }
   }
-  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, STAGES, SWAP, CTAS>, ta, tb, p));
+  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BM, BN, STAGES, SWAP>, ta, tb, p));
   return 0;
 }
 
-// CTA-pair tiles (cta_group::2): on by default for the 256-wide prefill tile; VCLA_GEMM_2CTA=0 keeps the single-CTA 128 x 256 tile
-static int g_two_cta = -1;
-static bool two_cta_enabled() {
-  if (g_two_cta < 0) { const char* e = getenv("VCLA_GEMM_2CTA"); g_two_cta = (e == nullptr) ? 1 : (atoi(e) != 0); }
-  return g_two_cta != 0;
-}
-void gemm_set_two_cta(int on) { g_two_cta = on ? 1 : 0; }
-
 // tile width of a non-swap GEMM with M rows and N output columns (the widest tile that still gives every SM work)
 int gemm_pick_bn(int M, int N) {
-  const long m_tiles = (M + kBlockM - 1) / kBlockM;
+  const long m_tiles = (M + 127) / 128;
   const long tiles256 = m_tiles * ((N + 255) / 256);
   const long tiles128 = m_tiles * ((N + 127) / 128);
   if (tiles256 >= num_sms() || N >= 4096) return 256;
@@ -787,7 +646,7 @@ int gemm_tc(const GemmCall& c, cudaStream_t st) {
   GemmParams p;
   memset(&p, 0, sizeof(p));
   p.M = c.M; p.N = c.N; p.K = c.K;
-  p.m_tiles = (c.M + kBlockM - 1) / kBlockM;
+  p.m_tiles = (c.M + kSwapBlockM - 1) / kSwapBlockM;
   p.kb_total = (c.K + kBlockK - 1) / kBlockK;
   p.mode = c.mode; p.act = c.act; p.accumulate = c.accumulate;
   p.out = c.out; p.ldo = c.ldo; p.bias = c.bias;
@@ -809,9 +668,9 @@ int gemm_tc(const GemmCall& c, cudaStream_t st) {
     if (c.N > 64 || c.ws_rows < c.N) { set_error("gemm: swap-AB batch rows %d (ws_rows %d) unsupported", c.N, c.ws_rows); return -1; }
     if (c.fix.mode != FIX_NONE && (c.fix.tile_counters == nullptr || c.ws_rows != c.N || c.ldo != c.M)) { set_error("gemm: split-K fixup needs tile counters, ws_rows == batch and ldo == rows"); return -1; }
     if (c.fix.mode == FIX_SWIGLU && (c.M % 64) != 0) { set_error("gemm: SwiGLU fixup needs rows %% 64 == 0"); return -1; }
-    if (c.N <= 16) return launch<16, 5, true>(c, p, st);
-    if (c.N <= 32) return launch<32, 5, true>(c, p, st);
-    return launch<64, 4, true>(c, p, st);
+    if (c.N <= 16) return launch<128, 16, 5, true>(c, p, st);
+    if (c.N <= 32) return launch<128, 32, 5, true>(c, p, st);
+    return launch<128, 64, 4, true>(c, p, st);
   }
   p.splits = 1;
   p.kb_per_split = p.kb_total;
@@ -823,10 +682,9 @@ int gemm_tc(const GemmCall& c, cudaStream_t st) {
   int bn = c.bn;
   if (c.rope.cos != nullptr) bn = 256;    // two whole heads per tile
   if (bn == 0) bn = gemm_pick_bn(c.M, c.N);
-  if (bn == 256 && two_cta_enabled() && p.m_tiles >= 2) return launch<256, 6, false, 2>(c, p, st);
-  if (bn == 256) return launch<256, 4, false>(c, p, st);
-  if (bn == 128) return launch<128, 6, false>(c, p, st);
-  if (bn == 64) return launch<64, 8, false>(c, p, st);
+  if (bn == 256) return launch<64, 256, 5, false>(c, p, st);
+  if (bn == 128) return launch<128, 128, 6, false>(c, p, st);
+  if (bn == 64) return launch<128, 64, 8, false>(c, p, st);
   set_error("gemm: unsupported tile N %d", bn);
   return -1;
 }

@@ -1,12 +1,12 @@
-// Decode weight-streaming GEMM with the split-K reduction INSIDE a thread-block cluster (sm_100a).
+// Decode weight-streaming GEMM with the split-K reduction INSIDE a thread-block cluster (sm_90a).
 //
-//   out[b, n] = sum_k W[n, k] * x[b, k]        W = nn.Linear weight [N_out, K] (the 128-row UMMA M operand, streamed once from HBM
-//                                              through TMA), x = the <= 32 activation rows of the batch (the UMMA N operand)
+//   out[b, n] = sum_k W[n, k] * x[b, k]        W = nn.Linear weight [N_out, K] (the 128-row wgmma M operand, streamed once from HBM
+//                                              through TMA), x = the <= 32 activation rows of the batch (the wgmma N operand)
 //
 // gemm.cu's swap-AB kernel writes one fp32 partial per K split to an L2 workspace and leaves the reduction to the next kernel
 // (dec_resid_norm / dec_silu_mul / the attention prologue): 3 extra kernel boundaries per layer and S x the output in L2 traffic.
 // Here the S CTAs that share a 128-row tile form ONE CLUSTER (cluster dims (S,1,1), S <= 8): each CTA accumulates its K slice in
-// TMEM, then the cluster reduce-scatters over the batch columns through distributed shared memory -- CTA r receives, from every
+// registers, then the cluster reduce-scatters over the batch columns through distributed shared memory -- CTA r receives, from every
 // peer, the columns it owns (st.shared::cluster into its buffer, one remote mbarrier arrive per peer) -- sums them in a fixed
 // order (deterministic) and applies the consumer that used to be a kernel of its own:
 //   CSK_OUT_F32 : out[b, n]  = rstd[b] * acc                                   (fused QKV projection, lm_head)
@@ -20,8 +20,8 @@
 // is one remote arrive per peer and tile), 1 = one buffer + a second 'consumed' barrier, which frees shared memory for a deeper TMA
 // ring (used for the 32-column batch tile).  Two CTAs per SM; the launch assumes that occupancy (see csk_max_clusters).
 //
-// Per CTA (192 threads): warp 0 = TMA producer (weight tiles are requested BEFORE griddepcontrol.wait: they never depend on the
-// previous kernel), warp 1 = tcgen05.mma issuer + TMEM owner, warps 2..5 = epilogue: TMEM -> peers' smem -> reduce -> consumer.
+// Per CTA (160 threads): warp 4 = TMA producer (weight tiles are requested BEFORE griddepcontrol.wait: they never depend on the
+// previous kernel), warps 0..3 = one wgmma warpgroup: MMAs (2 x m64nBNk16 per k step) -> peers' smem -> reduce -> consumer.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -32,7 +32,7 @@
 
 namespace vcla {
 
-constexpr int kCskThreads = 192;
+constexpr int kCskThreads = 160;
 constexpr int kCskBlockM = 128;
 constexpr int kCskBlockK = 64;
 constexpr int kCskMaxSplits = 8;
@@ -59,9 +59,8 @@ struct CskCfg {
   static constexpr int RED_BYTES = RED_COLS * kCskBlockM * 4;             // one reduce buffer: [source][owned column][128 rows] fp32
   static constexpr int RED_OFF = STAGES * STAGE_BYTES;
   static constexpr int BAR_OFF = RED_OFF + NBUF * RED_BYTES;        // NBUF = 2: double-buffered reduce; 1: one buffer + a 'consumed' barrier
-  static constexpr int MISC_OFF = BAR_OFF + 256;                          // rstd[BN], ssq warp partials [4][BN], tmem slot
+  static constexpr int MISC_OFF = BAR_OFF + 256;                          // rstd[BN], ssq warp partials [4][BN]
   static constexpr int SMEM_BYTES = MISC_OFF + 1024 + 1024;              // + slack for the 1024 B alignment of the ring
-  static constexpr int TMEM_COLS = (2 * BN <= 32) ? 32 : 64;
   static_assert(STAGE_BYTES % 1024 == 0, "stage must keep 1024 B alignment for SWIZZLE_128B");
   static_assert(BN == 16 || BN == 32, "decode batch tile");
 };
@@ -89,10 +88,7 @@ __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity)
   if (mbar_try_wait_cluster(bar, parity)) return;
   long long t0 = clock64();
   while (!mbar_try_wait_cluster(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {
-      printf("vcla: cluster mbarrier wait timeout (block %d thread %d bar 0x%x parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();   // no printf: a call anywhere in the kernel serialises its wgmma
   }
 }
 __device__ __forceinline__ void cluster_sync_all() {
@@ -110,13 +106,9 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
   const uint32_t bar0 = base + C::BAR_OFF;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar0 + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar0 + 8u * (2 * STAGES + 2 + a); };
-  auto red_bar = [&](int b) { return bar0 + 8u * (2 * STAGES + 4 + b); };
+  auto red_bar = [&](int b) { return bar0 + 8u * (2 * STAGES + b); };
   float* s_rstd = reinterpret_cast<float*>(base_ptr + C::MISC_OFF);                 // [BN]
   float* s_part = s_rstd + BN;                                                       // [4][BN] warp partial sums of squares
-  const uint32_t tmem_slot = base + C::MISC_OFF + 4u * (BN + 4 * BN);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + C::MISC_OFF + 4 * (BN + 4 * BN));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = p.splits;
@@ -126,27 +118,22 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
     for (int b = 0; b < 2; ++b) mbar_init(red_bar(b), (uint32_t)S);            // one arrive per source CTA (this one included)
     fence_barrier_init();
     tma_prefetch_desc(&tmW);
     tma_prefetch_desc(&tmX);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, C::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  // Cluster rendezvous, split: everybody ARRIVES now (this CTA's barriers are initialised), only the epilogue warps WAIT, right before
-  // their first remote access -- the TMA producer starts streaming weights without waiting for the peers to become resident.
+  // Cluster rendezvous, split: everybody ARRIVES now (this CTA's barriers are initialised), only the MMA / epilogue warps WAIT, right
+  // before their first remote access -- the TMA producer starts streaming weights without waiting for the peers to become resident.
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   pdl_launch_dependents();
 
   const int kb0 = rank * p.kb_per_split;
   const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       // ===================== TMA producer =====================
       int stage = 0; uint32_t phase = 0;
@@ -155,14 +142,13 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       uint32_t pend_dst[STAGES], pend_bar[STAGES]; int pend_c0[STAGES];
       auto flush_pending = [&]() {
         pdl_wait();
-        trace.dep();
         for (int i = 0; i < npend; ++i) tma_load_2d(pend_dst[i], &tmX, pend_c0[i], 0, pend_bar[i], p.policy_x);
         npend = 0;
         dep_ready = true;
       };
       for (int t = cluster_id; t < p.m_tiles; t += p.n_clusters) {
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
+          mbar_wait_mma(empty_bar(stage), phase ^ 1u);
           mbar_arrive_expect_tx(full_bar(stage), C::STAGE_BYTES);
           const uint32_t sa = base + stage * C::STAGE_BYTES;
           tma_load_2d(sa, &tmW, kb * kCskBlockK, t * kCskBlockM, full_bar(stage), p.policy_w);          // weights: no dependency
@@ -178,43 +164,20 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       if (!dep_ready) flush_pending();
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===================== MMA issuer =====================
-      constexpr uint32_t idesc = make_idesc_bf16(kCskBlockM, BN);
-      int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t accphase = 0;
-      for (int t = cluster_id; t < p.m_tiles; t += p.n_clusters) {
-        mbar_wait(tempty_bar(acc), accphase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sa = base + stage * C::STAGE_BYTES;
-          const uint64_t adesc = make_desc_sw128(sa), bdesc = make_desc_sw128(sa + C::A_BYTES);
-#pragma unroll
-          for (int k = 0; k < kCskBlockK / 16; ++k) umma_bf16(d_tmem, adesc + 2u * k, bdesc + 2u * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          umma_commit(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(tfull_bar(acc));
-        acc ^= 1;
-        if (acc == 0) accphase ^= 1u;
-      }
-    }
-    __syncwarp();
   } else {
-    // ===================== epilogue warps: TMEM -> reduce-scatter over the cluster -> consumer =====================
-    const int q = warp & 3;                         // TMEM lane quadrant
-    const int row_in_tile = q * 32 + lane;
-    const int et = (warp - 2) * 32 + lane;          // 0..127 inside the epilogue group
+    // ===================== wgmma warpgroup: MMAs -> reduce-scatter over the cluster -> consumer =====================
+    const int q = warp;
+    const int row_in_tile = q * 32 + lane;          // this thread's row in the reduce / consumer phase
+    const int et = row_in_tile;                     // 0..127 inside the warpgroup
+    const int fr = warp * 16 + (lane >> 2), fc = 2 * (lane & 3);   // accumulator fragment: rows fr (+8) of each 64-row block
     const int cols_per = (p.B + S - 1) / S;         // batch columns owned by one CTA
     const int my_c0 = rank * cols_per;
     const int my_nc = max(0, min(cols_per, p.B - my_c0));
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");   // every peer's reduce barriers exist from here on
     pdl_wait();                                     // everything below reads / writes buffers of the previous kernels
+    trace.dep();                                    // (the trace slot belongs to thread 0, a thread of this warpgroup)
     // deferred RMSNorm scale of the operand rows
-    for (int b = warp - 2; b < BN; b += 4) {
+    for (int b = warp; b < BN; b += 4) {
       float v = 1.f;
       if (p.ssq_in != nullptr && b < p.B) {
         float ss = 0.f;
@@ -226,22 +189,36 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
 
-    int acc = 0; uint32_t accphase = 0; int buf = 0; uint32_t redphase[2] = {0u, 0u};
+    int stage = 0; uint32_t phase = 0;
+    int buf = 0; uint32_t redphase[2] = {0u, 0u};
+    float acc[2][BN / 2];
     // NBUF == 1: red_bar(1) counts, per tile, the S destinations that have consumed what this CTA delivered ("your slot in my buffer
     // is free again"); the scatter of the next tile waits for it.  A deeper TMA ring fits in the shared memory this saves.
     uint32_t freephase = 0u; bool first_tile = true;
     for (int t = cluster_id; t < p.m_tiles; t += p.n_clusters) {
       const bool last_tile = t + p.n_clusters >= p.m_tiles;
-      mbar_wait(tfull_bar(acc), accphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN);
-      uint32_t v[BN];
-      if constexpr (BN == 32) tmem_ld_32x32(taddr, v);
-      else tmem_ld_32x16(taddr, reinterpret_cast<uint32_t(&)[16]>(v));
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));               // the MMA warp may start the next tile
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait_mma(full_bar(stage), phase);
+        const uint32_t sa = base + stage * C::STAGE_BYTES;
+        const uint64_t bdesc = make_desc_sw128(sa + C::A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kCskBlockK / 16; ++k) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            wgmma_bf16<BN>(acc[h], make_desc_sw128(sa + h * 64 * 128) + 2u * k, bdesc + 2u * k, (kb > kb0 || k > 0) ? 1 : 0);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                            // the previous k-block's MMAs are done reading their stage
+        if (prev >= 0 && threadIdx.x == 0) mbar_arrive(empty_bar(prev));
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+      if (prev >= 0 && threadIdx.x == 0) mbar_arrive(empty_bar(prev));
       if constexpr (NBUF == 1) {
         if (!first_tile) { mbar_wait_cluster(red_bar(1), freephase); freephase ^= 1u; }
         first_tile = false;
@@ -249,11 +226,22 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       // scatter: column c of this partial goes to CTA c / cols_per, slot [source = rank][c % cols_per][row]
       const uint32_t red_local = base + C::RED_OFF + (uint32_t)buf * C::RED_BYTES;
 #pragma unroll
-      for (int c = 0; c < BN; ++c) {
-        if (c < p.B) {
-          const int dst = c / cols_per, cl = c - dst * cols_per;
-          const uint32_t off = (uint32_t)(((rank * cols_per + cl) * kCskBlockM + row_in_tile) * 4);
-          st_cluster_f32(mapa_u32(red_local + off, (uint32_t)dst), __uint_as_float(v[c]));
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int h2 = 0; h2 < 2; ++h2) {
+          const int r = h * 64 + fr + 8 * h2;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = 8 * j + fc + e;
+              if (c < p.B) {
+                const int dst = c / cols_per, cl = c - dst * cols_per;
+                const uint32_t off = (uint32_t)(((rank * cols_per + cl) * kCskBlockM + r) * 4);
+                st_cluster_f32(mapa_u32(red_local + off, (uint32_t)dst), acc[h][4 * j + 2 * h2 + e]);
+              }
+            }
+          }
         }
       }
       if (p.cluster_fence) asm volatile("fence.acq_rel.cluster;" ::: "memory");
@@ -304,7 +292,7 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
               p.xw[(size_t)b * p.M + row] = __float2bfloat16(r * __ldg(p.norm_w + row));
             }
             const float q2 = warp_sum(r * r);
-            if (lane == 0) s_part[(warp - 2) * BN + cl] = q2;
+            if (lane == 0) s_part[q * BN + cl] = q2;
           }
         }
         if (p.mode == CSK_RESID) {
@@ -320,17 +308,13 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       } else {
         buf ^= 1;
       }
-      acc ^= 1;
-      if (acc == 0) accphase ^= 1u;
     }
   }
 
   // No closing cluster barrier: a CTA leaves its last reduce only after all S peers have delivered (and arrived on) its buffer, i.e.
   // nobody addresses its shared memory afterwards, and every peer it wrote to is still waiting for exactly that delivery.
-  tc_fence_before();
   __syncthreads();
   trace.done();
-  if (warp == 1) tmem_dealloc(tmem_base, C::TMEM_COLS);
 }
 
 VCLA_DEFINE_TRACE_SETTER(trace_set_gemm_decode)
@@ -352,7 +336,7 @@ static int csk_init() {
       set_error("cuTensorMapEncodeTiled not available"); g_csk_rc = -1; return;
     }
     g_csk_encode = reinterpret_cast<PFN_encodeTiled>(fn);
-    // two CTAs per SM need (almost) the whole 228 KB as shared memory: ask for the maximum carve-out explicitly (the occupancy
+    // two CTAs per SM need (almost) the whole 228 KB of an SM as shared memory: ask for the maximum carve-out explicitly (the occupancy
     // query for cluster launches otherwise assumes a carve-out that holds only one CTA)
     auto prep = [](const void* fn, int bytes) {
       return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess &&
@@ -401,9 +385,8 @@ static int csk_max_clusters(int S) {
   int per_sm = 1;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_csk_kernel<BN, STAGES, NBUF>, kCskThreads, CskCfg<BN, STAGES, NBUF>::SMEM_BYTES) != cudaSuccess) { (void)cudaGetLastError(); per_sm = 1; }
   if (per_sm > 2) per_sm = 2;
-  // Measured on B200 (profiles/r2_csk_sweep_*.json): both occupancy queries answer 1 block per SM -- also for gemm.cu's swap-AB
-  // kernel, which demonstrably runs two -- while launching twice as many clusters makes every decode GEMM 10-30 % faster: the
-  // kernel is sized for 2 CTAs per SM (launch bound, <= 101 KB of shared memory), so that is what the launch assumes.
+  // Both occupancy queries may answer 1 block per SM for this cluster launch while the kernel is sized for 2 CTAs per SM (launch
+  // bound, <= 113 KB of shared memory each), so that is what the launch assumes; VCLA_CSK_OCC=1 restores the query's answer.
   int mult = 2;
   if (const char* e = getenv("VCLA_CSK_OCC")) { const int v = atoi(e); if (v >= 1 && v <= 2) mult = v; }
   if (getenv("VCLA_DEBUG")) fprintf(stderr, "[vcla] gemm_csk<%d,%d> S=%d: cluster query %d, blocks/SM %d, using x%d\n", BN, STAGES, S, n, per_sm, mult);
@@ -434,9 +417,8 @@ static int csk_launch(const CskCall& c, CskParams p, cudaStream_t st) {
   return 0;
 }
 
-// Reduce buffering, measured on B200 (profiles/r2_bench_ab.jsonl): batch <= 16 (16-column tile): double-buffered reduce + 4 TMA stages
-// (2.880 vs 2.899 ms/token at batch 8); batch 17..32 (32-column tile): ONE buffer + 'consumed' barrier, which frees the shared memory
-// for a 4th TMA stage (4.279 vs 4.375 ms/token at batch 32).  VCLA_CSK_NBUF = 1 / 2 forces one scheme for both.
+// Reduce buffering: batch <= 16 (16-column tile): double-buffered reduce + 4 TMA stages; batch 17..32 (32-column tile): ONE buffer
+// + 'consumed' barrier, which frees the shared memory for a 4th TMA stage.  VCLA_CSK_NBUF = 1 / 2 forces one scheme for both.
 static int csk_nbuf_env() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("VCLA_CSK_NBUF"); v = e != nullptr ? atoi(e) : 0; }

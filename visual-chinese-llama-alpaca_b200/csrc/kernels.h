@@ -26,7 +26,7 @@ void set_pdl(bool on);
   } while (0)
 
 // ------------------------------------------------------------------------------------------
-// tcgen05 GEMM:  D[M,N] = A[M,K] * B[N,K]^T   (both operands K-major bf16, fp32 accumulate in TMEM)
+// wgmma GEMM:  D[M,N] = A[M,K] * B[N,K]^T   (both operands K-major bf16, fp32 accumulate in registers)
 // ------------------------------------------------------------------------------------------
 enum GemmMode {
   GEMM_STORE_BF16 = 0,   // out_bf16[orow, col] = act(acc + bias[col])
@@ -104,10 +104,9 @@ struct GemmCall {
   GemmFix fix;               // fused consumer of the split-K partials (decode)
   GemmRowScale rowscale;     // deferred RMSNorm scale of the A rows (STORE_BF16 / SWIGLU_BF16)
   GemmEmitNorm emit;         // ADD_F32 + accumulate: also write the next operand + row statistics
-  GemmRope rope;             // STORE_BF16: RoPE + KV-cache append (needs BN = 256, N = 3T)
+  GemmRope rope;             // STORE_BF16: RoPE + KV-cache append (runs on the 64 x 256 tile, N = 3T)
 };
 int gemm_tc(const GemmCall& c, cudaStream_t st);
-void gemm_set_two_cta(int on);     // CTA-pair (cta_group::2) 256 x 256 tiles for the 256-wide prefill GEMMs (default on)
 int gemm_pick_bn(int M, int N);   // tile width gemm_tc picks for a non-swap GEMM (= the number of ssq slots per row it emits: ceil(N / bn))
 // correctness reference for the tests only (CUDA-core, one thread per output)
 int gemm_naive(const GemmCall& c, cudaStream_t st);
@@ -153,10 +152,10 @@ struct AttnCall {
   int causal = 0;
   const int32_t* kv_start = nullptr;   // [B] first visible kv index per sequence (left padding); null: 0
 };
-int attention_prefill(const AttnCall& c, cudaStream_t st);      // dispatches to the tcgen05 kernel (attention_tc.cu) unless switched off
-int attention_prefill_tc(const AttnCall& c, cudaStream_t st);   // tcgen05: QK^T and PV as UMMA, S / O in TMEM, Q / K / V by TMA
+int attention_prefill(const AttnCall& c, cudaStream_t st);      // dispatches to the wgmma kernel (attention_tc.cu) unless switched off
+int attention_prefill_tc(const AttnCall& c, cudaStream_t st);   // wgmma: QK^T and PV on the tensor cores, S / O in registers, Q / K / V by TMA
 int attention_prefill_mma(const AttnCall& c, cudaStream_t st);  // mma.sync m16n8k16 fallback (attention.cu)
-void attention_set_tc(int mode);                                 // 0: mma.sync everywhere, 1 (default): tcgen05 at head dim 128, 2: tcgen05 everywhere (VCLA_ATTN_TC)
+void attention_set_tc(int mode);                                 // 0: mma.sync everywhere, 1 (default): wgmma at head dim 128, 2: wgmma everywhere (VCLA_ATTN_TC)
 int trace_set_attention_tc(void* buf, unsigned long long cap);
 
 struct DecodeAttnCall {

@@ -1,5 +1,5 @@
 """`visualcla` -- drop-in replacement of the reference package's public surface
-(ref: models/visualcla/__init__.py:1-8), backed by hand-written sm_100a CUDA kernels (libvcla.so)."""
+(ref: models/visualcla/__init__.py:1-8), backed by hand-written sm_90a CUDA kernels (libvcla.so)."""
 from .modeling_visualcla import VisualCLAModel
 from .configuration_visualcla import VisualCLAConfig
 from .processing_visualcla import VisualCLAProcessor

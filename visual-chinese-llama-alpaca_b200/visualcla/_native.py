@@ -74,7 +74,6 @@ _SIGNATURES = [
     ("vcla_op_gemm_csk_clusters", C.c_int, [C.c_int, C.c_int]),
     ("vcla_debug_set_csk_splits", C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     ("vcla_debug_get_csk_splits", C.c_int, [_P, C.c_int, C.POINTER(C.c_int * 5)]),
-    ("vcla_set_gemm_two_cta", None, [C.c_int]),
     ("vcla_set_attention_tc", None, [C.c_int]),
     ("vcla_op_attention", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, C.c_int,
                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _P]),

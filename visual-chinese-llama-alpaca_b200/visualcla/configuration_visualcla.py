@@ -32,7 +32,7 @@ class VisualCLAConfig(PretrainedConfig):
     def to_path_config(self) -> Dict:
         t, v, r = self.text_config or {}, self.vision_config or {}, self.visual_resampler_config or {}
         if not self.use_visual_resampler:
-            raise NotImplementedError("the B200 path implements the resampler variant only (VisualCLA-7B-v0.1 ships "
+            raise NotImplementedError("the H100 path implements the resampler variant only (VisualCLA-7B-v0.1 ships "
                                       "use_visual_resampler=True)")
         rope = t.get("rope_theta", None)
         if rope is None:

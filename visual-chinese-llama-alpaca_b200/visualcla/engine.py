@@ -26,7 +26,7 @@ class Engine:
     def __init__(self, path_cfg: Dict, max_batch: int = 8, max_seq: int = 512, max_prefill_tokens: Optional[int] = None,
                  device: Optional[torch.device] = None, page_tokens: int = 64):
         if not torch.cuda.is_available():
-            raise N.NativeError("visualcla (B200) needs a CUDA device: there is no CPU fallback")
+            raise N.NativeError("visualcla (H100) needs a CUDA device: there is no CPU fallback")
         self.lib = N.load()
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if self.device.index is None:

@@ -3,7 +3,7 @@
 Mirrors the call signatures of ref: models/visualcla/modeling_utils.py --
 `get_model_and_tokenizer_and_processor` (:83-141), `chat` (:143-178), `chat_in_stream` (:180-247),
 `hijack_samplers` (:395-400), `DEFAULT_GENERATION_CONFIG` (:36-47) -- so that scripts/inference/*.py run
-unchanged, while the model underneath is the B200-native engine.
+unchanged, while the model underneath is the H100-native engine.
 """
 from __future__ import annotations
 
@@ -84,7 +84,7 @@ def get_model_and_tokenizer_and_processor(visualcla_model=None, text_model=None,
                                           torch_dtype=torch.float16, default_device=None, device_map=None,
                                           load_in_8bit=False, **engine_kwargs):
     """Same signature and return triple as the reference loader (:83-141).  `engine_kwargs` (max_batch, max_seq,
-    max_prefill_tokens) size the device arenas of the B200 engine."""
+    max_prefill_tokens) size the device arenas of the H100 engine."""
     from transformers import CLIPImageProcessor, LlamaTokenizer
     tokenizer = _attach_image_tokens(LlamaTokenizer.from_pretrained(visualcla_model or lora_model))
     if visualcla_model is not None:

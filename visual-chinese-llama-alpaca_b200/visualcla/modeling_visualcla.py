@@ -1,4 +1,4 @@
-"""VisualCLAModel on the B200-native path.
+"""VisualCLAModel on the H100-native path.
 
 Same public surface as the reference's composite model (ref: models/visualcla/modeling_visualcla.py:70-404):
 `from_pretrained / from_merged_pretrained / from_vision_text_pretrained`, `forward`, `generate`,
@@ -6,7 +6,7 @@ Same public surface as the reference's composite model (ref: models/visualcla/mo
 `.image_processor`, `.num_patch`, `.image_at_head`, `.device`, `.config`, `.text_model`, `.vision_model`,
 `.visual_resampler`, `.image_projection_layer`) and the nn.Module verbs they use (`.eval() .float() .half()
 .to() .state_dict() .resize_token_embeddings()`).  Underneath there are no nn.Modules: all arithmetic runs in
-hand-written sm_100a kernels behind the C ABI in include/vcla.h (see engine.py / _native.py).
+hand-written sm_90a kernels behind the C ABI in include/vcla.h (see engine.py / _native.py).
 """
 from __future__ import annotations
 
@@ -85,7 +85,7 @@ class VisualCLAModel:
         if config is None:
             raise ValueError("VisualCLAModel needs a VisualCLAConfig")
         if vision_model is not None or text_model is not None:
-            raise NotImplementedError("pre-built nn.Module sub-models are not used on the B200 path; load weights with "
+            raise NotImplementedError("pre-built nn.Module sub-models are not used on the H100 path; load weights with "
                                       "from_merged_pretrained / from_vision_text_pretrained / load_state_dict")
         self.config = config
         self._engine = Engine(config.to_path_config(), max_batch=max_batch, max_seq=max_seq,
@@ -117,13 +117,13 @@ class VisualCLAModel:
     def requires_grad_(self, *_a, **_k): return self
     def train(self, mode: bool = False):
         if mode:
-            raise NotImplementedError("the B200 path is inference-only (the reference ships no training code)")
+            raise NotImplementedError("the H100 path is inference-only (the reference ships no training code)")
         return self
 
     def to(self, *args, **kwargs):
         for a in list(args) + list(kwargs.values()):
             if isinstance(a, (str, torch.device)) and torch.device(a).type != "cuda":
-                raise N.NativeError("the B200 path has no CPU fallback: model.to('cpu') is not supported")
+                raise N.NativeError("the H100 path has no CPU fallback: model.to('cpu') is not supported")
         return self
 
     def parameters(self):
@@ -209,7 +209,7 @@ class VisualCLAModel:
         _device_map = kwargs.pop("device_map")          # whole model lives on one GPU (14.5 GB of 180 GB); DP replicates it
         load_in_8bit = kwargs.pop("load_in_8bit")
         if load_in_8bit:
-            raise NotImplementedError("load_in_8bit (bitsandbytes) is out of scope of the B200 path (bf16 weights)")
+            raise NotImplementedError("load_in_8bit (bitsandbytes) is out of scope of the H100 path (bf16 weights)")
         config = VisualCLAConfig.from_pretrained(path)
         text_dir, vision_dir = os.path.join(path, "text_encoder"), os.path.join(path, "vision_encoder")
         with open(os.path.join(text_dir, "config.json")) as f:
@@ -247,7 +247,7 @@ class VisualCLAModel:
         if text_model_name_or_path is None:
             raise ValueError("If `text_model` is not defined as an argument, a `text_model_name_or_path` has to be defined")
         if load_in_8bit:
-            raise NotImplementedError("load_in_8bit is out of scope of the B200 path")
+            raise NotImplementedError("load_in_8bit is out of scope of the H100 path")
         if isinstance(visualcla_config, str):
             visualcla_config = VisualCLAConfig.from_pretrained(visualcla_config)
         config = copy.deepcopy(visualcla_config)
@@ -333,7 +333,7 @@ class VisualCLAModel:
         T = m.shape[1]
         expect = torch.arange(T)[None, :] >= pads[:, None]
         if not torch.equal(m, expect):
-            raise NotImplementedError("only left padding (attention_mask = [0]*p + [1]*(T-p)) is supported on the B200 path")
+            raise NotImplementedError("only left padding (attention_mask = [0]*p + [1]*(T-p)) is supported on the H100 path")
         if bool((pads >= T).any()):
             raise ValueError("attention_mask masks a whole sequence")
         if image_mode == N.IMAGE_AT_HEAD:
@@ -381,7 +381,7 @@ class VisualCLAModel:
         if unused:
             raise ValueError(f"generate(): unsupported arguments {sorted(unused)}")
         if getattr(gc, "num_beams", 1) not in (None, 1) or getattr(gc, "num_return_sequences", 1) not in (None, 1):
-            raise NotImplementedError("beam search / num_return_sequences > 1 are not on the B200 path")
+            raise NotImplementedError("beam search / num_return_sequences > 1 are not on the H100 path")
         return gc
 
     @staticmethod
@@ -396,7 +396,7 @@ class VisualCLAModel:
                  logits_processor=None, stopping_criteria=None, prefix_allowed_tokens_fn=None, synced_gpus=False, **kwargs):
         gc = self._resolve_generation_config(generation_config, kwargs)
         if prefix_allowed_tokens_fn is not None:
-            raise NotImplementedError("prefix_allowed_tokens_fn is not supported on the B200 path")
+            raise NotImplementedError("prefix_allowed_tokens_fn is not supported on the H100 path")
         eng = self._engine
         B = input_ids.shape[0]
         if B > eng.max_batch:
