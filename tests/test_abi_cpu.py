@@ -98,18 +98,34 @@ def test_version_and_error_strings(lib):
     assert isinstance(lib.vcla_last_error(), bytes)
 
 
+def _tiny_config():
+    from visualcla import _native
+    return _native.VclaConfig(v_hidden=128, v_layers=1, v_heads=2, v_ffn=256, v_patch=14, v_image=56, v_eps=1e-5,
+                              r_hidden=128, r_layers=1, r_heads=2, r_ffn=256, r_queries=8, r_eps=1e-12,
+                              t_hidden=256, t_layers=1, t_heads=2, t_ffn=448, t_vocab=100, t_eps=1e-6, rope_theta=1e4,
+                              max_batch=1, max_seq=32, max_prefill_tokens=32, page_tokens=16)
+
+
+@pytest.mark.parametrize("var,value", [("VCLA_DECODE_SCHEDULE", "fix"), ("VCLA_DECODE_SCHEDULE", "unfused"),
+                                       ("VCLA_FUSED_DECODE", "1"), ("VCLA_PREFILL_FUSED", "0")])
+def test_removed_schedule_switches_refused(lib, monkeypatch, var, value):
+    """A switch of a removed schedule makes vcla_create fail (before it looks for a device) and name the switch, so an old A/B
+    script cannot measure the default schedule under the alternative's name."""
+    monkeypatch.setenv(var, value)
+    ctx = C.c_void_p()
+    assert lib.vcla_create(C.byref(_tiny_config()), C.byref(ctx)) != 0
+    err = lib.vcla_last_error()
+    assert var.encode() in err and b"removed" in err
+
+
 def test_no_cpu_fallback(lib):
     """Without a CUDA device the product must fail loudly, never compute on the CPU."""
     import torch
     if torch.cuda.is_available():
         pytest.skip("has a GPU")
     from visualcla import _native
-    cfg = _native.VclaConfig(v_hidden=128, v_layers=1, v_heads=2, v_ffn=256, v_patch=14, v_image=56, v_eps=1e-5,
-                             r_hidden=128, r_layers=1, r_heads=2, r_ffn=256, r_queries=8, r_eps=1e-12,
-                             t_hidden=256, t_layers=1, t_heads=2, t_ffn=448, t_vocab=100, t_eps=1e-6, rope_theta=1e4,
-                             max_batch=1, max_seq=32, max_prefill_tokens=32, page_tokens=16)
     ctx = C.c_void_p()
-    rc = lib.vcla_create(C.byref(cfg), C.byref(ctx))
+    rc = lib.vcla_create(C.byref(_tiny_config()), C.byref(ctx))
     assert rc != 0 and b"no CUDA device" in lib.vcla_last_error()
     import visualcla
     with pytest.raises(_native.NativeError):

@@ -189,20 +189,6 @@ def test_long_context_vs_oracle():
     assert nbad == 0, f"{nbad} decisive tokens differ ({ndec}/{ntot} decisive)"
 
 
-@pytest.mark.parametrize("schedule", ["unfused", "fix"])
-def test_alternative_decode_schedules_match(monkeypatch, schedule):
-    """The default decode schedule is the cluster split-K one (gemm_decode.cu, 5 kernels / layer).  The two older schedules stay
-    selectable for A/B measurements -- "unfused": split-K partials in an L2 workspace + separate consumer kernels (8 / layer);
-    "fix": last-arriver fixup inside the GEMM through global atomics -- and must satisfy the same parity bar.  Likewise the
-    8-kernel prefill schedule (VCLA_PREFILL_FUSED=0) against the default fused-epilogue one."""
-    cfg = O.PathConfig(v_layers=1, r_layers=1, t_hidden=512, t_heads=4, t_ffn=1408, t_layers=3, t_vocab=2003)
-    monkeypatch.setenv("VCLA_DECODE_SCHEDULE", schedule)
-    monkeypatch.setenv("VCLA_PREFILL_FUSED", "0")
-    m, err, nbad, ndec, ntot, _, _ = _run_vs_oracle(cfg, 13, 3, 40, 20, 160)
-    assert err <= LOGIT_TOL, f"teacher-forced logits rel err {err:.3e}"
-    assert nbad == 0, f"{nbad} decisive tokens differ ({ndec}/{ntot} decisive)"
-
-
 def test_persistent_decode_attention(monkeypatch):
     """The warp-specialised persistent decode-attention kernel (used when sequences x heads outnumber the resident CTAs, e.g.
     batch 32 x 32 heads) forced onto a small problem with 5 CTAs, so every CTA walks several (sequence, head) items and the
@@ -361,10 +347,12 @@ def test_prefill_attention_kernels_end_to_end(golden_dir, impl):
         lib.vcla_set_attention_tc(int(os.environ.get("VCLA_ATTN_TC", "1")))
 
 
-@pytest.mark.parametrize("B", [1, 5, 16, 17, 32])
-def test_cluster_splitk_decode_over_batch_sizes(B):
-    """Cluster split-K decode GEMMs: every batch tile (16 / 32 columns), uneven column ownership (batch not a multiple of the
-    cluster size, clusters larger than the batch) and multi-round cluster walks, against the oracle."""
+@pytest.mark.parametrize("B", [1, 5, 16, 17, 32, 33, 64])
+def test_decode_over_batch_sizes(B):
+    """Both decode schedules against the oracle, each chosen by the batch size as in use.  Batches <= 32, cluster split-K
+    decode GEMMs: every batch tile (16 / 32 columns), uneven column ownership (batch not a multiple of the cluster size,
+    clusters larger than the batch) and multi-round cluster walks.  Batches 33..64 (both ends): split-K partials in the L2
+    workspaces with separate consumer kernels."""
     cfg = O.PathConfig(v_layers=1, r_layers=1, t_hidden=1024, t_heads=8, t_ffn=2752, t_layers=2, t_vocab=5003)
     m, err, nbad, ndec, ntot, _, _ = _run_vs_oracle(cfg, 19, B, 24, 8, 128)
     assert err <= LOGIT_TOL, f"teacher-forced logits rel err {err:.3e}"

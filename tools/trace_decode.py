@@ -66,4 +66,4 @@ print("in-situ mean us per kernel kind:", {k: round(sum(v) / len(v), 2) for k, v
 print("per layer (sum of the per-layer kernels):", round(sum(sum(v) / len(v) for k, v in per.items() if len(v) >= 32), 2), "us")
 if out_path:
     json.dump({"B": B, "pdl": pdl, "event_us": e0.elapsed_time(e1) * 1000, "insitu_mean_us": {k: sum(v) / len(v) for k, v in per.items()},
-               "schedule": os.environ.get("VCLA_DECODE_SCHEDULE", "csk"), "events": rows}, open(out_path, "w"))
+               "schedule": "csk" if B <= 32 else "workspace", "events": rows}, open(out_path, "w"))

@@ -310,10 +310,6 @@ __global__ void __launch_bounds__(kDecWarps * 32, kDecStages == 2 ? 3 : 2) attn_
         qv += __ldcg(row + h * HD + d);
         if (owns_new) { kv += __ldcg(row + T + h * HD + d); vv += __ldcg(row + 2 * T + h * HD + d); }
       }
-      if (c.rstd != nullptr) {          // deferred RMSNorm scale of the projection input (a row scalar commutes with the GEMM)
-        const float rs = __ldcg(c.rstd + b);
-        qv *= rs; kv *= rs; vv *= rs;
-      }
       s_q[d] = qv; s_k[d] = kv; s_v[d] = vv;
     }
     __syncthreads();
@@ -573,7 +569,6 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
           v4[0] += t[u][2].x; v4[1] += t[u][2].y; v4[2] += t[u][2].z; v4[3] += t[u][2].w;
         }
       }
-      const float rs = c.rstd ? __ldcg(c.rstd + b) : 1.f;
       const float4 cs4 = *reinterpret_cast<const float4*>(rope_cos + (size_t)L * (HD / 2) + ((4 * lane) & 63));
       const float4 sn4 = *reinterpret_cast<const float4*>(rope_sin + (size_t)L * (HD / 2) + ((4 * lane) & 63));
       const float cs[4] = {cs4.x, cs4.y, cs4.z, cs4.w}, sn[4] = {sn4.x, sn4.y, sn4.z, sn4.w};
@@ -581,7 +576,7 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
       uint32_t kpk[2], vpk[2];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const float qv = q4[j] * rs, kv = k4[j] * rs, vv = v4[j] * rs;
+        const float qv = q4[j], kv = k4[j], vv = v4[j];
         const float qp = __shfl_xor_sync(0xffffffffu, qv, 16), kp = __shfl_xor_sync(0xffffffffu, kv, 16);   // dims d +- 64
         const float sgn = (lane < 16) ? -1.f : 1.f;
         qo[j] = (qv * cs[j] + sgn * qp * sn[j]) * c.scale;

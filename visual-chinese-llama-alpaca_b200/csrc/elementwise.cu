@@ -1,4 +1,4 @@
-// HBM-bound kernels of the VisualCLA path: normalisation, embedding / splice, RoPE + KV-cache append, the decode
+// HBM-bound kernels of the VisualCLA path: normalisation, embedding / splice, the decode
 // consumers of the split-K partial sums, argmax, synthetic-weight generation and checkpoint repacking.
 // All are simple streaming kernels: 128-bit coalesced accesses where layouts allow, fp32 statistics.
 #include "common.cuh"
@@ -245,9 +245,9 @@ int embed_tokens_i32(const int32_t* ids, int B, int D, const bf16* table, int vo
 }
 
 // decode step entry (one CTA per sequence): embedding row -> fp32 residual, bf16 GEMM operand pre-multiplied by the first
-// layer's RMSNorm weight, and the row's deferred scale 1/rms
+// layer's RMSNorm weight, and the row's sum of squares (the consuming GEMM turns it into the deferred scale 1/rms)
 __global__ void dec_embed_kernel(const int32_t* __restrict__ ids, int D, const bf16* __restrict__ table, int vocab, float* __restrict__ resid,
-                                 const float* __restrict__ norm_w, float eps, bf16* __restrict__ xw, float* __restrict__ rstd, float* __restrict__ ssq, int slots) {
+                                 const float* __restrict__ norm_w, bf16* __restrict__ xw, float* __restrict__ ssq, int slots) {
   __shared__ float red[32];
   TraceScope trace(13);
   pdl_launch_dependents();   // dependents may become resident early; they block in their own griddepcontrol.wait
@@ -273,14 +273,13 @@ __global__ void dec_embed_kernel(const int32_t* __restrict__ ids, int D, const b
     for (int j = 0; j < 8; ++j) q += f[j] * f[j];
   }
   q = block_sum(q, red);
-  if (threadIdx.x == 0 && rstd != nullptr) rstd[b] = rsqrtf(q / D + eps);
   // deferred-norm chain head: the row's sum of squares in slot 0, the other slots empty
-  if (ssq != nullptr) for (int i = threadIdx.x; i < slots; i += blockDim.x) ssq[(size_t)b * slots + i] = i == 0 ? q : 0.f;
+  for (int i = threadIdx.x; i < slots; i += blockDim.x) ssq[(size_t)b * slots + i] = i == 0 ? q : 0.f;
 }
-int dec_embed(const int32_t* ids, int B, int D, const bf16* table, int vocab, float* resid, const float* norm_w, float eps, bf16* xw, float* rstd,
+int dec_embed(const int32_t* ids, int B, int D, const bf16* table, int vocab, float* resid, const float* norm_w, bf16* xw,
               float* ssq, int slots, cudaStream_t st) {
   if (D % 8) { set_error("dec_embed: D %% 8 != 0"); return -1; }
-  VCLA_LAUNCH(dec_embed_kernel, dim3(B), dim3(256), 0, st, ids, D, table, vocab, resid, norm_w, eps, xw, rstd, ssq, slots);
+  VCLA_LAUNCH(dec_embed_kernel, dim3(B), dim3(256), 0, st, ids, D, table, vocab, resid, norm_w, xw, ssq, slots);
   return 0;
 }
 
@@ -326,66 +325,6 @@ int rope_fill_tables(int max_pos, int head_dim, float theta, float* cos_dev, flo
   }
   VCLA_CUDA_OK(cudaMemcpy(cos_dev, hc.data(), hc.size() * 4, cudaMemcpyHostToDevice));
   VCLA_CUDA_OK(cudaMemcpy(sin_dev, hs.data(), hs.size() * 4, cudaMemcpyHostToDevice));
-  return 0;
-}
-
-// prefill: rotate q,k in place inside the fused [B*S, 3T] projection buffer; append k,v to the paged cache.
-// One CTA per token; each thread owns 8 consecutive rotary pairs of one head: 128-bit loads/stores throughout.
-__global__ void rope_and_cache_kernel(bf16* __restrict__ qkv, int S, int H, int HD, const float* __restrict__ rc, const float* __restrict__ rs,
-                                      bf16* __restrict__ kv_pages, const int32_t* __restrict__ page_table, int pages_per_seq,
-                                      int page_tokens, const int32_t* __restrict__ left_pad, int pos_from_mask) {
-  TraceScope trace(7);
-  pdl_launch_dependents();   // dependents may become resident early; they block in their own griddepcontrol.wait
-  pdl_wait();
-  trace.dep();
-  const int s = blockIdx.x, b = blockIdx.y;
-  const int T = H * HD, half = HD / 2, groups = half / 8;
-  const int pad = left_pad ? left_pad[b] : 0;
-  if (s < pad) return;                                 // padding row: not rotated, not cached, masked in attention
-  const int cpos = s - pad;                            // index inside the (compact) KV cache
-  const int pos = pos_from_mask ? cpos : s;            // rotary position
-  bf16* row = qkv + ((size_t)b * S + s) * 3 * T;
-  const int page = page_table[(size_t)b * pages_per_seq + cpos / page_tokens];
-  const int slot = cpos % page_tokens;
-  for (int idx = threadIdx.x; idx < H * groups; idx += blockDim.x) {
-    const int h = idx / groups, i = (idx % groups) * 8;
-    float cs[8], sn[8];
-    *reinterpret_cast<float4*>(cs) = *reinterpret_cast<const float4*>(rc + (size_t)pos * half + i);
-    *reinterpret_cast<float4*>(cs + 4) = *reinterpret_cast<const float4*>(rc + (size_t)pos * half + i + 4);
-    *reinterpret_cast<float4*>(sn) = *reinterpret_cast<const float4*>(rs + (size_t)pos * half + i);
-    *reinterpret_cast<float4*>(sn + 4) = *reinterpret_cast<const float4*>(rs + (size_t)pos * half + i + 4);
-    bf16* kd = kv_pages + ((((size_t)page * 2 + 0) * H + h) * page_tokens + slot) * HD;
-    bf16* vd = kv_pages + ((((size_t)page * 2 + 1) * H + h) * page_tokens + slot) * HD;
-#pragma unroll
-    for (int which = 0; which < 2; ++which) {   // 0: q, 1: k
-      bf16* x = row + which * T + h * HD;
-      const uint4 lo = *reinterpret_cast<const uint4*>(x + i), hi = *reinterpret_cast<const uint4*>(x + i + half);
-      const uint32_t lw[4] = {lo.x, lo.y, lo.z, lo.w}, hw[4] = {hi.x, hi.y, hi.z, hi.w};
-      uint32_t ol[4], oh[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 a = unpack_bf16x2(lw[j]), c2 = unpack_bf16x2(hw[j]);
-        ol[j] = pack_bf16x2(a.x * cs[2 * j] - c2.x * sn[2 * j], a.y * cs[2 * j + 1] - c2.y * sn[2 * j + 1]);
-        oh[j] = pack_bf16x2(c2.x * cs[2 * j] + a.x * sn[2 * j], c2.y * cs[2 * j + 1] + a.y * sn[2 * j + 1]);
-      }
-      const uint4 vlo = make_uint4(ol[0], ol[1], ol[2], ol[3]), vhi = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-      *reinterpret_cast<uint4*>(x + i) = vlo;
-      *reinterpret_cast<uint4*>(x + i + half) = vhi;
-      if (which == 1) {
-        *reinterpret_cast<uint4*>(kd + i) = vlo;
-        *reinterpret_cast<uint4*>(kd + i + half) = vhi;
-      }
-    }
-    const bf16* v = row + 2 * T + h * HD;
-    *reinterpret_cast<uint4*>(vd + i) = *reinterpret_cast<const uint4*>(v + i);
-    *reinterpret_cast<uint4*>(vd + i + half) = *reinterpret_cast<const uint4*>(v + i + half);
-  }
-}
-int rope_and_cache(bf16* qkv, int B, int S, int H, int HD, const float* rope_cos, const float* rope_sin, bf16* kv_pages,
-                   const int32_t* page_table, int pages_per_seq, int page_tokens, const int32_t* left_pad, int pos_from_mask, cudaStream_t st) {
-  if (!rope_cos || !rope_sin) { set_error("rope table not initialised"); return -1; }
-  VCLA_LAUNCH(rope_and_cache_kernel, dim3(S, B), dim3(256), 0, st, qkv, S, H, HD, rope_cos, rope_sin,
-              kv_pages, page_table, pages_per_seq, page_tokens, left_pad, pos_from_mask);
   return 0;
 }
 
@@ -477,7 +416,7 @@ int dec_silu_mul(const float* partial, int splits, int ws_rows, int B, int F, bf
 // logits + argmax: stage 1 per (vocab chunk, b) -> candidate ; stage 2 per b
 constexpr int kArgChunks = kArgmaxChunks;
 __global__ void dec_logits_stage1(const float* __restrict__ partial, int splits, int ws_rows, int ldp, int V, float* __restrict__ logits,
-                                  int ld_logits, float* __restrict__ cand_val, int* __restrict__ cand_idx, const float* __restrict__ rstd) {
+                                  int ld_logits, float* __restrict__ cand_val, int* __restrict__ cand_idx) {
   __shared__ float sv[32];
   __shared__ int si[32];
   TraceScope trace(10);
@@ -485,7 +424,6 @@ __global__ void dec_logits_stage1(const float* __restrict__ partial, int splits,
   pdl_wait();
   trace.dep();
   const int b = blockIdx.y, ch = blockIdx.x;
-  const float rs = rstd ? __ldcg(rstd + b) : 1.f;       // deferred RMSNorm scale of the final norm
   const int per = (V + kArgChunks - 1) / kArgChunks;
   const int v0 = ch * per, v1 = min(V, v0 + per);
   float best = -INFINITY;
@@ -493,7 +431,6 @@ __global__ void dec_logits_stage1(const float* __restrict__ partial, int splits,
   for (int v = v0 + threadIdx.x; v < v1; v += blockDim.x) {
     float x = 0.f;
     for (int s = 0; s < splits; ++s) x += __ldcg(partial + ((size_t)s * ws_rows + b) * (size_t)ldp + v);
-    x *= rs;
     if (logits) logits[(size_t)b * ld_logits + v] = x;
     if (x > best) { best = x; bi = v; }   // strided order: smaller index kept on ties via the reduction below
   }
@@ -539,17 +476,17 @@ __global__ void dec_logits_stage2(const float* __restrict__ cand_val, const int*
   }
 }
 int dec_logits_argmax(const float* partial, int splits, int ws_rows, int ldp, int B, int V, float* logits, int ld_logits, int32_t* tok,
-                      int32_t* history, const int32_t* step_idx, const float* rstd, float* cand_val, int32_t* cand_idx, int32_t* dp_send, cudaStream_t st) {
+                      int32_t* history, const int32_t* step_idx, float* cand_val, int32_t* cand_idx, int32_t* dp_send, cudaStream_t st) {
   if (!cand_val || !cand_idx) { set_error("argmax scratch missing"); return -1; }
-  VCLA_LAUNCH(dec_logits_stage1, dim3(kArgChunks, B), dim3(256), 0, st, partial, splits, ws_rows, ldp, V, logits, ld_logits, cand_val, (int*)cand_idx, rstd);
+  VCLA_LAUNCH(dec_logits_stage1, dim3(kArgChunks, B), dim3(256), 0, st, partial, splits, ws_rows, ldp, V, logits, ld_logits, cand_val, (int*)cand_idx);
   VCLA_LAUNCH(dec_logits_stage2, dim3(B), dim3(32), 0, st, (const float*)cand_val, (const int*)cand_idx, tok, history, step_idx, dp_send);
   return 0;
 }
 
-int dec_logits_reduce(const float* partial, int splits, int ws_rows, int ldp, int B, int V, float* logits, int ld_logits, const float* rstd,
+int dec_logits_reduce(const float* partial, int splits, int ws_rows, int ldp, int B, int V, float* logits, int ld_logits,
                       float* cand_val, int32_t* cand_idx, cudaStream_t st) {
   if (!logits || !cand_val || !cand_idx) { set_error("dec_logits_reduce: missing buffers"); return -1; }
-  VCLA_LAUNCH(dec_logits_stage1, dim3(kArgChunks, B), dim3(256), 0, st, partial, splits, ws_rows, ldp, V, logits, ld_logits, cand_val, (int*)cand_idx, rstd);
+  VCLA_LAUNCH(dec_logits_stage1, dim3(kArgChunks, B), dim3(256), 0, st, partial, splits, ws_rows, ldp, V, logits, ld_logits, cand_val, (int*)cand_idx);
   return 0;
 }
 

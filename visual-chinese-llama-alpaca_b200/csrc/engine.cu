@@ -119,21 +119,15 @@ struct vcla_ctx {
   // prefill activations
   float* resid = nullptr; bf16 *xn = nullptr, *qkv = nullptr, *attn = nullptr, *hmid = nullptr;
   float* p_ssq = nullptr;    // [max_prefill_tokens][t_hidden / 64] row statistics of the deferred-RMSNorm prefill schedule
-  int prefill_fused = 1;     // VCLA_PREFILL_FUSED=0: the 8-kernel/layer schedule with separate rmsnorm / rope_and_cache kernels
   // decode activations
   float* d_resid = nullptr; bf16 *d_xn = nullptr, *d_attn = nullptr, *d_h = nullptr;
   float *ws_qkv = nullptr, *ws_o = nullptr, *ws_gu = nullptr, *ws_d = nullptr, *ws_lm = nullptr;
   float* attn_scratch = nullptr; int32_t* attn_counters = nullptr;
   int32_t* d_tok = nullptr;
   int32_t *tok_hist = nullptr, *step_idx = nullptr;
-  float *d_rstd = nullptr, *d_ssq = nullptr; int32_t *cnt_o = nullptr, *cnt_gu = nullptr, *cnt_d = nullptr;   // fused split-K consumers (decode)
-  // decode schedule: 2 (default, batch <= 32) = cluster split-K GEMMs with fused consumers, 5 kernels / layer (gemm_decode.cu);
-  // 0 = split-K partials in an L2 workspace + separate consumer kernels, 8 kernels / layer; 1 = VCLA_FUSED_DECODE (below).
-  int decode_schedule = 2;
+  float* d_ssq = nullptr;    // [64][t_hidden / 128] row statistics of the deferred-RMSNorm decode schedule (cluster split-K)
   int csk_qkv = 0, csk_o = 0, csk_gu = 0, csk_d = 0, csk_lm = 0;   // CTAs per cluster (= K splits), chosen per batch on first use
   int csk_batch = 0;
-  int fused_decode = 0;   // VCLA_FUSED_DECODE=1: 5-kernel/layer schedule with in-GEMM split-K fixup (parity-tested; the fence->atomic->reload
-                          // chain per tile is serial latency, so the cluster split-K schedule is the default)
   int sp_qkv = 1, sp_o = 1, sp_gu = 1, sp_d = 1, sp_lm = 1, kv_splits = 1;
   int l2_prefetch_kb = 0;    // decode GEMMs: weight k-blocks per CTA prefetched into L2 during the dependency wait (VCLA_L2_PREFETCH_KB).
                              // Off by default: the prefetch traffic can delay the latency-critical consumer kernel in front of the GEMM.
@@ -319,11 +313,7 @@ void layout_activations(vcla_ctx* c) {
   c->d_tok = a_alloc<int32_t>(c, Bp);
   c->tok_hist = a_alloc<int32_t>(c, (size_t)(g.max_seq + 2) * Bp);
   c->step_idx = a_alloc<int32_t>(c, 16);
-  c->d_rstd = a_alloc<float>(c, Bp);
   c->d_ssq = a_alloc<float>(c, Bp * ((T + 127) / 128));
-  c->cnt_o = a_alloc<int32_t>(c, (T + 127) / 128 + 1);
-  c->cnt_d = a_alloc<int32_t>(c, (T + 127) / 128 + 1);
-  c->cnt_gu = a_alloc<int32_t>(c, (2 * F + 127) / 128 + 1);
   c->page_table = a_alloc<int32_t>(c, (size_t)g.max_batch * c->pages_per_seq);
   c->seq_len = a_alloc<int32_t>(c, g.max_batch);
   c->img_row_default = a_alloc<int32_t>(c, g.max_batch);
@@ -368,6 +358,28 @@ int pick_splits(int n_out, int K) {
 }
 
 int count(vcla_ctx* c, int n = 1) { c->launches += n; return 0; }
+
+// Destroys every captured decode graph, so the next decode call captures one with the current settings.
+int drop_graphs(vcla_ctx* c) {
+  if (c->graphs.empty()) return 0;
+  const cudaError_t e = cudaDeviceSynchronize();   // a launch of one of them may still be in flight
+  for (auto& kv : c->graphs) cudaGraphExecDestroy(kv.second);
+  c->graphs.clear(); c->graph_launches.clear(); c->graph_lru.clear();
+  if (e != cudaSuccess) { set_error("drop_graphs: device error %s", cudaGetErrorString(e)); return -1; }
+  return 0;
+}
+
+// Points the in-kernel timeline of every kernel family at buf (nullptr: tracing off).
+int trace_set_all(void* buf, unsigned long long cap) {
+  int rc = 0;
+  rc |= trace_set_gemm(buf, cap);
+  rc |= trace_set_attention_tc(buf, cap);
+  rc |= trace_set_gemm_decode(buf, cap);
+  rc |= trace_set_sampler(buf, cap);
+  rc |= trace_set_attention(buf, cap);
+  rc |= trace_set_elementwise(buf, cap);
+  return rc;
+}
 
 }  // namespace
 
@@ -417,6 +429,16 @@ void vcla_set_pdl(int on) { set_pdl(on != 0); }
 
 int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   if (!cfg || !out) { set_error("vcla_create: null argument"); return -1; }
+  // Switches of removed schedules: refuse them, or a stale A/B script would measure the default and report it as the alternative.
+  for (const char* v : {"VCLA_DECODE_SCHEDULE", "VCLA_FUSED_DECODE"}) {
+    if (getenv(v)) {
+      set_error("vcla_create: %s is set, but the decode schedules it selected were removed (the batch size picks the schedule)", v);
+      return -1;
+    }
+  }
+  if (const char* e = getenv("VCLA_PREFILL_FUSED")) {
+    if (atoi(e) == 0) { set_error("vcla_create: VCLA_PREFILL_FUSED=0 is set, but the 8-kernel prefill schedule was removed"); return -1; }
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     set_error("vcla_create: no CUDA device (this library has no CPU fallback)");
@@ -449,11 +471,6 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   c->sp_d = pick_splits(g.t_hidden, g.t_ffn);
   c->sp_lm = pick_splits(g.t_vocab, g.t_hidden);
   if (const char* e = getenv("VCLA_L2_PREFETCH_KB")) c->l2_prefetch_kb = atoi(e);
-  if (const char* e = getenv("VCLA_FUSED_DECODE")) c->fused_decode = atoi(e);
-  if (const char* e = getenv("VCLA_PREFILL_FUSED")) c->prefill_fused = atoi(e);
-  if (const char* e = getenv("VCLA_DECODE_SCHEDULE")) c->decode_schedule = !strcmp(e, "unfused") ? 0 : (!strcmp(e, "fix") ? 1 : 2);
-  if (c->fused_decode) c->decode_schedule = 1;
-  c->fused_decode = c->decode_schedule == 1;
   c->kv_splits = g.max_seq >= 1536 ? 4 : (g.max_seq >= 768 ? 2 : 1);   // context-driven minimum; raised per call for small batches
   if (const char* e = getenv("VCLA_KV_SPLITS")) { const int v = atoi(e); if (v >= 1 && v <= 8) c->kv_splits = v; }   // tuning override
 
@@ -492,19 +509,18 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
 
 void vcla_destroy(vcla_ctx* c) {
   if (!c) return;
-  for (auto& kv : c->graphs) cudaGraphExecDestroy(kv.second);
+  drop_graphs(c);
   if (c->w_arena) cudaFree(c->w_arena);
   if (c->a_arena) cudaFree(c->a_arena);
   if (c->kv_arena) cudaFree(c->kv_arena);
   if (c->staging) cudaFree(c->staging);
-  c->graphs.clear();
   if (c->comm) { cudaDeviceSynchronize(); g_nccl.CommDestroy(c->comm); c->comm = nullptr; }
   if (c->dp_send) cudaFree(c->dp_send);
   if (c->dp_stream) cudaStreamDestroy(c->dp_stream);
   if (c->dp_fork) cudaEventDestroy(c->dp_fork);
   if (c->dp_join) cudaEventDestroy(c->dp_join);
   if (c->cap_stream) cudaStreamDestroy(c->cap_stream);
-  if (c->trace_buf) { trace_set_gemm(nullptr, 0); trace_set_attention_tc(nullptr, 0); trace_set_gemm_decode(nullptr, 0); trace_set_sampler(nullptr, 0); trace_set_attention(nullptr, 0); trace_set_elementwise(nullptr, 0); cudaFree(c->trace_buf); }
+  if (c->trace_buf) { trace_set_all(nullptr, 0); cudaFree(c->trace_buf); }
   delete c;
 }
 
@@ -733,13 +749,68 @@ int vcla_vision_encode(vcla_ctx* c, const void* pixels, int pixel_dtype, int B, 
 }
 
 // -------------------------------------------------------------------------------------------------
-// prefill
+// decode launches (the prefill's last-position lm_head uses the workspace one too)
 // -------------------------------------------------------------------------------------------------
-static int swap_gemm(vcla_ctx* c, const bf16* W, int n_out, int K, const bf16* X, int B, int splits, float* ws, cudaStream_t st, const GemmFix* fix = nullptr) {
-  GemmCall g; g.A = W; g.B = X; g.M = n_out; g.N = B; g.K = K; g.lda = K; g.ldb = K; g.mode = GEMM_PARTIAL_F32; g.out = ws; g.ldo = n_out;
-  g.splits = splits; g.ws_rows = B; g.weights_are_A = 1; g.l2_prefetch_kb = c->l2_prefetch_kb;
-  if (fix) g.fix = *fix;
-  count(c); return gemm_tc(g, st);
+// The batch size alone picks the decode schedule: up to 32 rows the cluster split-K GEMMs with fused consumers (5 kernels
+// per layer); 33..64 rows split-K partials in an L2 workspace reduced by separate consumer kernels (8 kernels per layer).
+static bool decode_uses_csk(int B) { return B <= 32; }
+
+// The five weight-streaming GEMMs of a decode step (numbering of vcla_bench_decode_gemm's `which`).
+enum DecodeGemm { DG_QKV = 0, DG_O = 1, DG_GATE_UP = 2, DG_DOWN = 3, DG_LM_HEAD = 4 };
+
+// GEMM `which` of decode layer i (i is ignored for the lm_head) on the workspace schedule: swap-AB split-K partials of
+// the d_xn / d_attn / d_h rows into that GEMM's fp32 L2 workspace, reduced by the next consumer kernel.
+static int ws_gemm(vcla_ctx* c, int which, int i, int B, cudaStream_t st) {
+  const vcla_config& g = c->cfg;
+  const int TH = g.t_hidden, F = g.t_ffn;
+  const TextLayer* L = which == DG_LM_HEAD ? nullptr : &c->tl[i];
+  GemmCall gc; gc.N = B; gc.mode = GEMM_PARTIAL_F32; gc.ws_rows = B; gc.weights_are_A = 1; gc.l2_prefetch_kb = c->l2_prefetch_kb;
+  switch (which) {
+    case DG_QKV: gc.A = L->wqkv; gc.B = c->d_xn; gc.M = 3 * TH; gc.K = TH; gc.splits = c->sp_qkv; gc.out = c->ws_qkv; break;
+    case DG_O: gc.A = L->wo; gc.B = c->d_attn; gc.M = TH; gc.K = TH; gc.splits = c->sp_o; gc.out = c->ws_o; break;
+    case DG_GATE_UP: gc.A = L->wgu; gc.B = c->d_xn; gc.M = 2 * F; gc.K = TH; gc.splits = c->sp_gu; gc.out = c->ws_gu; break;
+    case DG_DOWN: gc.A = L->wd; gc.B = c->d_h; gc.M = TH; gc.K = F; gc.splits = c->sp_d; gc.out = c->ws_d; break;
+    default: gc.A = c->lm_head; gc.B = c->d_xn; gc.M = g.t_vocab; gc.K = TH; gc.splits = c->sp_lm; gc.out = c->ws_lm; break;
+  }
+  gc.lda = gc.ldb = gc.K; gc.ldo = gc.M;
+  count(c); return gemm_tc(gc, st);
+}
+
+// GEMM `which` of decode layer i on the cluster split-K schedule (gemm_decode.cu): the split-K reduction and the consumer run
+// inside the GEMM, with RMSNorm's row scale deferred to the next GEMM through the per-row sums of squares in d_ssq.
+static int csk_gemm(vcla_ctx* c, int which, int i, int B, cudaStream_t st) {
+  const vcla_config& g = c->cfg;
+  const int TH = g.t_hidden, F = g.t_ffn;
+  const TextLayer* L = which == DG_LM_HEAD ? nullptr : &c->tl[i];
+  CskCall k; k.B = B; k.inv_dim = 1.0f / (float)TH; k.eps = g.t_eps;
+  switch (which) {
+    case DG_QKV: k.W = L->wqkv; k.X = c->d_xn; k.M = 3 * TH; k.K = TH; k.splits = c->csk_qkv; k.mode = CSK_OUT_F32; k.out = c->ws_qkv; break;
+    case DG_O: k.W = L->wo; k.X = c->d_attn; k.M = TH; k.K = TH; k.splits = c->csk_o; k.mode = CSK_RESID; k.norm_w = L->ln2; break;
+    case DG_GATE_UP: k.W = L->wgu; k.X = c->d_xn; k.M = 2 * F; k.K = TH; k.splits = c->csk_gu; k.mode = CSK_SWIGLU; k.h = c->d_h; break;
+    case DG_DOWN: k.W = L->wd; k.X = c->d_h; k.M = TH; k.K = F; k.splits = c->csk_d; k.mode = CSK_RESID;
+      k.norm_w = (i + 1 < g.t_layers) ? c->tl[i + 1].ln1 : c->final_norm; break;
+    default: k.W = c->lm_head; k.X = c->d_xn; k.M = g.t_vocab; k.K = TH; k.splits = c->csk_lm; k.mode = CSK_OUT_F32; k.out = c->ws_lm; break;
+  }
+  if (k.mode == CSK_OUT_F32) k.ldo = k.M;
+  if (k.mode == CSK_RESID) {
+    k.resid = c->d_resid; k.xw = c->d_xn; k.ssq_out = c->d_ssq;
+  } else {
+    k.ssq_in = c->d_ssq; k.ssq_slots = (TH + 127) / 128;   // one slot per 128-row tile of the o / down projections
+  }
+  count(c); return gemm_csk(k, st);
+}
+
+// Decode attention of layer L over the paged KV cache, reading the fused QKV projection from ws_qkv (qkv_splits partials).
+static DecodeAttnCall decode_attn_call(const vcla_ctx* c, const TextLayer& L, int B, int qkv_splits) {
+  const vcla_config& g = c->cfg;
+  DecodeAttnCall a; a.qkv_partial = c->ws_qkv; a.splits = qkv_splits; a.ws_rows = B; a.kv_pages = L.kv; a.page_table = c->page_table;
+  a.pages_per_seq = c->pages_per_seq; a.page_tokens = c->page_tokens; a.seq_len = c->seq_len; a.out = c->d_attn; a.scratch = c->attn_scratch;
+  a.counters = c->attn_counters; a.B = B; a.H = g.t_heads; a.HD = 128; a.scale = 1.0f / sqrtf(128.f); a.rope_theta = g.rope_theta;
+  a.rope_cos = c->rope_cos; a.rope_sin = c->rope_sin; a.persistent_mode = c->attn_persistent_mode; a.persistent_grid = c->attn_persistent_grid;
+  // enough CTAs to cover the SMs for small batches; long contexts split so a CTA streams <= ~12 pages
+  const int want = (num_sms() + B * a.H - 1) / (B * a.H);
+  a.kv_splits = std::min(8, std::max(want, c->kv_splits));
+  return a;
 }
 
 // ---- data parallel token exchange -------------------------------------------------------------------------------
@@ -765,7 +836,7 @@ static int dp_wait(vcla_ctx* c, cudaStream_t st) {
 }
 
 // logits reduce + argmax (+ token exchange when data parallel)
-static int logits_argmax(vcla_ctx* c, int B, float* logits, int32_t* tok, const float* rstd, int fork, cudaStream_t st, int lm_splits = 0) {
+static int logits_argmax(vcla_ctx* c, int B, float* logits, int32_t* tok, int fork, cudaStream_t st, int lm_splits = 0) {
   const vcla_config& g = c->cfg;
   const int sp_lm = lm_splits > 0 ? lm_splits : c->sp_lm;     // 1: ws_lm already holds the reduced logits (cluster split-K lm_head)
   if (c->dp_on() && dp_wait(c, st)) return -1;            // the previous step's exchange must have read dp_send before it is rewritten
@@ -773,14 +844,14 @@ static int logits_argmax(vcla_ctx* c, int B, float* logits, int32_t* tok, const 
     // logits -> [repetition penalty, no-repeat-ngram, temperature, top-k, top-p, draw] in one kernel; raw logits stay available
     float* lg = logits ? logits : c->samp_logits;
     count(c, 2);
-    if (dec_logits_reduce(c->ws_lm, sp_lm, B, g.t_vocab, B, g.t_vocab, lg, g.t_vocab, rstd, c->cand_val, c->cand_idx, st)) return -1;
+    if (dec_logits_reduce(c->ws_lm, sp_lm, B, g.t_vocab, B, g.t_vocab, lg, g.t_vocab, c->cand_val, c->cand_idx, st)) return -1;
     if (dec_sample(lg, g.t_vocab, g.t_vocab, B, c->tok_hist, c->step_idx, c->samp_params, tok, c->tok_hist, c->dp_on() ? c->dp_send : nullptr, c->finished,
                    nullptr, st)) return -1;
     if (c->dp_on()) return dp_gather(c, st, fork);
     return 0;
   }
   count(c, 2);
-  if (dec_logits_argmax(c->ws_lm, sp_lm, B, g.t_vocab, B, g.t_vocab, logits, g.t_vocab, tok, c->tok_hist, c->step_idx, rstd, c->cand_val, c->cand_idx,
+  if (dec_logits_argmax(c->ws_lm, sp_lm, B, g.t_vocab, B, g.t_vocab, logits, g.t_vocab, tok, c->tok_hist, c->step_idx, c->cand_val, c->cand_idx,
                         c->dp_on() ? c->dp_send : nullptr, st)) return -1;
   if (c->dp_on()) return dp_gather(c, st, fork);
   return 0;
@@ -790,8 +861,8 @@ static int lm_head_last(vcla_ctx* c, int B, float* logits_dev, int32_t* tok_dev,
   // d_resid[B, T] holds the hidden state of the positions to score
   const vcla_config& g = c->cfg;
   count(c); if (dec_resid_norm(nullptr, 0, B, c->d_resid, B, g.t_hidden, c->final_norm, g.t_eps, c->d_xn, st)) return -1;
-  if (swap_gemm(c, c->lm_head, g.t_vocab, g.t_hidden, c->d_xn, B, c->sp_lm, c->ws_lm, st)) return -1;
-  return logits_argmax(c, B, logits_dev, tok_dev ? tok_dev : c->d_tok, nullptr, 0, st);
+  if (ws_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
+  return logits_argmax(c, B, logits_dev, tok_dev ? tok_dev : c->d_tok, 0, st);
 }
 
 int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, const int32_t* img_row, const int32_t* left_pad,
@@ -815,57 +886,39 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
     count(c); if (scatter_image_rows(c->img_embeds, B, nq, TH, rs, S, c->resid, st)) return -1;
   }
   const float scale = 1.0f / sqrtf(128.f);
-  if (c->prefill_fused) {
-    // 5 kernels per layer: RMSNorm is deferred (operand = bf16(resid * norm_w); the row scale commutes with the GEMM and is applied in
-    // the consuming GEMM's epilogue from the per-tile sums of squares the producing GEMM wrote), RoPE + KV-cache append run in the
-    // QKV GEMM's epilogue on the fp32 accumulator, SwiGLU in the gate/up epilogue, the residual add in the O / down epilogues.
-    const int slots = (TH + gemm_pick_bn(rows, TH) - 1) / gemm_pick_bn(rows, TH);
-    GemmRowScale rsc; rsc.ssq = c->p_ssq; rsc.slots = slots; rsc.inv_dim = 1.0f / (float)TH; rsc.eps = g.t_eps;
-    count(c); if (prenorm_rows(c->resid, rows, TH, c->tl[0].ln1, c->xn, c->p_ssq, slots, st)) return -1;
-    for (int i = 0; i < g.t_layers; ++i) {
-      const TextLayer& L = c->tl[i];
-      {
-        GemmCall gc; gc.A = c->xn; gc.B = L.wqkv; gc.M = rows; gc.N = 3 * TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_STORE_BF16; gc.out = c->qkv; gc.ldo = 3 * TH;
-        gc.rowscale = rsc;
-        gc.rope.cos = c->rope_cos; gc.rope.sin = c->rope_sin; gc.rope.kv_pages = L.kv; gc.rope.page_table = c->page_table; gc.rope.pages_per_seq = c->pages_per_seq;
-        gc.rope.page_tokens = c->page_tokens; gc.rope.S = S; gc.rope.T = TH; gc.rope.H = H; gc.rope.left_pad = left_pad; gc.rope.pos_from_mask = pos_from_mask;
-        count(c); if (gemm_tc(gc, st)) return -1;
-      }
-      AttnCall a; a.q = c->qkv; a.q_stride = 3 * TH; a.k0 = c->qkv + TH; a.v0 = c->qkv + 2 * TH; a.kv0_stride = 3 * TH; a.n0 = S;
-      a.out = c->attn; a.o_stride = TH; a.B = B; a.H = H; a.Sq = S; a.HD = 128; a.scale = scale; a.causal = 1; a.kv_start = left_pad;
-      count(c); if (attention_prefill(a, st)) return -1;
-      {
-        GemmCall gc; gc.A = c->attn; gc.B = L.wo; gc.M = rows; gc.N = TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_ADD_F32; gc.accumulate = 1; gc.out = c->resid; gc.ldo = TH;
-        gc.emit.norm_w = L.ln2; gc.emit.xw = c->xn; gc.emit.ldxw = TH; gc.emit.ssq_out = c->p_ssq;
-        count(c); if (gemm_tc(gc, st)) return -1;
-      }
-      {
-        GemmCall gc; gc.A = c->xn; gc.B = L.wgu; gc.M = rows; gc.N = 2 * F; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_SWIGLU_BF16; gc.out = c->hmid; gc.ldo = F;
-        gc.rowscale = rsc;
-        count(c); if (gemm_tc(gc, st)) return -1;
-      }
-      {
-        GemmCall gc; gc.A = c->hmid; gc.B = L.wd; gc.M = rows; gc.N = TH; gc.K = F; gc.lda = F; gc.ldb = F; gc.mode = GEMM_ADD_F32; gc.accumulate = 1; gc.out = c->resid; gc.ldo = TH;
-        gc.emit.norm_w = (i + 1 < g.t_layers) ? c->tl[i + 1].ln1 : c->final_norm; gc.emit.xw = c->xn; gc.emit.ldxw = TH; gc.emit.ssq_out = c->p_ssq;
-        count(c); if (gemm_tc(gc, st)) return -1;
-      }
-    }
-  } else
+  // 5 kernels per layer: RMSNorm is deferred (operand = bf16(resid * norm_w); the row scale commutes with the GEMM and is applied in
+  // the consuming GEMM's epilogue from the per-tile sums of squares the producing GEMM wrote), RoPE + KV-cache append run in the
+  // QKV GEMM's epilogue on the fp32 accumulator, SwiGLU in the gate/up epilogue, the residual add in the O / down epilogues.
+  const int slots = (TH + gemm_pick_bn(rows, TH) - 1) / gemm_pick_bn(rows, TH);
+  GemmRowScale rsc; rsc.ssq = c->p_ssq; rsc.slots = slots; rsc.inv_dim = 1.0f / (float)TH; rsc.eps = g.t_eps;
+  count(c); if (prenorm_rows(c->resid, rows, TH, c->tl[0].ln1, c->xn, c->p_ssq, slots, st)) return -1;
   for (int i = 0; i < g.t_layers; ++i) {
     const TextLayer& L = c->tl[i];
-    count(c); if (rmsnorm(c->resid, rows, TH, L.ln1, g.t_eps, c->xn, st)) return -1;
-    if (gemm_bf16(c, c->xn, rows, TH, TH, L.wqkv, 3 * TH, TH, nullptr, ACT_NONE, c->qkv, 3 * TH, st)) return -1;
-    count(c); if (rope_and_cache(c->qkv, B, S, H, 128, c->rope_cos, c->rope_sin, L.kv, c->page_table, c->pages_per_seq, c->page_tokens, left_pad, pos_from_mask, st)) return -1;
+    {
+      GemmCall gc; gc.A = c->xn; gc.B = L.wqkv; gc.M = rows; gc.N = 3 * TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_STORE_BF16; gc.out = c->qkv; gc.ldo = 3 * TH;
+      gc.rowscale = rsc;
+      gc.rope.cos = c->rope_cos; gc.rope.sin = c->rope_sin; gc.rope.kv_pages = L.kv; gc.rope.page_table = c->page_table; gc.rope.pages_per_seq = c->pages_per_seq;
+      gc.rope.page_tokens = c->page_tokens; gc.rope.S = S; gc.rope.T = TH; gc.rope.H = H; gc.rope.left_pad = left_pad; gc.rope.pos_from_mask = pos_from_mask;
+      count(c); if (gemm_tc(gc, st)) return -1;
+    }
     AttnCall a; a.q = c->qkv; a.q_stride = 3 * TH; a.k0 = c->qkv + TH; a.v0 = c->qkv + 2 * TH; a.kv0_stride = 3 * TH; a.n0 = S;
     a.out = c->attn; a.o_stride = TH; a.B = B; a.H = H; a.Sq = S; a.HD = 128; a.scale = scale; a.causal = 1; a.kv_start = left_pad;
     count(c); if (attention_prefill(a, st)) return -1;
-    if (gemm_f32(c, c->attn, rows, TH, TH, L.wo, TH, TH, nullptr, 1, c->resid, TH, st)) return -1;
-    count(c); if (rmsnorm(c->resid, rows, TH, L.ln2, g.t_eps, c->xn, st)) return -1;
     {
-      GemmCall gc; gc.A = c->xn; gc.B = L.wgu; gc.M = rows; gc.N = 2 * F; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_SWIGLU_BF16; gc.out = c->hmid; gc.ldo = F;
+      GemmCall gc; gc.A = c->attn; gc.B = L.wo; gc.M = rows; gc.N = TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_ADD_F32; gc.accumulate = 1; gc.out = c->resid; gc.ldo = TH;
+      gc.emit.norm_w = L.ln2; gc.emit.xw = c->xn; gc.emit.ldxw = TH; gc.emit.ssq_out = c->p_ssq;
       count(c); if (gemm_tc(gc, st)) return -1;
     }
-    if (gemm_f32(c, c->hmid, rows, F, F, L.wd, TH, F, nullptr, 1, c->resid, TH, st)) return -1;
+    {
+      GemmCall gc; gc.A = c->xn; gc.B = L.wgu; gc.M = rows; gc.N = 2 * F; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_SWIGLU_BF16; gc.out = c->hmid; gc.ldo = F;
+      gc.rowscale = rsc;
+      count(c); if (gemm_tc(gc, st)) return -1;
+    }
+    {
+      GemmCall gc; gc.A = c->hmid; gc.B = L.wd; gc.M = rows; gc.N = TH; gc.K = F; gc.lda = F; gc.ldb = F; gc.mode = GEMM_ADD_F32; gc.accumulate = 1; gc.out = c->resid; gc.ldo = TH;
+      gc.emit.norm_w = (i + 1 < g.t_layers) ? c->tl[i + 1].ln1 : c->final_norm; gc.emit.xw = c->xn; gc.emit.ldxw = TH; gc.emit.ssq_out = c->p_ssq;
+      count(c); if (gemm_tc(gc, st)) return -1;
+    }
   }
   if (logits_all) {
     count(c); if (rmsnorm(c->resid, rows, TH, c->final_norm, g.t_eps, c->xn, st)) return -1;
@@ -886,36 +939,30 @@ static int advance_and_reserve(vcla_ctx* c, int B, cudaStream_t st) {
 // -------------------------------------------------------------------------------------------------
 // decode
 // -------------------------------------------------------------------------------------------------
-// Legacy schedule (8 kernels per layer: separate norm / silu consumers).  Kept for A/B measurements (VCLA_FUSED_DECODE=0).
-static int decode_enqueue_unfused(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, cudaStream_t st) {
+// ---- workspace schedule (batches 33..64): 8 kernels per layer, split-K partials in L2 workspaces + separate consumer kernels ----
+static int decode_enqueue_workspace(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, cudaStream_t st) {
   const vcla_config& g = c->cfg;
-  const int TH = g.t_hidden, F = g.t_ffn, H = g.t_heads;
+  const int TH = g.t_hidden, F = g.t_ffn;
   count(c); if (embed_tokens_i32(tok_in, B, TH, c->embed, g.t_vocab, c->d_resid, st)) return -1;
-  const float scale = 1.0f / sqrtf(128.f);
   for (int i = 0; i < g.t_layers; ++i) {
     const TextLayer& L = c->tl[i];
     count(c); if (dec_resid_norm(i == 0 ? nullptr : c->ws_d, c->sp_d, B, c->d_resid, B, TH, L.ln1, g.t_eps, c->d_xn, st)) return -1;
-    if (swap_gemm(c, L.wqkv, 3 * TH, TH, c->d_xn, B, c->sp_qkv, c->ws_qkv, st)) return -1;
-    DecodeAttnCall a; a.qkv_partial = c->ws_qkv; a.splits = c->sp_qkv; a.ws_rows = B; a.kv_pages = L.kv; a.page_table = c->page_table;
-    a.pages_per_seq = c->pages_per_seq; a.page_tokens = c->page_tokens; a.seq_len = c->seq_len; a.out = c->d_attn; a.scratch = c->attn_scratch;
-    a.counters = c->attn_counters; a.B = B; a.H = H; a.HD = 128; a.scale = scale; a.rope_theta = g.rope_theta;
-    a.rope_cos = c->rope_cos; a.rope_sin = c->rope_sin; a.persistent_mode = c->attn_persistent_mode; a.persistent_grid = c->attn_persistent_grid;
-    { int want = (num_sms() + B * H - 1) / (B * H); int ks = want > c->kv_splits ? want : c->kv_splits; a.kv_splits = ks > 8 ? 8 : ks; }
-    count(c); if (attention_decode(a, st)) return -1;
-    if (swap_gemm(c, L.wo, TH, TH, c->d_attn, B, c->sp_o, c->ws_o, st)) return -1;
+    if (ws_gemm(c, DG_QKV, i, B, st)) return -1;
+    count(c); if (attention_decode(decode_attn_call(c, L, B, c->sp_qkv), st)) return -1;
+    if (ws_gemm(c, DG_O, i, B, st)) return -1;
     count(c); if (dec_resid_norm(c->ws_o, c->sp_o, B, c->d_resid, B, TH, L.ln2, g.t_eps, c->d_xn, st)) return -1;
-    if (swap_gemm(c, L.wgu, 2 * F, TH, c->d_xn, B, c->sp_gu, c->ws_gu, st)) return -1;
+    if (ws_gemm(c, DG_GATE_UP, i, B, st)) return -1;
     count(c); if (dec_silu_mul(c->ws_gu, c->sp_gu, B, B, F, c->d_h, st)) return -1;
-    if (swap_gemm(c, L.wd, TH, F, c->d_h, B, c->sp_d, c->ws_d, st)) return -1;
+    if (ws_gemm(c, DG_DOWN, i, B, st)) return -1;
   }
   count(c); if (dec_resid_norm(c->ws_d, c->sp_d, B, c->d_resid, B, TH, c->final_norm, g.t_eps, c->d_xn, st)) return -1;
-  if (swap_gemm(c, c->lm_head, g.t_vocab, TH, c->d_xn, B, c->sp_lm, c->ws_lm, st)) return -1;
-  if (logits_argmax(c, B, logits, tok_out, nullptr, 1, st)) return -1;
+  if (ws_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
+  if (logits_argmax(c, B, logits, tok_out, 1, st)) return -1;
   count(c); if (advance_and_reserve(c, B, st)) return -1;
   return 0;
 }
 
-// ---- cluster split-K schedule (default for batch <= 32): 5 kernels per layer, no split-K workspace, no consumer kernels ----------
+// ---- cluster split-K schedule (batches <= 32): 5 kernels per layer, no split-K workspace, no consumer kernels ----------
 // CTAs per cluster for a [M, K] weight at batch B: the choice that keeps the largest share of the 2 x SMs CTA slots busy over whole
 // rounds of cluster-tiles (clusters are gang-scheduled: floor(slots / S) of them are resident).
 static int csk_pick(int M, int K, int B) {
@@ -950,76 +997,26 @@ static int csk_prepare(vcla_ctx* c, int B) {
   return 0;
 }
 
+// Decode step, 5 kernels per layer:  QKV GEMM [rstd] -> attention(+RoPE, append) -> O GEMM [+residual, norm weight, sum sq]
+//   -> gate/up GEMM [rstd, SiLU*mul] -> down GEMM [+residual, next norm weight, sum sq].  The bracketed consumers run inside the
+// GEMM after the cluster's split-K reduction; RMSNorm's per-row scale rstd is deferred to the consuming GEMM.
 static int decode_enqueue_csk(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, cudaStream_t st) {
   const vcla_config& g = c->cfg;
-  const int TH = g.t_hidden, F = g.t_ffn, H = g.t_heads;
-  const int slots = (TH + 127) / 128;                            // per-row sum-of-squares slots = 128-row tiles of the o / down projections
-  const float inv_dim = 1.0f / (float)TH;
-  count(c); if (dec_embed(tok_in, B, TH, c->embed, g.t_vocab, c->d_resid, c->tl[0].ln1, g.t_eps, c->d_xn, nullptr, c->d_ssq, slots, st)) return -1;
-  const float scale = 1.0f / sqrtf(128.f);
-  auto base = [&](const bf16* W, const bf16* X, int M, int K, int splits, int mode) {
-    CskCall k; k.W = W; k.X = X; k.M = M; k.B = B; k.K = K; k.splits = splits; k.mode = mode; k.inv_dim = inv_dim; k.eps = g.t_eps;
-    return k;
-  };
+  const int TH = g.t_hidden;
+  count(c); if (dec_embed(tok_in, B, TH, c->embed, g.t_vocab, c->d_resid, c->tl[0].ln1, c->d_xn, c->d_ssq, (TH + 127) / 128, st)) return -1;
   for (int i = 0; i < g.t_layers; ++i) {
-    const TextLayer& L = c->tl[i];
-    { CskCall k = base(L.wqkv, c->d_xn, 3 * TH, TH, c->csk_qkv, CSK_OUT_F32); k.out = c->ws_qkv; k.ldo = 3 * TH; k.ssq_in = c->d_ssq; k.ssq_slots = slots;
-      count(c); if (gemm_csk(k, st)) return -1; }
-    DecodeAttnCall a; a.qkv_partial = c->ws_qkv; a.splits = 1; a.ws_rows = B; a.kv_pages = L.kv; a.page_table = c->page_table;
-    a.pages_per_seq = c->pages_per_seq; a.page_tokens = c->page_tokens; a.seq_len = c->seq_len; a.out = c->d_attn; a.scratch = c->attn_scratch;
-    a.counters = c->attn_counters; a.B = B; a.H = H; a.HD = 128; a.scale = scale; a.rope_theta = g.rope_theta;
-    a.rope_cos = c->rope_cos; a.rope_sin = c->rope_sin; a.persistent_mode = c->attn_persistent_mode; a.persistent_grid = c->attn_persistent_grid;
-    { int want = (num_sms() + B * H - 1) / (B * H); int ks = want > c->kv_splits ? want : c->kv_splits; a.kv_splits = ks > 8 ? 8 : ks; }
-    count(c); if (attention_decode(a, st)) return -1;
-    { CskCall k = base(L.wo, c->d_attn, TH, TH, c->csk_o, CSK_RESID); k.resid = c->d_resid; k.norm_w = L.ln2; k.xw = c->d_xn; k.ssq_out = c->d_ssq;
-      count(c); if (gemm_csk(k, st)) return -1; }
-    { CskCall k = base(L.wgu, c->d_xn, 2 * F, TH, c->csk_gu, CSK_SWIGLU); k.h = c->d_h; k.ssq_in = c->d_ssq; k.ssq_slots = slots;
-      count(c); if (gemm_csk(k, st)) return -1; }
-    { CskCall k = base(L.wd, c->d_h, TH, F, c->csk_d, CSK_RESID); k.resid = c->d_resid; k.norm_w = (i + 1 < g.t_layers) ? c->tl[i + 1].ln1 : c->final_norm;
-      k.xw = c->d_xn; k.ssq_out = c->d_ssq;
-      count(c); if (gemm_csk(k, st)) return -1; }
+    if (csk_gemm(c, DG_QKV, i, B, st)) return -1;
+    count(c); if (attention_decode(decode_attn_call(c, c->tl[i], B, 1), st)) return -1;
+    if (csk_gemm(c, DG_O, i, B, st) || csk_gemm(c, DG_GATE_UP, i, B, st) || csk_gemm(c, DG_DOWN, i, B, st)) return -1;
   }
-  { CskCall k = base(c->lm_head, c->d_xn, g.t_vocab, TH, c->csk_lm, CSK_OUT_F32); k.out = c->ws_lm; k.ldo = g.t_vocab; k.ssq_in = c->d_ssq; k.ssq_slots = slots;
-    count(c); if (gemm_csk(k, st)) return -1; }
-  if (logits_argmax(c, B, logits, tok_out, nullptr, 1, st, 1)) return -1;
+  if (csk_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
+  if (logits_argmax(c, B, logits, tok_out, 1, st, 1)) return -1;
   count(c); if (advance_and_reserve(c, B, st)) return -1;
   return 0;
 }
 
-// Decode step, 5 kernels per layer:  QKV GEMM -> attention(+reduce, rstd, RoPE, append) -> O GEMM [+residual, norm weight, sum sq]
-//   -> gate/up GEMM [+rstd, SiLU*mul] -> down GEMM [+residual, next norm weight, sum sq].  The bracketed consumers run inside
-// the GEMM, in the CTA whose split-K partial completes a tile; RMSNorm's per-row scale is deferred to the next consumer.
 static int decode_enqueue(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, cudaStream_t st) {
-  if (c->decode_schedule == 2 && B <= 32) return decode_enqueue_csk(c, tok_in, B, logits, tok_out, st);
-  if (!c->fused_decode) return decode_enqueue_unfused(c, tok_in, B, logits, tok_out, st);
-  const vcla_config& g = c->cfg;
-  const int TH = g.t_hidden, F = g.t_ffn, H = g.t_heads;
-  count(c); if (dec_embed(tok_in, B, TH, c->embed, g.t_vocab, c->d_resid, c->tl[0].ln1, g.t_eps, c->d_xn, c->d_rstd, nullptr, 0, st)) return -1;
-  const float scale = 1.0f / sqrtf(128.f);
-  GemmFix fr;   // residual + deferred norm
-  fr.mode = FIX_RESID; fr.resid = c->d_resid; fr.xw_out = c->d_xn; fr.ssq = c->d_ssq; fr.rstd_out = c->d_rstd; fr.inv_dim = 1.0f / (float)TH; fr.eps = g.t_eps;
-  GemmFix fs;   // SwiGLU
-  fs.mode = FIX_SWIGLU; fs.tile_counters = c->cnt_gu; fs.rstd_in = c->d_rstd; fs.h_out = c->d_h;
-  for (int i = 0; i < g.t_layers; ++i) {
-    const TextLayer& L = c->tl[i];
-    if (swap_gemm(c, L.wqkv, 3 * TH, TH, c->d_xn, B, c->sp_qkv, c->ws_qkv, st)) return -1;
-    DecodeAttnCall a; a.qkv_partial = c->ws_qkv; a.splits = c->sp_qkv; a.ws_rows = B; a.kv_pages = L.kv; a.page_table = c->page_table;
-    a.pages_per_seq = c->pages_per_seq; a.page_tokens = c->page_tokens; a.seq_len = c->seq_len; a.out = c->d_attn; a.scratch = c->attn_scratch;
-    a.counters = c->attn_counters; a.B = B; a.H = H; a.HD = 128; a.scale = scale; a.rope_theta = g.rope_theta; a.rstd = c->d_rstd;
-    a.rope_cos = c->rope_cos; a.rope_sin = c->rope_sin; a.persistent_mode = c->attn_persistent_mode; a.persistent_grid = c->attn_persistent_grid;
-    // enough CTAs to cover the SMs for small batches; long contexts split so a CTA streams <= ~12 pages
-    { int want = (num_sms() + B * H - 1) / (B * H); int ks = want > c->kv_splits ? want : c->kv_splits; a.kv_splits = ks > 8 ? 8 : ks; }
-    count(c); if (attention_decode(a, st)) return -1;
-    fr.tile_counters = c->cnt_o; fr.norm_w = L.ln2;
-    if (swap_gemm(c, L.wo, TH, TH, c->d_attn, B, c->sp_o, c->ws_o, st, &fr)) return -1;
-    if (swap_gemm(c, L.wgu, 2 * F, TH, c->d_xn, B, c->sp_gu, c->ws_gu, st, &fs)) return -1;
-    fr.tile_counters = c->cnt_d; fr.norm_w = (i + 1 < g.t_layers) ? c->tl[i + 1].ln1 : c->final_norm;
-    if (swap_gemm(c, L.wd, TH, F, c->d_h, B, c->sp_d, c->ws_d, st, &fr)) return -1;
-  }
-  if (swap_gemm(c, c->lm_head, g.t_vocab, TH, c->d_xn, B, c->sp_lm, c->ws_lm, st)) return -1;
-  if (logits_argmax(c, B, logits, tok_out, c->d_rstd, 1, st)) return -1;
-  count(c); if (advance_and_reserve(c, B, st)) return -1;
-  return 0;
+  return decode_uses_csk(B) ? decode_enqueue_csk(c, tok_in, B, logits, tok_out, st) : decode_enqueue_workspace(c, tok_in, B, logits, tok_out, st);
 }
 
 static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, int n_steps, cudaStream_t st) {
@@ -1083,7 +1080,7 @@ int vcla_decode_step(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, i
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_in || !tok_out) { set_error("decode: null token buffers"); return -1; }
   if (decode_capacity(c, 1)) return -1;
-  if (c->decode_schedule == 2 && B <= 32 && csk_prepare(c, B)) return -1;      // occupancy queries: never inside a capture
+  if (decode_uses_csk(B) && csk_prepare(c, B)) return -1;      // occupancy queries: never inside a capture
   int rc = use_graph ? decode_graph(c, tok_in, B, logits, tok_out, 1, st) : decode_enqueue(c, tok_in, B, logits, tok_out, st);
   if (rc == 0 && !use_graph && c->dp_on()) rc = dp_wait(c, st);
   if (rc == 0) c->len_bound += 1;
@@ -1096,7 +1093,7 @@ int vcla_decode_multi(vcla_ctx* c, int32_t* tok_inout, int B, int n_steps, vcla_
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_inout || n_steps < 1 || n_steps > 64) { set_error("decode_multi: bad arguments"); return -1; }
   if (decode_capacity(c, n_steps)) return -1;
-  if (c->decode_schedule == 2 && B <= 32 && csk_prepare(c, B)) return -1;
+  if (decode_uses_csk(B) && csk_prepare(c, B)) return -1;
   const int rc = decode_graph(c, tok_inout, B, nullptr, tok_inout, n_steps, (cudaStream_t)stream);
   if (rc == 0) c->len_bound += n_steps;
   return rc;
@@ -1188,10 +1185,7 @@ int vcla_nccl_init(vcla_ctx* c, const uint8_t* id128, int rank, int world, int w
   VCLA_CUDA_OK(cudaEventCreateWithFlags(&c->dp_fork, cudaEventDisableTiming));
   VCLA_CUDA_OK(cudaEventCreateWithFlags(&c->dp_join, cudaEventDisableTiming));
   // graphs captured before the communicator existed do not contain the exchange
-  VCLA_CUDA_OK(cudaDeviceSynchronize());
-  for (auto& kv : c->graphs) cudaGraphExecDestroy(kv.second);
-  c->graphs.clear(); c->graph_launches.clear(); c->graph_lru.clear();
-  return 0;
+  return drop_graphs(c);
 }
 
 int vcla_allgather_tokens(vcla_ctx* c, const int32_t* local_dev, int n, int32_t* all_dev, vcla_stream stream) {
@@ -1251,34 +1245,11 @@ int vcla_bench_decode_gemm(vcla_ctx* c, int which, int B, int reps, float* avg_u
   cudaEvent_t e0, e1;
   VCLA_CUDA_OK(cudaEventCreate(&e0));
   VCLA_CUDA_OK(cudaEventCreate(&e1));
-  const bool csk = c->decode_schedule == 2 && B <= 32;
+  const bool csk = decode_uses_csk(B);
   if (csk && csk_prepare(c, B)) return -1;
-  const int slots = (TH + 127) / 128;
-  auto csk_one = [&](int w, const TextLayer* L) -> int {
-    CskCall k; k.B = B; k.inv_dim = 1.0f / (float)TH; k.eps = g.t_eps;
-    if (w == 0) { k.W = L->wqkv; k.X = c->d_xn; k.M = 3 * TH; k.K = TH; k.splits = c->csk_qkv; k.mode = CSK_OUT_F32; k.out = c->ws_qkv; k.ldo = 3 * TH; k.ssq_in = c->d_ssq; k.ssq_slots = slots; }
-    if (w == 1) { k.W = L->wo; k.X = c->d_attn; k.M = TH; k.K = TH; k.splits = c->csk_o; k.mode = CSK_RESID; k.resid = c->d_resid; k.norm_w = L->ln2; k.xw = c->d_xn; k.ssq_out = c->d_ssq; }
-    if (w == 2) { k.W = L->wgu; k.X = c->d_xn; k.M = 2 * F; k.K = TH; k.splits = c->csk_gu; k.mode = CSK_SWIGLU; k.h = c->d_h; k.ssq_in = c->d_ssq; k.ssq_slots = slots; }
-    if (w == 3) { k.W = L->wd; k.X = c->d_h; k.M = TH; k.K = F; k.splits = c->csk_d; k.mode = CSK_RESID; k.resid = c->d_resid; k.norm_w = L->ln1; k.xw = c->d_xn; k.ssq_out = c->d_ssq; }
-    if (w == 4) { k.W = c->lm_head; k.X = c->d_xn; k.M = g.t_vocab; k.K = TH; k.splits = c->csk_lm; k.mode = CSK_OUT_F32; k.out = c->ws_lm; k.ldo = g.t_vocab; k.ssq_in = c->d_ssq; k.ssq_slots = slots; }
-    count(c); return gemm_csk(k, st);
-  };
   auto run_all = [&]() -> int {
-    if (csk) {
-      if (which == 4) return csk_one(4, nullptr);
-      for (int i = 0; i < g.t_layers; ++i) if (csk_one(which, &c->tl[i])) return -1;
-      return 0;
-    }
-    if (which == 4) return swap_gemm(c, c->lm_head, g.t_vocab, TH, c->d_xn, B, c->sp_lm, c->ws_lm, st);
-    for (int i = 0; i < g.t_layers; ++i) {
-      const TextLayer& L = c->tl[i];
-      int rc = 0;
-      if (which == 0) rc = swap_gemm(c, L.wqkv, 3 * TH, TH, c->d_xn, B, c->sp_qkv, c->ws_qkv, st);
-      if (which == 1) rc = swap_gemm(c, L.wo, TH, TH, c->d_attn, B, c->sp_o, c->ws_o, st);
-      if (which == 2) rc = swap_gemm(c, L.wgu, 2 * F, TH, c->d_xn, B, c->sp_gu, c->ws_gu, st);
-      if (which == 3) rc = swap_gemm(c, L.wd, TH, F, c->d_h, B, c->sp_d, c->ws_d, st);
-      if (rc) return rc;
-    }
+    const int layers = which == DG_LM_HEAD ? 1 : g.t_layers;
+    for (int i = 0; i < layers; ++i) if (csk ? csk_gemm(c, which, i, B, st) : ws_gemm(c, which, i, B, st)) return -1;
     return 0;
   };
   if (run_all()) return -1;  // warm-up
@@ -1308,13 +1279,13 @@ int vcla_read_history(vcla_ctx* c, int32_t* dst_dev, int B, int n_steps, vcla_st
 int vcla_trace_enable(vcla_ctx* c, int max_events) {
   // installs (max_events > 0) or removes (0) the timeline buffer every kernel's CTA 0 appends to
   VCLA_CUDA_OK(cudaDeviceSynchronize());
-  if (c->trace_buf) { trace_set_gemm(nullptr, 0); trace_set_attention_tc(nullptr, 0); trace_set_gemm_decode(nullptr, 0); trace_set_sampler(nullptr, 0); trace_set_attention(nullptr, 0); trace_set_elementwise(nullptr, 0); cudaFree(c->trace_buf); c->trace_buf = nullptr; c->trace_cap = 0; }
+  if (c->trace_buf) { trace_set_all(nullptr, 0); cudaFree(c->trace_buf); c->trace_buf = nullptr; c->trace_cap = 0; }
   if (max_events <= 0) return 0;
   const size_t bytes = 8 + (size_t)max_events * 32;
   VCLA_CUDA_OK(cudaMalloc(&c->trace_buf, bytes));
   VCLA_CUDA_OK(cudaMemset(c->trace_buf, 0, bytes));
   c->trace_cap = (unsigned long long)max_events;
-  if (trace_set_gemm(c->trace_buf, c->trace_cap) || trace_set_attention_tc(c->trace_buf, c->trace_cap) || trace_set_gemm_decode(c->trace_buf, c->trace_cap) || trace_set_sampler(c->trace_buf, c->trace_cap) || trace_set_attention(c->trace_buf, c->trace_cap) || trace_set_elementwise(c->trace_buf, c->trace_cap)) {
+  if (trace_set_all(c->trace_buf, c->trace_cap)) {
     set_error("vcla_trace_enable: cudaMemcpyToSymbol failed");
     return -1;
   }
@@ -1359,10 +1330,7 @@ int vcla_debug_set_csk_splits(vcla_ctx* c, int B, int qkv, int o, int gu, int d,
   int* dst[5] = {&c->csk_qkv, &c->csk_o, &c->csk_gu, &c->csk_d, &c->csk_lm};
   const int v[5] = {qkv, o, gu, d, lm};
   for (int i = 0; i < 5; ++i) if (v[i] >= 1 && v[i] <= 8) *dst[i] = v[i];
-  VCLA_CUDA_OK(cudaDeviceSynchronize());
-  for (auto& kv : c->graphs) cudaGraphExecDestroy(kv.second);
-  c->graphs.clear(); c->graph_launches.clear(); c->graph_lru.clear();
-  return 0;
+  return drop_graphs(c);
 }
 int vcla_debug_get_csk_splits(vcla_ctx* c, int B, int* out5) {
   if (!c || !out5 || B < 1 || B > 32) return -1;

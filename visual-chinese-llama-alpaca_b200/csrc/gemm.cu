@@ -65,7 +65,6 @@ struct GemmParams {
   int ws_rows;
   int l2_prefetch_kb;
   uint64_t policy_a, policy_b;
-  GemmFix fix;
   GemmRowScale rowscale;
   GemmEmitNorm emit;
   GemmRope rope;
@@ -73,7 +72,7 @@ struct GemmParams {
 
 constexpr int kBlockK = 64;
 constexpr int kGemmThreads = 160;   // warps 0..3 = the wgmma warpgroup (MMA + epilogue), warp 4 = TMA producer
-constexpr int kSwapBlockM = 128;    // swap-AB tiles: 128 weight rows (the split-K fixup's tile counters count these)
+constexpr int kSwapBlockM = 128;    // swap-AB tiles: 128 weight rows (the two 64-row wgmma blocks of one warpgroup)
 
 // BM x BN tile, BM / 64 wgmma row blocks; the accumulators take BM * BN / 128 fp32 registers per thread (<= 128)
 template <int BM, int BN, int STAGES>
@@ -83,8 +82,7 @@ struct GemmCfg {
   static constexpr int B_BYTES = BN * kBlockK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
-  static constexpr int FIX_OFF = BAR_OFF + 256;             // [4 warps][64] fp32 cross-warp scratch + 1 flag of the split-K fixup
-  static constexpr int SMEM_BYTES = FIX_OFF + 1088 + 1024;  // barriers + fixup scratch, + slack for 1024 B alignment
+  static constexpr int SMEM_BYTES = BAR_OFF + 256 + 1024;   // barriers, + slack for 1024 B alignment
   static_assert(STAGE_BYTES % 1024 == 0, "stage must keep 1024 B alignment for SWIZZLE_128B");
   static_assert(BM == 64 || BM == 128, "tile rows");
   static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256 && BM * BN <= 64 * 256, "wgmma N constraint / accumulator registers");
@@ -104,7 +102,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   static_assert(!SWAP || BM == kSwapBlockM, "swap-AB tiles are 128 weight rows");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
   const uint32_t bar0 = base + C::BAR_OFF;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
@@ -259,124 +256,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
           }
         }
-        if (p.fix.mode != FIX_NONE) {
-          // ---- split-K fixup: the CTA whose partial completes the tile reduces all partials (fixed order) and applies
-          //      the fused consumer.  Classic last-block pattern: fence, count, fence.  Thread t owns tile row t here.
-          const int q = warp;
-          const int row_in_tile = q * 32 + lane;
-          const int row = m_blk * BM + row_in_tile;
-          const bool row_ok = row < p.M;
-          volatile int* s_flag = reinterpret_cast<volatile int*>(base_ptr + C::FIX_OFF + 1024);
-          float* s_red = reinterpret_cast<float*>(base_ptr + C::FIX_OFF);          // [4][64]
-          __threadfence();
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          if (warp == 0 && lane == 0) {
-            const int old = atomicAdd(p.fix.tile_counters + m_blk, 1);
-            *s_flag = (old == p.splits - 1) ? 1 : 0;
-          }
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          if (*s_flag) {
-            __threadfence();
-            const int nb = p.ws_rows;                 // batch rows
-            if (p.fix.mode == FIX_RESID) {
-              for (int b0 = 0; b0 < nb; b0 += 8) {    // 8 batch rows per pass; partial loads issued 4 splits x 8 rows at a time
-                float r[8];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) r[j] = 0.f;
-                if (row_ok) {
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) if (b0 + j < nb) r[j] = p.fix.resid[(size_t)(b0 + j) * p.ldo + row];
-                  for (int sp0 = 0; sp0 < p.splits; sp0 += 4) {
-                    float t4[4][8];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u)
-#pragma unroll
-                      for (int j = 0; j < 8; ++j)
-                        t4[u][j] = (sp0 + u < p.splits && b0 + j < nb) ? __ldcg(ws + ((size_t)(sp0 + u) * nb + b0 + j) * (size_t)p.ldo + row) : 0.f;
-#pragma unroll
-                    for (int u = 0; u < 4; ++u)
-#pragma unroll
-                      for (int j = 0; j < 8; ++j) r[j] += t4[u][j];      // fixed split order: deterministic
-                  }
-                  const float wn = __ldg(p.fix.norm_w + row);
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) {
-                    if (b0 + j < nb) {
-                      p.fix.resid[(size_t)(b0 + j) * p.ldo + row] = r[j];
-                      p.fix.xw_out[(size_t)(b0 + j) * p.ldo + row] = __float2bfloat16(r[j] * wn);
-                    }
-                  }
-                }
-                // sum of squares over the tile's 128 rows, per batch row
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  float q2 = warp_sum(r[j] * r[j]);
-                  if (lane == 0) s_red[q * 64 + b0 + j] = q2;
-                }
-              }
-              asm volatile("bar.sync 1, 128;" ::: "memory");
-              const int t = row_in_tile;                // 0..127
-              if (t < nb) p.fix.ssq[(size_t)t * p.m_tiles + m_blk] = s_red[t] + s_red[64 + t] + s_red[128 + t] + s_red[192 + t];
-              // second level: the CTA that finishes the last tile turns the per-tile sums into the per-row scale
-              __threadfence();
-              asm volatile("bar.sync 1, 128;" ::: "memory");
-              if (warp == 0 && lane == 0) {
-                const int old = atomicAdd(p.fix.tile_counters + p.m_tiles, 1);
-                *s_flag = (old == p.m_tiles - 1) ? 2 : 1;
-              }
-              asm volatile("bar.sync 1, 128;" ::: "memory");
-              if (*s_flag == 2) {
-                __threadfence();
-                if (t < nb) {
-                  float ss = 0.f;
-                  for (int t0 = 0; t0 < p.m_tiles; t0 += 8) {
-                    float v8[8];
-#pragma unroll
-                    for (int u = 0; u < 8; ++u) v8[u] = (t0 + u < p.m_tiles) ? __ldcg(p.fix.ssq + (size_t)t * p.m_tiles + t0 + u) : 0.f;
-#pragma unroll
-                    for (int u = 0; u < 8; ++u) ss += v8[u];
-                  }
-                  p.fix.rstd_out[t] = rsqrtf(ss * p.fix.inv_dim + p.fix.eps);
-                }
-                if (warp == 0 && lane == 0) p.fix.tile_counters[p.m_tiles] = 0;
-              }
-            } else {  // FIX_SWIGLU: tile rows = [32 gate | 32 up | 32 gate | 32 up]
-              const int blk = row_in_tile >> 6, within = row_in_tile & 63;
-              const int gi = within & 31;                       // pair index inside the 64-row block
-              const int grow = m_blk * BM + blk * 64 + gi;      // gate row ; up row = grow + 32
-              const int jout = m_blk * 64 + blk * 32 + gi;      // output feature
-              const bool pair_ok = (grow + 32) < p.M;
-              const int half = (nb + 1) >> 1;
-              const int bs = (within < 32) ? 0 : half, be = (within < 32) ? half : nb;   // the two partner lanes split the batch
-              for (int b0 = bs; b0 < be; b0 += 4) {             // 4 batch rows x all splits in flight
-                float g[4] = {0.f, 0.f, 0.f, 0.f}, u[4] = {0.f, 0.f, 0.f, 0.f};
-                if (pair_ok) {
-                  for (int sp = 0; sp < p.splits; ++sp) {
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                      if (b0 + j < be) {
-                        const float* pr = ws + ((size_t)sp * nb + b0 + j) * (size_t)p.ldo;
-                        g[j] += __ldcg(pr + grow);
-                        u[j] += __ldcg(pr + grow + 32);
-                      }
-                    }
-                  }
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-                    if (b0 + j < be) {
-                      const float rstd = __ldcg(p.fix.rstd_in + b0 + j);
-                      const float gg = g[j] * rstd, uu = u[j] * rstd;
-                      p.fix.h_out[(size_t)(b0 + j) * (p.ldo >> 1) + jout] = __float2bfloat16(gg / (1.f + __expf(-gg)) * uu);
-                    }
-                  }
-                }
-              }
-            }
-            __syncwarp();
-            if (warp == 0 && lane == 0) p.fix.tile_counters[m_blk] = 0;   // ready for the next launch / graph replay
-          }
-        }
-        continue;
       } else {
         const int col_tile = n_blk * BN;
 #pragma unroll
@@ -654,7 +533,6 @@ int gemm_tc(const GemmCall& c, cudaStream_t st) {
   p.rows_per_group = c.rows_per_group; p.group_stride = c.group_stride; p.row_offset = c.row_offset;
   p.ws_rows = c.ws_rows;
   p.l2_prefetch_kb = c.l2_prefetch_kb;
-  p.fix = c.fix;
   p.rowscale = c.rowscale; p.emit = c.emit; p.rope = c.rope;
   p.policy_a = c.weights_are_A ? kEvictFirst : kEvictLast;
   p.policy_b = c.weights_are_A ? kEvictLast : kEvictNormal;
@@ -666,8 +544,6 @@ int gemm_tc(const GemmCall& c, cudaStream_t st) {
     p.splits = (p.kb_total + p.kb_per_split - 1) / p.kb_per_split;   // every split non-empty
     if (p.splits != splits) { set_error("gemm: split count %d not realisable for %d k-blocks (use %d)", splits, p.kb_total, p.splits); return -1; }
     if (c.N > 64 || c.ws_rows < c.N) { set_error("gemm: swap-AB batch rows %d (ws_rows %d) unsupported", c.N, c.ws_rows); return -1; }
-    if (c.fix.mode != FIX_NONE && (c.fix.tile_counters == nullptr || c.ws_rows != c.N || c.ldo != c.M)) { set_error("gemm: split-K fixup needs tile counters, ws_rows == batch and ldo == rows"); return -1; }
-    if (c.fix.mode == FIX_SWIGLU && (c.M % 64) != 0) { set_error("gemm: SwiGLU fixup needs rows %% 64 == 0"); return -1; }
     if (c.N <= 16) return launch<128, 16, 5, true>(c, p, st);
     if (c.N <= 32) return launch<128, 32, 5, true>(c, p, st);
     return launch<128, 64, 4, true>(c, p, st);

@@ -35,24 +35,6 @@ enum GemmMode {
   GEMM_PARTIAL_F32 = 3,  // swap-AB split-K partials: ws[(split*ws_rows + col) * ldo + row] = acc   (row = A row)
 };
 enum Act { ACT_NONE = 0, ACT_QUICK_GELU = 1, ACT_GELU_ERF = 2 };
-// Fused consumer of the split-K partials, run by the CTA that completes a tile ("last arriver", GEMM_PARTIAL_F32 only):
-//   FIX_RESID : r = resid[b,n] + sum_s partial ; resid = r ; xw[b,n] = bf16(r * norm_w[n]) ; ssq[b, tile] = sum_n r^2 ;
-//               the CTA that completes the LAST tile also writes rstd[b] = rsqrt(sum_tiles ssq / N + eps).
-//               (RMSNorm with the per-row scale deferred to the next consumer: a row scalar commutes with the next GEMM.)
-//   FIX_SWIGLU: g,u = rstd[b] * sum_s partial (rows interleaved [32 gate | 32 up]) ; h[b,j] = bf16(silu(g) * u)
-enum FixMode { FIX_NONE = 0, FIX_RESID = 1, FIX_SWIGLU = 2 };
-struct GemmFix {
-  int mode = FIX_NONE;
-  int32_t* tile_counters = nullptr;   // [m_tiles + 1] zero between launches; the last entry counts finished tiles
-  float* resid = nullptr;             // [B, N_out] fp32 (FIX_RESID)
-  const float* norm_w = nullptr;      // [N_out]
-  bf16* xw_out = nullptr;             // [B, N_out]
-  float* ssq = nullptr;               // [B, m_tiles] scratch
-  float* rstd_out = nullptr;          // [B]
-  float inv_dim = 0.f, eps = 0.f;
-  const float* rstd_in = nullptr;     // [B] (FIX_SWIGLU)
-  bf16* h_out = nullptr;              // [B, N_out/2]
-};
 
 // ---- prefill epilogue fusions (non-swap GEMMs) --------------------------------------------------------------------------
 // Deferred RMSNorm: the A operand holds xw = bf16(resid * norm_w) (NOT normalised); the row scale rstd[row] =
@@ -101,7 +83,6 @@ struct GemmCall {
   int weights_are_A = 0;     // cache-policy hint: A is the streamed-once operand (decode)
   int bn = 0;                // tile N override (0 = auto)
   int l2_prefetch_kb = 0;    // k-blocks of the weight operand each CTA prefetches into L2 while it waits for its dependency
-  GemmFix fix;               // fused consumer of the split-K partials (decode)
   GemmRowScale rowscale;     // deferred RMSNorm scale of the A rows (STORE_BF16 / SWIGLU_BF16)
   GemmEmitNorm emit;         // ADD_F32 + accumulate: also write the next operand + row statistics
   GemmRope rope;             // STORE_BF16: RoPE + KV-cache append (runs on the 64 x 256 tile, N = 3T)
@@ -170,7 +151,6 @@ struct DecodeAttnCall {
   int32_t* counters = nullptr;         // [B][H]
   int B = 0, H = 0, HD = 0, kv_splits = 1;
   float scale = 1.f, rope_theta = 10000.f;
-  const float* rstd = nullptr;         // [B] deferred RMSNorm scale of the QKV projection's input (null: 1)
   const float* rope_cos = nullptr;     // [max_pos][HD/2] fp32 tables owned by the context
   const float* rope_sin = nullptr;
   int persistent_mode = 1;             // VCLA_ATTN_PERSISTENT (read once per context)
@@ -201,12 +181,6 @@ int embed_tokens(const int64_t* ids, int B, int T, int S, int D, const bf16* tab
 int embed_tokens_i32(const int32_t* ids, int B, int D, const bf16* table, int vocab, float* dst, cudaStream_t st);
 // copy the projected image rows (B, nq, D) fp32 into the residual stream at per-sample row offsets
 int scatter_image_rows(const float* img, int B, int nq, int D, const int32_t* row_start, int S, float* dst, cudaStream_t st);
-// prefill: RoPE q,k in place in the fused qkv buffer [B*S, 3T] and append k,v to the paged cache
-// left_pad[b] (nullable): rows s < left_pad[b] are padding (skipped); the cache index of row s is s - left_pad[b]; the RoPE
-// position is s - left_pad[b] when pos_from_mask (HF generate) else s (plain forward without position_ids)
-int rope_and_cache(bf16* qkv, int B, int S, int H, int HD, const float* rope_cos, const float* rope_sin, bf16* kv_pages,
-                   const int32_t* page_table, int pages_per_seq, int page_tokens, const int32_t* left_pad, int pos_from_mask,
-                   cudaStream_t st);
 int gather_last_rows(const float* hidden, int B, int S, int D, float* dst, cudaStream_t st);
 
 // decode consumers of split-K partials
@@ -219,10 +193,10 @@ int dec_silu_mul(const float* partial, int splits, int ws_rows, int B, int F, bf
 // cand_val / cand_idx: [B][kArgmaxChunks] scratch owned by the context
 constexpr int kArgmaxChunks = 32;
 int dec_logits_argmax(const float* partial, int splits, int ws_rows, int ldp, int B, int V, float* logits, int ld_logits,
-                      int32_t* tok, int32_t* history, const int32_t* step_idx, const float* rstd, float* cand_val,
+                      int32_t* tok, int32_t* history, const int32_t* step_idx, float* cand_val,
                       int32_t* cand_idx, int32_t* dp_send, cudaStream_t st);
-// stage 1 only: logits[b, :] = rstd[b] * sum_s partial (the sampler consumes them)
-int dec_logits_reduce(const float* partial, int splits, int ws_rows, int ldp, int B, int V, float* logits, int ld_logits, const float* rstd,
+// stage 1 only: logits[b, :] = sum_s partial (the sampler consumes them)
+int dec_logits_reduce(const float* partial, int splits, int ws_rows, int ldp, int B, int V, float* logits, int ld_logits,
                       float* cand_val, int32_t* cand_idx, cudaStream_t st);
 // ---- device-side sampling (sampler.cu) ----------------------------------------------------------------------------------
 struct SamplerParams {     // lives in device memory: graphs captured once serve every parameter set
@@ -243,10 +217,10 @@ int sampler_init();
 int dec_sample(const float* logits, int ld, int V, int B, const int32_t* history, const int32_t* step_idx, const SamplerParams* params_dev,
                int32_t* tok, int32_t* history_out, int32_t* dp_send, int32_t* finished, float* scores_out, cudaStream_t st);
 int dp_unpack(const int32_t* recv, int n, int32_t* hist, int32_t* dp_step, cudaStream_t st);
-// decode step entry: resid[b,:] = table[ids[b]] ; xw = bf16(resid * norm_w) ; rstd[b] = rsqrt(mean(resid^2) + eps) (nullable) ;
-// ssq[b][0] = sum resid^2, ssq[b][1..slots) = 0 (nullable: head of the deferred-norm chain of the cluster split-K schedule)
-int dec_embed(const int32_t* ids, int B, int D, const bf16* table, int vocab, float* resid, const float* norm_w, float eps,
-              bf16* xw, float* rstd, float* ssq, int slots, cudaStream_t st);
+// decode step entry of the cluster split-K schedule: resid[b,:] = table[ids[b]] ; xw = bf16(resid * norm_w) ;
+// ssq[b][0] = sum resid^2, ssq[b][1..slots) = 0 (head of the deferred-norm chain)
+int dec_embed(const int32_t* ids, int B, int D, const bf16* table, int vocab, float* resid, const float* norm_w,
+              bf16* xw, float* ssq, int slots, cudaStream_t st);
 // ---- device-side KV page allocator (stream-ordered, graph-capturable; one thread walks the <= 64 sequences, so the
 //      assignment is deterministic) ------------------------------------------------------------------------------
 // kv_state[0] = free pages, kv_state[1] = error flag (pool exhausted); kv_free = stack of free physical pages;
