@@ -105,6 +105,10 @@ int vcla_reset(vcla_ctx* ctx, vcla_stream stream);
 int vcla_kv_geometry(const vcla_ctx* ctx, int* pages_per_seq, int* total_pages, int* page_tokens);
 int vcla_kv_read_pages(vcla_ctx* ctx, int32_t* table_host, int32_t* npages_host, int32_t* state_host);
 int vcla_kv_debug_shuffle(vcla_ctx* ctx, uint32_t seed);
+/* Keep each resident sequence's first min(current length, len_host[b]) cached tokens (b < B, B = the batch of the last
+ * vcla_prefill) and forget the rest; the pages stay owned by the sequence (vcla_reset returns them).  With vcla_prefill_extend this
+ * reuses the common prefix of a conversation: HF DynamicCache.crop (HF:cache_utils.py) before generate(past_key_values=...). */
+int vcla_kv_truncate(vcla_ctx* ctx, const int32_t* len_host, int B, vcla_stream stream);
 
 /* pixels (B,3,I,I) NCHW -> image embeddings (B, r_queries, t_hidden), kept inside the context for the
  * next vcla_prefill and optionally copied to `out_dev_f32`.  Replaces
@@ -131,6 +135,17 @@ int vcla_vision_encode(vcla_ctx* ctx, const void* pixels_dev, int pixel_dtype, i
 int vcla_prefill(vcla_ctx* ctx, const int64_t* ids_dev, int B, int T, int image_mode, const int32_t* img_row_dev,
                  const int32_t* left_pad_dev, int pos_from_mask, float* logits_all_dev, float* last_logits_dev,
                  int32_t* next_tok_dev, vcla_stream stream);
+
+/* Append T text tokens (ids_dev int64 (B,T)) to each of the B sequences resident since the last vcla_prefill (same B): the chunk
+ * row t of sequence b is token L_b + t (RoPE position and cache slot; L_b = its current cached length) and attends to all L_b
+ * cached tokens plus the chunk's rows up to itself.  No vision work: the cached prefix keeps its image rows.  Outputs as
+ * vcla_prefill, over the chunk's rows only (logits_all_dev f32 (B,T,V)); lengths grow by T.  Like vcla_prefill it restarts the
+ * token history (row 0 = this call's pick), the sampler's step counter and the finished flags.  Fails when nothing is resident,
+ * while the data-parallel exchange is active, when B*T > max_prefill_tokens or when a sequence could pass max_seq.  Replaces HF
+ * generate(input_ids, past_key_values=cache): the forward over the uncached tail of the prompt (HF:generation/utils.py,
+ * HF:models/llama/modeling_llama.py with past_key_values). */
+int vcla_prefill_extend(vcla_ctx* ctx, const int64_t* ids_dev, int B, int T, float* logits_all_dev, float* last_logits_dev,
+                        int32_t* next_tok_dev, vcla_stream stream);
 
 /* One greedy decode step for the B resident sequences: consumes tok_in_dev (int32 (B)), appends its K/V,
  * writes logits (f32 (B,V), optional) and the argmax (int32 (B)).  Captured into a CUDA graph on first use
@@ -232,6 +247,13 @@ void vcla_set_attention_tc(int mode);
 int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v0, int kv0_stride, int n0, const void* k1,
                       const void* v1, int kv1_stride, int n1, void* out, int o_stride, int B, int H, int Sq, int HD, float scale,
                       int causal, vcla_stream stream);
+/* The paged prefill attention of vcla_prefill_extend on caller buffers (head dim 128): q (B*T rows, q_stride) bf16; kv_pages a layer
+ * pool [pages][K|V][H][page_tokens][128] bf16; page_table int32 (B, pages_per_seq); base_len_dev int32 (B) cached tokens before the
+ * chunk (the chunk's own K/V must already be in the pool at slots base_len .. base_len + T - 1); out (B*T rows, o_stride) bf16.
+ * Key j is visible to chunk row t iff j <= base_len[b] + t.  Synchronises. */
+int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, const int32_t* page_table, int pages_per_seq,
+                            int page_tokens, const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T, float scale,
+                            vcla_stream stream);
 int vcla_op_layernorm(const float* x, int rows, int D, const float* w, const float* b, float eps, void* y_bf16, float* y_f32,
                       vcla_stream stream);
 int vcla_op_rmsnorm(const float* x, int rows, int D, const float* w, float eps, void* y_bf16, vcla_stream stream);

@@ -12,9 +12,18 @@
 // O accumulates in registers; the online-softmax rescale (O *= exp2(m_old - m_new)) is a multiply of the thread's fragment rows.
 // K/V tiles are double buffered, two CTAs share an SM.  Masks: keys past a segment's end, causal (key <= query + Sk - Sq), left
 // padding (kv_start).  Fully masked rows produce zeros, like the mma.sync kernel (csrc/attention.cu).
+//
+// PAGED = true is the prefill of a chunk of new tokens over a cached prefix (vcla_prefill_extend): the queries are the Sq new rows
+// of sequence b, the keys / values are its first base_len[b] + Sq cached tokens, read straight from the layer's page pool (the
+// chunk's own K/V were appended by the QKV GEMM epilogue).  Key j is visible to chunk row t iff j <= base_len[b] + t.  The pool
+// [pages][K|V][H][page_tokens][128] is one 2D tensor of 128-column rows (256 B pitch); a 64-key tile is 64 / page_tokens boxes of
+// page_tokens rows (a multiple of 8 rows = whole 128 B-swizzle atoms, so the boxes stack into the same smem image a 64-row box
+// gives) times two 64-column halves, each box addressed through the page table.  When the grid would leave SMs idle the key tiles
+// are split over kv_splits CTAs; each writes its unnormalised (O, m, l) and the last one to arrive combines them in split order.
 #include "common.cuh"
 #include "kernels.h"
 
+#include <algorithm>
 #include <mutex>
 #include <stdlib.h>
 #include <string.h>
@@ -24,6 +33,7 @@ namespace vcla {
 constexpr int kAtThreads = 160;                 // warps 0..3 = the wgmma warpgroup, warp 4 = TMA producer
 constexpr int kAtBQ = 64, kAtBKV = 64;
 constexpr int kAtStages = 2;
+constexpr int kAtMaxKvSplits = 16;
 
 struct AttnTcParams {
   int Sq, n0, n1, H;
@@ -31,6 +41,12 @@ struct AttnTcParams {
   int causal;
   const int32_t* kv_start;         // [B] or null
   bf16* out; int o_stride;
+  // PAGED only
+  const int32_t* page_table; int pages_per_seq, page_tokens;
+  const int32_t* base_len;         // [B] cached tokens before the chunk
+  int kv_splits;                   // CTAs per (query tile, head, sequence); blockIdx.z = b * kv_splits + split
+  float* part;                     // kv_splits > 1: [tile][split][64 rows][HD + 4] = unnormalised O, running max, row sum, pad
+  int32_t* counters;               // [tile] arrivals, back to 0 after the combine
 };
 
 template <int HD>
@@ -42,6 +58,7 @@ struct AttnTcCfg {
   static constexpr int KV_OFF = Q_BYTES;
   static constexpr int BAR_OFF = KV_OFF + kAtStages * (K_BYTES + V_BYTES);
   static constexpr int SMEM_BYTES = BAR_OFF + 256 + 1024;
+  static constexpr int PART_LD = HD + 4;                      // split-KV partial row: O[HD], m, l, 2 pad floats (16 B rows)
 };
 
 // MN-major operand, 128 B swizzle: rows (the contraction index) of 128 B = 64 contiguous MN elements, 8-row atoms 1024 B apart
@@ -61,7 +78,7 @@ __device__ __forceinline__ void wgmma_pv(float (&o)[HD / 2], const uint32_t (&a)
   else wgmma_bf16_rs_tb_n128(o, a, bdesc, 1);
 }
 
-template <int HD>
+template <int HD, bool PAGED>
 __global__ void __launch_bounds__(kAtThreads, 2)
 attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0, const __grid_constant__ CUtensorMap tmV0,
                        const __grid_constant__ CUtensorMap tmK1, const __grid_constant__ CUtensorMap tmV1, const AttnTcParams p) {
@@ -74,17 +91,28 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   auto kv_empty = [&](int s) { return bar0 + 8u * (1 + kAtStages + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * kAtBQ, h = blockIdx.y, b = blockIdx.z;
-  const int Sk = p.n0 + p.n1;
+  const int q0 = blockIdx.x * kAtBQ, h = blockIdx.y;
+  const int b = PAGED ? (int)blockIdx.z / p.kv_splits : (int)blockIdx.z;
+  const int split = PAGED ? (int)blockIdx.z % p.kv_splits : 0;
+  TraceScope trace(3);
+  // PAGED: the keys are the sequence's cached tokens; their count is read after the kernels that wrote it have finished
+  if constexpr (PAGED) pdl_wait();
+  const int base_len = PAGED ? p.base_len[b] : 0;
+  const int n0 = PAGED ? base_len + p.Sq : p.n0, n1 = PAGED ? 0 : p.n1;
+  const int Sk = n0 + n1;
   const int off = Sk - p.Sq;                                   // causal: key j visible to query i iff j <= i + off
   const int kv0 = p.kv_start ? __ldg(p.kv_start + b) : 0;
-  TraceScope trace(3);
 
   // KV tiles: segment 0 tiles first, then segment 1; causal launches have one segment and stop at the diagonal tile
-  const int nt0 = (p.n0 + kAtBKV - 1) / kAtBKV, nt1 = (p.n1 + kAtBKV - 1) / kAtBKV;
+  const int nt0 = (n0 + kAtBKV - 1) / kAtBKV, nt1 = (n1 + kAtBKV - 1) / kAtBKV;
   int nt = nt0 + nt1;
   if (p.causal) { const int kv_end = min(Sk, q0 + kAtBQ + off); nt = min(nt, (max(kv_end, 0) + kAtBKV - 1) / kAtBKV); }
-  const int jt0 = kv0 / kAtBKV;                                // tiles entirely left of the padding boundary are skipped
+  int jt0 = kv0 / kAtBKV;                                      // tiles entirely left of the padding boundary are skipped
+  if (PAGED && p.kv_splits > 1) {                              // split-KV: this CTA's contiguous share of the key tiles
+    const int per = (nt + p.kv_splits - 1) / p.kv_splits;
+    jt0 = split * per;
+    nt = min(nt, jt0 + per);
+  }
   const int n_tiles = max(nt - jt0, 0);
 
   if (threadIdx.x == 0) {
@@ -92,7 +120,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
     for (int s = 0; s < kAtStages; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 1); }
     fence_barrier_init();
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK0); tma_prefetch_desc(&tmV0);
-    if (p.n1 > 0) { tma_prefetch_desc(&tmK1); tma_prefetch_desc(&tmV1); }
+    if (n1 > 0) { tma_prefetch_desc(&tmK1); tma_prefetch_desc(&tmV1); }
   }
   __syncthreads();
   pdl_launch_dependents();
@@ -108,13 +136,28 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         mbar_wait_mma(kv_empty(stage), (((uint32_t)(i / kAtStages)) & 1u) ^ 1u);
         mbar_arrive_expect_tx(kv_full(stage), C::K_BYTES + C::V_BYTES);
         const uint32_t sk = base + C::KV_OFF + stage * (C::K_BYTES + C::V_BYTES), sv = sk + C::K_BYTES;
-        const bool seg1 = j >= nt0;
-        const CUtensorMap* mk = seg1 ? &tmK1 : &tmK0;
-        const CUtensorMap* mv = seg1 ? &tmV1 : &tmV0;
-        const int row = seg1 ? b * p.n1 + (j - nt0) * kAtBKV : b * p.n0 + j * kAtBKV;
-        for (int kb = 0; kb < C::KB; ++kb) {
-          tma_load_2d(sk + kb * kAtBKV * 128, mk, h * HD + kb * 64, row, kv_full(stage), kEvictNormal);
-          tma_load_2d(sv + kb * kAtBKV * 128, mv, h * HD + kb * 64, row, kv_full(stage), kEvictNormal);
+        if constexpr (PAGED) {
+          // one box of page_tokens rows per page and 64-column half; boxes past the sequence's last page re-read that page
+          // (only pages the sequence owns are touched; those rows are masked)
+          const int pt = p.page_tokens, last_page = (n0 - 1) / pt;
+          const int32_t* prow = p.page_table + (size_t)b * p.pages_per_seq;
+          for (int r = 0; r < kAtBKV; r += pt) {
+            const int page = prow[min((j * kAtBKV + r) / pt, last_page)];
+            const int krow = ((page * 2) * p.H + h) * pt, vrow = krow + p.H * pt;
+            for (int kb = 0; kb < C::KB; ++kb) {
+              tma_load_2d(sk + kb * kAtBKV * 128 + r * 128, &tmK0, kb * 64, krow, kv_full(stage), kEvictNormal);
+              tma_load_2d(sv + kb * kAtBKV * 128 + r * 128, &tmK0, kb * 64, vrow, kv_full(stage), kEvictNormal);
+            }
+          }
+        } else {
+          const bool seg1 = j >= nt0;
+          const CUtensorMap* mk = seg1 ? &tmK1 : &tmK0;
+          const CUtensorMap* mv = seg1 ? &tmV1 : &tmV0;
+          const int row = seg1 ? b * n1 + (j - nt0) * kAtBKV : b * n0 + j * kAtBKV;
+          for (int kb = 0; kb < C::KB; ++kb) {
+            tma_load_2d(sk + kb * kAtBKV * 128, mk, h * HD + kb * 64, row, kv_full(stage), kEvictNormal);
+            tma_load_2d(sv + kb * kAtBKV * 128, mv, h * HD + kb * 64, row, kv_full(stage), kEvictNormal);
+          }
         }
       }
     }
@@ -134,11 +177,24 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
     for (int i = 0; i < n_tiles; ++i) {
       const int j = jt0 + i, stage = i % kAtStages;
       const bool seg1 = j >= nt0;
-      const int kbase = seg1 ? p.n0 + (j - nt0) * kAtBKV : j * kAtBKV;       // global key index of the tile's first row
-      const int kvalid = seg1 ? p.n1 - (j - nt0) * kAtBKV : p.n0 - j * kAtBKV; // keys of this tile that exist in the segment
+      const int kbase = seg1 ? n0 + (j - nt0) * kAtBKV : j * kAtBKV;         // global key index of the tile's first row
+      const int kvalid = seg1 ? n1 - (j - nt0) * kAtBKV : n0 - j * kAtBKV;   // keys of this tile that exist in the segment
       const int lo = max(kv0 - kbase, 0);
       const uint32_t sk = base + C::KV_OFF + stage * (C::K_BYTES + C::V_BYTES), sv = sk + C::K_BYTES;
       mbar_wait_mma(kv_full(stage), ((uint32_t)(i / kAtStages)) & 1u);
+      if constexpr (PAGED) {
+        // V rows past the sequence end are cache slots nobody wrote (any bits, NaN included) and P = 0 does not cancel a NaN
+        // in the PV product: zero them (whole 128 B rows, so the swizzle does not matter) before the tensor core reads them
+        if (kvalid < kAtBKV) {
+          for (int idx = threadIdx.x; idx < C::KB * (kAtBKV - kvalid) * 8; idx += 128) {
+            const int kb = idx / ((kAtBKV - kvalid) * 8), rem = idx % ((kAtBKV - kvalid) * 8);
+            const uint32_t addr = sv + kb * kAtBKV * 128 + (kvalid + rem / 8) * 128 + (rem % 8) * 16;
+            asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(addr), "r"(0u) : "memory");
+          }
+          fence_proxy_async();
+          asm volatile("bar.sync 1, 128;" ::: "memory");
+        }
+      }
       float s[kAtBKV / 2];
       wgmma_fence();
 #pragma unroll
@@ -200,6 +256,15 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       float l = l_run[h2];
       l += __shfl_xor_sync(0xffffffffu, l, 1);
       l += __shfl_xor_sync(0xffffffffu, l, 2);
+      if (PAGED && p.kv_splits > 1) {
+        // this split's unnormalised rows: O, the running max (log2 domain, scaled) and the row sum
+        float* prow = p.part + ((((size_t)(b * p.H + h) * gridDim.x + blockIdx.x) * p.kv_splits + split) * kAtBQ + fr + 8 * h2) * C::PART_LD;
+#pragma unroll
+        for (int jj = 0; jj < HD / 8; ++jj)
+          *reinterpret_cast<float2*>(prow + 8 * jj + fc) = make_float2(o[4 * jj + 2 * h2], o[4 * jj + 2 * h2 + 1]);
+        if ((lane & 3) == 0) *reinterpret_cast<float2*>(prow + HD) = make_float2(m_run[h2], l);
+        continue;
+      }
       const float inv = l > 0.f ? 1.f / l : 0.f;
       const int qi = q0 + fr + 8 * h2;
       if (qi < p.Sq) {
@@ -207,6 +272,44 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 #pragma unroll
         for (int jj = 0; jj < HD / 8; ++jj)
           *reinterpret_cast<uint32_t*>(orow + 8 * jj + fc) = pack_bf16x2(o[4 * jj + 2 * h2] * inv, o[4 * jj + 2 * h2 + 1] * inv);
+      }
+    }
+  }
+
+  if constexpr (PAGED) {
+    if (p.kv_splits > 1) {
+      // split-KV combine: the last CTA of this (query tile, head, sequence) to arrive merges every split's partial in split order,
+      // so the result does not depend on which CTA that is (bit-deterministic)
+      __shared__ int s_last;
+      const size_t tile = (size_t)(b * p.H + h) * gridDim.x + blockIdx.x;
+      __threadfence();
+      __syncthreads();
+      if (threadIdx.x == 0) s_last = atomicAdd(p.counters + tile, 1) == p.kv_splits - 1;
+      __syncthreads();
+      if (s_last) {
+        __threadfence();
+        const float* part = p.part + tile * p.kv_splits * kAtBQ * C::PART_LD;
+        for (int idx = threadIdx.x; idx < kAtBQ * (HD / 4); idx += kAtThreads) {
+          const int r = idx / (HD / 4), d = (idx % (HD / 4)) * 4;
+          if (q0 + r >= p.Sq) continue;
+          float mx = -INFINITY;
+          for (int s = 0; s < p.kv_splits; ++s) mx = fmaxf(mx, __ldcg(part + ((size_t)s * kAtBQ + r) * C::PART_LD + HD));
+          float l = 0.f;
+          float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (mx != -INFINITY) {
+            for (int s = 0; s < p.kv_splits; ++s) {
+              const float* prow = part + ((size_t)s * kAtBQ + r) * C::PART_LD;
+              const float w = exp2f(__ldcg(prow + HD) - mx);      // 0 for a split that saw no visible key of this row
+              l += __ldcg(prow + HD + 1) * w;
+              const float4 v = __ldcg(reinterpret_cast<const float4*>(prow + d));
+              acc.x += v.x * w; acc.y += v.y * w; acc.z += v.z * w; acc.w += v.w * w;
+            }
+          }
+          const float inv = l > 0.f ? 1.f / l : 0.f;
+          bf16* orow = p.out + (size_t)(b * p.Sq + q0 + r) * p.o_stride + h * HD + d;
+          *reinterpret_cast<uint2*>(orow) = make_uint2(pack_bf16x2(acc.x * inv, acc.y * inv), pack_bf16x2(acc.z * inv, acc.w * inv));
+        }
+        if (threadIdx.x == 0) p.counters[tile] = 0;           // ready for the next launch
       }
     }
   }
@@ -234,20 +337,21 @@ static int attn_tc_init() {
       set_error("cuTensorMapEncodeTiled not available"); g_at_rc = -1; return;
     }
     g_at_encode = reinterpret_cast<PFN_encodeTiled>(fn);
-    if (cudaFuncSetAttribute(attn_prefill_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnTcCfg<64>::SMEM_BYTES) != cudaSuccess ||
-        cudaFuncSetAttribute(attn_prefill_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnTcCfg<128>::SMEM_BYTES) != cudaSuccess) {
+    if (cudaFuncSetAttribute(attn_prefill_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnTcCfg<64>::SMEM_BYTES) != cudaSuccess ||
+        cudaFuncSetAttribute(attn_prefill_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnTcCfg<128>::SMEM_BYTES) != cudaSuccess ||
+        cudaFuncSetAttribute(attn_prefill_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnTcCfg<128>::SMEM_BYTES) != cudaSuccess) {
       set_error("attention_tc: cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError())); g_at_rc = -1;
     }
   });
   return g_at_rc;
 }
 
-// rows x cols bf16 view with a row pitch of `ld` elements; boxes of 64 rows x 64 columns (128 B), 128 B swizzle
-static int attn_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld) {
+// rows x cols bf16 view with a row pitch of `ld` elements; boxes of `box_rows` (default 64) rows x 64 columns (128 B), 128 B swizzle
+static int attn_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, int box_rows = kAtBQ) {
   if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ld * 2) % 16 != 0) { set_error("attention_tc: operands must be 16 B aligned with a 16 B-multiple pitch"); return -1; }
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {ld * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)kAtBQ};
+  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = g_at_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -282,11 +386,53 @@ int attention_prefill_tc(const AttnCall& c, cudaStream_t st) {
   cfg.attrs = attr; cfg.numAttrs = na;
   if (c.HD == 64) {
     cfg.dynamicSmemBytes = AttnTcCfg<64>::SMEM_BYTES;
-    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_prefill_tc_kernel<64>, tq, tk0, tv0, tk1, tv1, p));
+    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_prefill_tc_kernel<64, false>, tq, tk0, tv0, tk1, tv1, p));
   } else {
     cfg.dynamicSmemBytes = AttnTcCfg<128>::SMEM_BYTES;
-    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_prefill_tc_kernel<128>, tq, tk0, tv0, tk1, tv1, p));
+    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_prefill_tc_kernel<128, false>, tq, tk0, tv0, tk1, tv1, p));
   }
+  return 0;
+}
+
+int attention_paged_partials() { return 3 * num_sms(); }
+
+// Split count of a paged launch: none once the grid covers the SMs; otherwise enough CTAs for two per SM, each with >= 2 key
+// tiles of the longest possible sequence.  ctas * splits < 2 * SMs + ctas < attention_paged_partials().
+static int paged_kv_splits(int ctas, int max_kv) {
+  const int sms = num_sms();
+  if (ctas >= sms) return 1;
+  const int tiles = (max_kv + kAtBKV - 1) / kAtBKV;
+  int s = std::min((2 * sms + ctas - 1) / ctas, (tiles + 1) / 2);
+  return std::max(1, std::min(s, kAtMaxKvSplits));
+}
+
+int attention_paged(const AttnPagedCall& c, cudaStream_t st) {
+  if (attn_tc_init()) return -1;
+  if (c.page_tokens < 8 || c.page_tokens > 64 || c.page_tokens % 8 != 0) { set_error("attention_paged: page_tokens %d must be a multiple of 8 <= 64", c.page_tokens); return -1; }
+  if (c.B < 1 || c.H < 1 || c.T < 1 || c.pool_pages < 1) { set_error("attention_paged: empty launch"); return -1; }
+  if ((c.o_stride % 8) != 0) { set_error("attention_paged: output pitch must keep 16 B alignment"); return -1; }
+  CUtensorMap tq, tkv;
+  if (attn_tmap(&tq, c.q, (uint64_t)c.B * c.T, (uint64_t)c.H * 128, c.q_stride)) return -1;
+  if (attn_tmap(&tkv, c.kv_pages, (uint64_t)c.pool_pages * 2 * c.H * c.page_tokens, 128, 128, c.page_tokens)) return -1;
+  const int qt = (c.T + kAtBQ - 1) / kAtBQ, ctas = qt * c.H * c.B;
+  const int splits = paged_kv_splits(ctas, c.max_kv);
+  if (splits > 1 && (c.part == nullptr || c.counters == nullptr || (int64_t)ctas * splits > attention_paged_partials())) {
+    set_error("attention_paged: split-KV scratch missing or too small"); return -1;
+  }
+  AttnTcParams p;
+  memset(&p, 0, sizeof(p));
+  p.Sq = c.T; p.H = c.H; p.sl2 = c.scale * 1.4426950408889634f; p.causal = 1; p.out = c.out; p.o_stride = c.o_stride;
+  p.page_table = c.page_table; p.pages_per_seq = c.pages_per_seq; p.page_tokens = c.page_tokens; p.base_len = c.base_len;
+  p.kv_splits = splits; p.part = c.part; p.counters = c.counters;
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(qt, c.H, c.B * splits); cfg.blockDim = dim3(kAtThreads); cfg.stream = st;
+  cfg.dynamicSmemBytes = AttnTcCfg<128>::SMEM_BYTES;
+  cudaLaunchAttribute attr[1];
+  int na = 0;
+  if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
+  cfg.attrs = attr; cfg.numAttrs = na;
+  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_prefill_tc_kernel<128, true>, tq, tkv, tkv, tkv, tkv, p));
   return 0;
 }
 

@@ -546,16 +546,30 @@ __device__ void kv_reserve_serial(int32_t* kv_free, int32_t* kv_state, int32_t* 
   kv_state[0] = top;
 }
 __global__ void kv_reserve_kernel(int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq,
-                                  int page_tokens, int B, int S, const int32_t* __restrict__ left_pad) {
+                                  int page_tokens, int B, int S, const int32_t* __restrict__ left_pad, const int32_t* __restrict__ base_len) {
   __shared__ int s_tokens[64];
-  if (threadIdx.x < B) s_tokens[threadIdx.x] = S - (left_pad ? left_pad[threadIdx.x] : 0);
+  if (threadIdx.x < B) s_tokens[threadIdx.x] = (base_len ? base_len[threadIdx.x] : 0) + S - (left_pad ? left_pad[threadIdx.x] : 0);
   __syncthreads();
   if (threadIdx.x == 0) kv_reserve_serial(kv_free, kv_state, kv_npages, page_table, pages_per_seq, page_tokens, B, s_tokens);
 }
 int kv_reserve(int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, int B, int S,
-               const int32_t* left_pad, cudaStream_t st) {
+               const int32_t* left_pad, cudaStream_t st, const int32_t* base_len) {
   if (B > 64) { set_error("kv_reserve: batch %d > 64", B); return -1; }
-  kv_reserve_kernel<<<1, 64, 0, st>>>(kv_free, kv_state, kv_npages, page_table, pages_per_seq, page_tokens, B, S, left_pad);
+  kv_reserve_kernel<<<1, 64, 0, st>>>(kv_free, kv_state, kv_npages, page_table, pages_per_seq, page_tokens, B, S, left_pad, base_len);
+  VCLA_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+struct KvLens { int32_t v[64]; };
+__global__ void kv_truncate_kernel(int32_t* seq_len, int B, const KvLens len) {
+  const int b = threadIdx.x;
+  if (b < B) seq_len[b] = min(seq_len[b], len.v[b]);
+}
+int kv_truncate(int32_t* seq_len, const int32_t* len_host, int B, cudaStream_t st) {
+  if (B < 1 || B > 64) { set_error("kv_truncate: batch %d not in 1..64", B); return -1; }
+  KvLens len;
+  for (int b = 0; b < 64; ++b) len.v[b] = b < B ? len_host[b] : 0;
+  kv_truncate_kernel<<<1, 64, 0, st>>>(seq_len, B, len);
   VCLA_CUDA_OK(cudaGetLastError());
   return 0;
 }

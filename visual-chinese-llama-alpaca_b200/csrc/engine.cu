@@ -111,6 +111,7 @@ struct vcla_ctx {
   // device-side sampling (vcla_set_sampler): replaces the argmax by the fused logits-processor chain + draw
   SamplerParams* samp_params = nullptr; float* samp_logits = nullptr; int32_t* finished = nullptr; bool samp_on = false;
   int64_t len_bound = 0;   // host-side upper bound of the cached tokens per sequence (prefill S + decode steps issued since)
+  int resident_b = 0;      // sequences resident since the last vcla_prefill (0 after vcla_reset)
   // vision activations
   bf16 *v_im2col = nullptr, *v_norm = nullptr, *v_qkv = nullptr, *v_attn = nullptr, *v_ffn = nullptr;
   float *v_hidden = nullptr, *v_postln_f32 = nullptr;
@@ -123,6 +124,7 @@ struct vcla_ctx {
   float* d_resid = nullptr; bf16 *d_xn = nullptr, *d_attn = nullptr, *d_h = nullptr;
   float *ws_qkv = nullptr, *ws_o = nullptr, *ws_gu = nullptr, *ws_d = nullptr, *ws_lm = nullptr;
   float* attn_scratch = nullptr; int32_t* attn_counters = nullptr;
+  float* pa_part = nullptr; int32_t* pa_counters = nullptr;   // split-KV partials / arrival counters of the paged prefill attention
   int32_t* d_tok = nullptr;
   int32_t *tok_hist = nullptr, *step_idx = nullptr;
   float* d_ssq = nullptr;    // [64][t_hidden / 128] row statistics of the deferred-RMSNorm decode schedule (cluster split-K)
@@ -310,6 +312,8 @@ void layout_activations(vcla_ctx* c) {
   c->ws_lm = a_alloc<float>(c, (size_t)c->sp_lm * Bp * g.t_vocab);
   c->attn_scratch = a_alloc<float>(c, (size_t)Bp * g.t_heads * 8 * (128 + 2));   // up to 8 KV splits
   c->attn_counters = a_alloc<int32_t>(c, (size_t)Bp * g.t_heads);
+  c->pa_part = a_alloc<float>(c, (size_t)attention_paged_partials() * kAttnPartialFloats);
+  c->pa_counters = a_alloc<int32_t>(c, (size_t)attention_paged_partials());
   c->d_tok = a_alloc<int32_t>(c, Bp);
   c->tok_hist = a_alloc<int32_t>(c, (size_t)(g.max_seq + 2) * Bp);
   c->step_idx = a_alloc<int32_t>(c, 16);
@@ -646,6 +650,21 @@ int vcla_reset(vcla_ctx* c, vcla_stream stream) {
   if (c->dp_step) VCLA_CUDA_OK(cudaMemsetAsync(c->dp_step, 0, 4, (cudaStream_t)stream));
   VCLA_CUDA_OK(cudaMemsetAsync(c->finished, 0, 64 * 4, (cudaStream_t)stream));
   c->len_bound = 0;
+  c->resident_b = 0;
+  return 0;
+}
+
+int vcla_kv_truncate(vcla_ctx* c, const int32_t* len_host, int B, vcla_stream stream) {
+  if (!c || !len_host) { set_error("vcla_kv_truncate: null arguments"); return -1; }
+  if (c->resident_b <= 0) { set_error("vcla_kv_truncate: no resident sequences (call vcla_prefill first)"); return -1; }
+  if (B != c->resident_b) { set_error("vcla_kv_truncate: batch %d differs from the %d resident sequences", B, c->resident_b); return -1; }
+  int64_t longest = 0;
+  for (int b = 0; b < B; ++b) {
+    if (len_host[b] < 0) { set_error("vcla_kv_truncate: negative length %d for sequence %d", len_host[b], b); return -1; }
+    longest = std::max<int64_t>(longest, len_host[b]);
+  }
+  count(c); if (kv_truncate(c->seq_len, len_host, B, (cudaStream_t)stream)) return -1;
+  c->len_bound = std::min(c->len_bound, longest);
   return 0;
 }
 
@@ -865,26 +884,13 @@ static int lm_head_last(vcla_ctx* c, int B, float* logits_dev, int32_t* tok_dev,
   return logits_argmax(c, B, logits_dev, tok_dev ? tok_dev : c->d_tok, 0, st);
 }
 
-int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, const int32_t* img_row, const int32_t* left_pad,
-                 int pos_from_mask, float* logits_all, float* last_logits, int32_t* next_tok, vcla_stream stream) {
-  cudaStream_t st = (cudaStream_t)stream;
+// The LLaMA stack over the B x S rows already embedded in c->resid.  base_len == nullptr: a whole prompt (causal attention over its
+// own rows); otherwise a chunk appended to the base_len[b] cached tokens of each sequence (RoPE positions and cache slots start at
+// base_len[b], attention reads the cached prefix from the page pool).
+static int prefill_layers(vcla_ctx* c, int B, int S, const int32_t* left_pad, int pos_from_mask, const int32_t* base_len, cudaStream_t st) {
   const vcla_config& g = c->cfg;
-  const int nq = g.r_queries, TH = g.t_hidden, F = g.t_ffn, H = g.t_heads;
-  const int S = (image_mode == VCLA_IMAGE_AT_HEAD) ? T + nq : T;
-  if (B < 1 || B > g.max_batch || B > 64) { set_error("prefill: batch %d exceeds capacity (max_batch %d, <= 64 per call)", B, g.max_batch); return -1; }
-  if ((long)B * S > g.max_prefill_tokens) { set_error("prefill: %d x %d tokens exceed max_prefill_tokens %d", B, S, g.max_prefill_tokens); return -1; }
-  if (S > g.max_seq) { set_error("prefill: sequence %d exceeds max_seq %d", S, g.max_seq); return -1; }
-  if (image_mode == VCLA_IMAGE_AT_HEAD && T < 2) { set_error("prefill: image_at_head needs >= 2 text tokens"); return -1; }
-  if (image_mode == VCLA_IMAGE_AT_HEAD && left_pad != nullptr) { set_error("prefill: left padding is not defined for the image_at_head layout"); return -1; }
+  const int TH = g.t_hidden, F = g.t_ffn, H = g.t_heads;
   const int rows = B * S;
-  if (vcla_reset(c, stream)) return -1;
-  // pages for the prompt's tokens (real tokens only: left padding is never cached)
-  count(c); if (kv_reserve(c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, B, S, left_pad, st)) return -1;
-  count(c); if (embed_tokens(ids, B, T, S, TH, c->embed, g.t_vocab, image_mode == VCLA_IMAGE_AT_HEAD ? 1 : 0, nq, c->resid, st)) return -1;
-  if (image_mode != VCLA_TEXT_ONLY) {
-    const int32_t* rs = (image_mode == VCLA_IMAGE_AT_HEAD || img_row == nullptr) ? c->img_row_default : img_row;
-    count(c); if (scatter_image_rows(c->img_embeds, B, nq, TH, rs, S, c->resid, st)) return -1;
-  }
   const float scale = 1.0f / sqrtf(128.f);
   // 5 kernels per layer: RMSNorm is deferred (operand = bf16(resid * norm_w); the row scale commutes with the GEMM and is applied in
   // the consuming GEMM's epilogue from the per-tile sums of squares the producing GEMM wrote), RoPE + KV-cache append run in the
@@ -899,11 +905,19 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
       gc.rowscale = rsc;
       gc.rope.cos = c->rope_cos; gc.rope.sin = c->rope_sin; gc.rope.kv_pages = L.kv; gc.rope.page_table = c->page_table; gc.rope.pages_per_seq = c->pages_per_seq;
       gc.rope.page_tokens = c->page_tokens; gc.rope.S = S; gc.rope.T = TH; gc.rope.H = H; gc.rope.left_pad = left_pad; gc.rope.pos_from_mask = pos_from_mask;
+      gc.rope.base_len = base_len;
       count(c); if (gemm_tc(gc, st)) return -1;
     }
-    AttnCall a; a.q = c->qkv; a.q_stride = 3 * TH; a.k0 = c->qkv + TH; a.v0 = c->qkv + 2 * TH; a.kv0_stride = 3 * TH; a.n0 = S;
-    a.out = c->attn; a.o_stride = TH; a.B = B; a.H = H; a.Sq = S; a.HD = 128; a.scale = scale; a.causal = 1; a.kv_start = left_pad;
-    count(c); if (attention_prefill(a, st)) return -1;
+    if (base_len == nullptr) {
+      AttnCall a; a.q = c->qkv; a.q_stride = 3 * TH; a.k0 = c->qkv + TH; a.v0 = c->qkv + 2 * TH; a.kv0_stride = 3 * TH; a.n0 = S;
+      a.out = c->attn; a.o_stride = TH; a.B = B; a.H = H; a.Sq = S; a.HD = 128; a.scale = scale; a.causal = 1; a.kv_start = left_pad;
+      count(c); if (attention_prefill(a, st)) return -1;
+    } else {
+      AttnPagedCall a; a.q = c->qkv; a.q_stride = 3 * TH; a.kv_pages = L.kv; a.pool_pages = c->total_pages; a.page_table = c->page_table;
+      a.pages_per_seq = c->pages_per_seq; a.page_tokens = c->page_tokens; a.base_len = base_len; a.max_kv = (int)c->len_bound + S;
+      a.out = c->attn; a.o_stride = TH; a.B = B; a.H = H; a.T = S; a.scale = scale; a.part = c->pa_part; a.counters = c->pa_counters;
+      count(c); if (attention_paged(a, st)) return -1;
+    }
     {
       GemmCall gc; gc.A = c->attn; gc.B = L.wo; gc.M = rows; gc.N = TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_ADD_F32; gc.accumulate = 1; gc.out = c->resid; gc.ldo = TH;
       gc.emit.norm_w = L.ln2; gc.emit.xw = c->xn; gc.emit.ldxw = TH; gc.emit.ssq_out = c->p_ssq;
@@ -920,15 +934,68 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
       count(c); if (gemm_tc(gc, st)) return -1;
     }
   }
+  return 0;
+}
+
+// logits of every row (optional) and of each sequence's last row (+ the argmax / sampler pick), from the final residual stream
+static int prefill_logits(vcla_ctx* c, int B, int S, float* logits_all, float* last_logits, int32_t* next_tok, cudaStream_t st) {
+  const vcla_config& g = c->cfg;
+  const int TH = g.t_hidden, rows = B * S;
   if (logits_all) {
     count(c); if (rmsnorm(c->resid, rows, TH, c->final_norm, g.t_eps, c->xn, st)) return -1;
     if (gemm_f32(c, c->xn, rows, TH, TH, c->lm_head, g.t_vocab, TH, nullptr, 0, logits_all, g.t_vocab, st)) return -1;
   }
   count(c); if (gather_last_rows(c->resid, B, S, TH, c->d_resid, st)) return -1;
-  if (lm_head_last(c, B, last_logits, next_tok, st)) return -1;
+  return lm_head_last(c, B, last_logits, next_tok, st);
+}
+
+int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, const int32_t* img_row, const int32_t* left_pad,
+                 int pos_from_mask, float* logits_all, float* last_logits, int32_t* next_tok, vcla_stream stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const vcla_config& g = c->cfg;
+  const int nq = g.r_queries, TH = g.t_hidden;
+  const int S = (image_mode == VCLA_IMAGE_AT_HEAD) ? T + nq : T;
+  if (B < 1 || B > g.max_batch || B > 64) { set_error("prefill: batch %d exceeds capacity (max_batch %d, <= 64 per call)", B, g.max_batch); return -1; }
+  if ((long)B * S > g.max_prefill_tokens) { set_error("prefill: %d x %d tokens exceed max_prefill_tokens %d", B, S, g.max_prefill_tokens); return -1; }
+  if (S > g.max_seq) { set_error("prefill: sequence %d exceeds max_seq %d", S, g.max_seq); return -1; }
+  if (image_mode == VCLA_IMAGE_AT_HEAD && T < 2) { set_error("prefill: image_at_head needs >= 2 text tokens"); return -1; }
+  if (image_mode == VCLA_IMAGE_AT_HEAD && left_pad != nullptr) { set_error("prefill: left padding is not defined for the image_at_head layout"); return -1; }
+  if (vcla_reset(c, stream)) return -1;
+  // pages for the prompt's tokens (real tokens only: left padding is never cached)
+  count(c); if (kv_reserve(c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, B, S, left_pad, st)) return -1;
+  count(c); if (embed_tokens(ids, B, T, S, TH, c->embed, g.t_vocab, image_mode == VCLA_IMAGE_AT_HEAD ? 1 : 0, nq, c->resid, st)) return -1;
+  if (image_mode != VCLA_TEXT_ONLY) {
+    const int32_t* rs = (image_mode == VCLA_IMAGE_AT_HEAD || img_row == nullptr) ? c->img_row_default : img_row;
+    count(c); if (scatter_image_rows(c->img_embeds, B, nq, TH, rs, S, c->resid, st)) return -1;
+  }
+  if (prefill_layers(c, B, S, left_pad, pos_from_mask, nullptr, st) || prefill_logits(c, B, S, logits_all, last_logits, next_tok, st)) return -1;
   // sequence lengths become S - pad; the page the first decoded token will be appended to is reserved here
   count(c); if (advance_seq(c->seq_len, B, S, left_pad, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st)) return -1;
   c->len_bound = S;
+  c->resident_b = B;
+  return 0;
+}
+
+int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* logits_all, float* last_logits, int32_t* next_tok, vcla_stream stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const vcla_config& g = c->cfg;
+  if (!ids || T < 1) { set_error("prefill_extend: no tokens"); return -1; }
+  if (c->resident_b <= 0) { set_error("prefill_extend: no resident sequences (call vcla_prefill first)"); return -1; }
+  if (B != c->resident_b) { set_error("prefill_extend: batch %d differs from the %d resident sequences", B, c->resident_b); return -1; }
+  if (c->dp_on()) { set_error("prefill_extend: not available while the data-parallel token exchange is active"); return -1; }
+  if ((long)B * T > g.max_prefill_tokens) { set_error("prefill_extend: %d x %d tokens exceed max_prefill_tokens %d", B, T, g.max_prefill_tokens); return -1; }
+  if (c->len_bound + T > g.max_seq) {
+    set_error("prefill_extend: %lld cached tokens + %d exceed the context capacity max_seq=%d", (long long)c->len_bound, T, g.max_seq);
+    return -1;
+  }
+  // like vcla_prefill: the token history, the step counter and the finished flags start over with this call's pick
+  VCLA_CUDA_OK(cudaMemsetAsync(c->step_idx, 0, 4, st));
+  VCLA_CUDA_OK(cudaMemsetAsync(c->finished, 0, 64 * 4, st));
+  count(c); if (kv_reserve(c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, B, T, nullptr, st, c->seq_len)) return -1;
+  count(c); if (embed_tokens(ids, B, T, T, g.t_hidden, c->embed, g.t_vocab, 0, g.r_queries, c->resid, st)) return -1;
+  if (prefill_layers(c, B, T, nullptr, 1, c->seq_len, st) || prefill_logits(c, B, T, logits_all, last_logits, next_tok, st)) return -1;
+  count(c); if (advance_seq(c->seq_len, B, T, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st)) return -1;
+  c->len_bound += T;
   return 0;
 }
 
@@ -1346,6 +1413,37 @@ int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v
   a.k1 = (const bf16*)k1; a.v1 = (const bf16*)v1; a.kv1_stride = kv1_stride; a.n1 = n1; a.out = (bf16*)out; a.o_stride = o_stride;
   a.B = B; a.H = H; a.Sq = Sq; a.HD = HD; a.scale = scale; a.causal = causal;
   return attention_prefill(a, (cudaStream_t)stream);
+}
+int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, const int32_t* page_table, int pages_per_seq, int page_tokens,
+                            const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T, float scale, vcla_stream stream) {
+  // operator entry for tests: the pool extent and the longest sequence are read back from the caller's table and lengths, the
+  // split-KV scratch is allocated for the call.  Synchronises.
+  if (!q || !kv_pages || !page_table || !base_len_dev || !out || B < 1 || B > 64 || H < 1 || T < 1 || pages_per_seq < 1) {
+    set_error("vcla_op_attention_paged: bad arguments"); return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<int32_t> table((size_t)B * pages_per_seq), len((size_t)B);
+  VCLA_CUDA_OK(cudaStreamSynchronize(st));
+  VCLA_CUDA_OK(cudaMemcpy(table.data(), page_table, table.size() * 4, cudaMemcpyDeviceToHost));
+  VCLA_CUDA_OK(cudaMemcpy(len.data(), base_len_dev, len.size() * 4, cudaMemcpyDeviceToHost));
+  int max_kv = 0; int64_t pool_pages = 0;
+  for (int b = 0; b < B; ++b) {
+    const int64_t kv = (int64_t)len[b] + T;
+    if (len[b] < 0 || kv > (int64_t)pages_per_seq * page_tokens) { set_error("vcla_op_attention_paged: sequence %d (%d + %d tokens) exceeds its table row", b, len[b], T); return -1; }
+    max_kv = std::max(max_kv, (int)kv);
+    for (int i = 0; i < (int)((kv + page_tokens - 1) / page_tokens); ++i) pool_pages = std::max<int64_t>(pool_pages, (int64_t)table[(size_t)b * pages_per_seq + i] + 1);
+  }
+  const int n = attention_paged_partials();
+  void* scratch = nullptr;
+  VCLA_CUDA_OK(cudaMalloc(&scratch, (size_t)n * kAttnPartialFloats * 4 + (size_t)n * 4));
+  int32_t* counters = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(scratch) + (size_t)n * kAttnPartialFloats);
+  AttnPagedCall a; a.q = (const bf16*)q; a.q_stride = q_stride; a.kv_pages = (const bf16*)kv_pages; a.pool_pages = pool_pages; a.page_table = page_table;
+  a.pages_per_seq = pages_per_seq; a.page_tokens = page_tokens; a.base_len = base_len_dev; a.max_kv = max_kv; a.out = (bf16*)out; a.o_stride = o_stride;
+  a.B = B; a.H = H; a.T = T; a.scale = scale; a.part = reinterpret_cast<float*>(scratch); a.counters = counters;
+  int rc = cudaMemsetAsync(counters, 0, (size_t)n * 4, st) == cudaSuccess ? attention_paged(a, st) : -1;
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_attention_paged: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
+  cudaFree(scratch);
+  return rc;
 }
 int vcla_op_layernorm(const float* x, int rows, int D, const float* w, const float* b, float eps, void* y_bf16, float* y_f32, vcla_stream stream) {
   return layernorm(x, rows, D, w, b, eps, (bf16*)y_bf16, y_f32, (cudaStream_t)stream);

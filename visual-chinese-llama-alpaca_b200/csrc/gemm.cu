@@ -282,9 +282,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 if (row_ok) {
                   const int bq = row / R.S, sq = row % R.S;
                   const int pad = (R.left_pad != nullptr) ? __ldg(R.left_pad + bq) : 0;
-                  const int cpos = sq - pad;                               // index inside the (compact) KV cache
+                  const int cbase = (R.base_len != nullptr) ? __ldg(R.base_len + bq) : 0;   // tokens cached before this chunk
+                  const int cpos = cbase + sq - pad;                       // index inside the (compact) KV cache
                   const bool cached = cpos >= 0;                           // padding rows are neither rotated nor cached
-                  const int pos = R.pos_from_mask ? (cpos > 0 ? cpos : 0) : sq;
+                  const int pos = R.base_len != nullptr ? cpos : (R.pos_from_mask ? (cpos > 0 ? cpos : 0) : sq);
                   int page = 0, slot = 0;
                   if (cached) { page = __ldg(R.page_table + (size_t)bq * R.pages_per_seq + cpos / R.page_tokens); slot = cpos % R.page_tokens; }
                   const float* ct = R.cos + (size_t)pos * 64;

@@ -58,6 +58,7 @@ struct GemmRope {
   bf16* kv_pages = nullptr; const int32_t* page_table = nullptr; int pages_per_seq = 0, page_tokens = 0;
   int S = 0, T = 0, H = 0;                     // rows per sequence, hidden size (= H * 128), heads
   const int32_t* left_pad = nullptr; int pos_from_mask = 0;
+  const int32_t* base_len = nullptr;           // [B] or null: row t of sequence b is token base_len[b] + t (position and cache slot)
 };
 
 struct GemmCall {
@@ -138,6 +139,26 @@ int attention_prefill_tc(const AttnCall& c, cudaStream_t st);   // wgmma: QK^T a
 int attention_prefill_mma(const AttnCall& c, cudaStream_t st);  // mma.sync m16n8k16 fallback (attention.cu)
 void attention_set_tc(int mode);                                 // 0: mma.sync everywhere, 1 (default): wgmma at head dim 128, 2: wgmma everywhere (VCLA_ATTN_TC)
 int trace_set_attention_tc(void* buf, unsigned long long cap);
+
+// Causal prefill of a chunk of T new rows per sequence over its cached prefix (head dim 128, wgmma kernel of attention_tc.cu):
+// queries q[(b*T + t)*q_stride + h*128 + d]; keys / values = the first base_len[b] + T tokens of sequence b in the layer's page
+// pool kv_pages [pool_pages][2][H][page_tokens][128], read through page_table [b][pages_per_seq] with TMA; key j is visible to row
+// t iff j <= base_len[b] + t.  max_kv (an upper bound of base_len + T) and the grid size choose the split-KV factor; a split launch
+// needs part (attention_paged_partials() x 64 x 132 floats) and counters (attention_paged_partials() int32, zeroed once).
+struct AttnPagedCall {
+  const bf16* q = nullptr; int q_stride = 0;
+  const bf16* kv_pages = nullptr; int64_t pool_pages = 0;
+  const int32_t* page_table = nullptr; int pages_per_seq = 0, page_tokens = 0;
+  const int32_t* base_len = nullptr;
+  int max_kv = 0;
+  bf16* out = nullptr; int o_stride = 0;
+  int B = 0, H = 0, T = 0;
+  float scale = 1.f;
+  float* part = nullptr; int32_t* counters = nullptr;
+};
+int attention_paged(const AttnPagedCall& c, cudaStream_t st);
+int attention_paged_partials();   // (query tile, head, sequence, split) partials a split launch may need at most
+constexpr int kAttnPartialFloats = 64 * 132;
 
 struct DecodeAttnCall {
   const float* qkv_partial = nullptr;  // [splits][ws_rows][3*T] fp32 split-K partials of the fused QKV projection
@@ -228,8 +249,11 @@ int dec_embed(const int32_t* ids, int B, int D, const bf16* table, int vocab, fl
 int kv_reset(int32_t* kv_free, const int32_t* kv_order, int32_t* kv_state, int32_t* kv_npages, int total_pages, int max_batch,
              cudaStream_t st);
 // make sure sequence b owns pages for (S - left_pad[b]) tokens, b < B; pages are handed out round-robin over the sequences
+// (base_len non-null: make sure sequence b owns pages for base_len[b] + S tokens -- a chunk appended to cached tokens)
 int kv_reserve(int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens,
-               int B, int S, const int32_t* left_pad, cudaStream_t st);
+               int B, int S, const int32_t* left_pad, cudaStream_t st, const int32_t* base_len = nullptr);
+// seq_len[b] = min(seq_len[b], len[b]) for b < B <= 64 (the pages stay owned)
+int kv_truncate(int32_t* seq_len, const int32_t* len_host, int B, cudaStream_t st);
 // seq_len[b] += by - left_pad[b] ; *step_idx += 1 ; then reserve the page the NEXT token of every sequence will be appended to
 int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, int32_t* kv_free, int32_t* kv_state,
                 int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, cudaStream_t st);

@@ -52,8 +52,10 @@ _SIGNATURES = [
     ("vcla_kv_geometry", C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("vcla_kv_read_pages", C.c_int, [_P, _P, _P, _P]),
     ("vcla_kv_debug_shuffle", C.c_int, [_P, C.c_uint32]),
+    ("vcla_kv_truncate", C.c_int, [_P, _P, C.c_int, _P]),
     ("vcla_vision_encode", C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
     ("vcla_prefill", C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P]),
+    ("vcla_prefill_extend", C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     ("vcla_decode_step", C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, _P]),
     ("vcla_decode_multi", C.c_int, [_P, _P, C.c_int, C.c_int, _P]),
     ("vcla_read_history", C.c_int, [_P, _P, C.c_int, C.c_int, _P]),
@@ -77,6 +79,8 @@ _SIGNATURES = [
     ("vcla_set_attention_tc", None, [C.c_int]),
     ("vcla_op_attention", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, C.c_int,
                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _P]),
+    ("vcla_op_attention_paged", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int,
+                                          C.c_float, _P]),
     ("vcla_op_layernorm", C.c_int, [_P, C.c_int, C.c_int, _P, _P, C.c_float, _P, _P, _P]),
     ("vcla_op_rmsnorm", C.c_int, [_P, C.c_int, C.c_int, _P, C.c_float, _P, _P]),
     ("vcla_bench_decode_gemm", C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int64), _P]),

@@ -44,6 +44,9 @@ class Engine:
         self._names = None
         self._table_cache = None
         self._dp_tok = {}
+        # bumped by every call that changes the cached sequences or the weights: a KV-cache handle (VclaKVCache) taken at one value
+        # describes the cache only while the counter still has it
+        self.session = 0
 
     # ---- lifetime ---------------------------------------------------------------------------
     def close(self):
@@ -96,6 +99,7 @@ class Engine:
             t = t.float()
         t = t.contiguous()
         on_dev = 1 if t.is_cuda else 0
+        self.session += 1
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_load_weight(self._ctx, name.encode(), N.ptr(t), _DTYPE[t.dtype], t.numel(), on_dev, self._stream()),
                     f"vcla_load_weight({name})")
@@ -123,6 +127,7 @@ class Engine:
         return out
 
     def init_synthetic(self, seed: int = 0):
+        self.session += 1
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_init_synthetic(self._ctx, seed, self._stream()), "vcla_init_synthetic")
 
@@ -153,14 +158,37 @@ class Engine:
         tok = torch.empty(B, dtype=torch.int32, device=self.device)
         rows = None if img_rows is None else img_rows.to(self.device, dtype=torch.int32).contiguous()
         pad = None if left_pad is None else left_pad.to(self.device, dtype=torch.int32).contiguous()
+        self.session += 1
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_prefill(self._ctx, N.ptr(ids), B, T, image_mode, N.ptr(rows), N.ptr(pad), 1 if pos_from_mask else 0,
                                           N.ptr(la), N.ptr(ll), N.ptr(tok), self._stream()), "vcla_prefill")
         return ll, tok, la
 
+    def extend(self, input_ids: torch.Tensor, all_logits: bool = False, last_logits: bool = True):
+        """Append the (B, T) tokens to the B sequences resident since the last prefill (vcla_prefill_extend): they attend to the
+        cached prefix, no vision work runs.  -> (last logits (B,V) or None, picked tokens (B,) int32, logits (B,T,V) or None)."""
+        ids = input_ids.to(self.device, dtype=torch.int64).contiguous()
+        B, T = ids.shape
+        la = torch.empty(B, T, self.vocab, dtype=torch.float32, device=self.device) if all_logits else None
+        ll = torch.empty(B, self.vocab, dtype=torch.float32, device=self.device) if last_logits else None
+        tok = torch.empty(B, dtype=torch.int32, device=self.device)
+        self.session += 1
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_prefill_extend(self._ctx, N.ptr(ids), B, T, N.ptr(la), N.ptr(ll), N.ptr(tok), self._stream()),
+                    "vcla_prefill_extend")
+        return ll, tok, la
+
+    def truncate(self, lengths):
+        """Keep the first min(current, lengths[b]) cached tokens of each resident sequence (vcla_kv_truncate)."""
+        n = torch.as_tensor(lengths, dtype=torch.int32).reshape(-1).contiguous()
+        self.session += 1
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_kv_truncate(self._ctx, N.ptr(n), n.numel(), self._stream()), "vcla_kv_truncate")
+
     def decode_step(self, tok_in: torch.Tensor, tok_out: torch.Tensor, logits: Optional[torch.Tensor] = None, use_graph: bool = True):
         """tok_in / tok_out: int32 CUDA tensors of shape (B,) that stay alive (and at the same address) across steps."""
         B = tok_in.shape[0]
+        self.session += 1
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_decode_step(self._ctx, N.ptr(tok_in), B, N.ptr(logits), N.ptr(tok_out), 1 if use_graph else 0,
                                               self._stream()), "vcla_decode_step")
@@ -171,6 +199,7 @@ class Engine:
         """n_steps greedy steps on the in-place int32 token buffer `tok` (B,), replayed in graphs of GRAPH_CHUNK steps."""
         B = tok.shape[0]
         left = n_steps
+        self.session += 1
         with torch.cuda.device(self.device):
             while left > 0:
                 k = self.GRAPH_CHUNK
@@ -272,6 +301,7 @@ class Engine:
         return out
 
     def reset(self):
+        self.session += 1
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_reset(self._ctx, self._stream()), "vcla_reset")
 
@@ -293,6 +323,7 @@ class Engine:
         return table, owned, int(state[0]), int(state[1])
 
     def kv_debug_shuffle(self, seed: int):
+        self.session += 1
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_kv_debug_shuffle(self._ctx, seed), "vcla_kv_debug_shuffle")
 

@@ -82,9 +82,10 @@ def _attach_image_tokens(tokenizer):
 
 def get_model_and_tokenizer_and_processor(visualcla_model=None, text_model=None, vision_model=None, lora_model=None,
                                           torch_dtype=torch.float16, default_device=None, device_map=None,
-                                          load_in_8bit=False, **engine_kwargs):
+                                          load_in_8bit=False, reuse_kv_cache=False, **engine_kwargs):
     """Same signature and return triple as the reference loader (:83-141).  `engine_kwargs` (max_batch, max_seq,
-    max_prefill_tokens) size the device arenas of the H100 engine."""
+    max_prefill_tokens) size the device arenas of the H100 engine; reuse_kv_cache=True makes chat() / chat_in_stream() keep
+    the KV cache between turns (model.reuse_kv_cache)."""
     from transformers import CLIPImageProcessor, LlamaTokenizer
     tokenizer = _attach_image_tokens(LlamaTokenizer.from_pretrained(visualcla_model or lora_model))
     if visualcla_model is not None:
@@ -107,6 +108,7 @@ def get_model_and_tokenizer_and_processor(visualcla_model=None, text_model=None,
     model.tokenizer = tokenizer
     model.image_processor = image_processor
     model.image_at_head = False
+    model.reuse_kv_cache = bool(reuse_kv_cache)
     nq = model.config.visual_resampler_config["num_query_tokens"]
     model.num_patch = nq if nq != -1 else (image_processor.size["shortest_edge"] // image_processor.patch_size) ** 2 + 1
     return model, tokenizer, image_processor
@@ -136,12 +138,30 @@ def _prepare(model, image, text, history, generation_config):
     return enc, generation_config
 
 
+def _cache_kwargs(model):
+    """With model.reuse_kv_cache, generate() gets the previous turn's KV-cache handle: the conversation so far is a prefix of
+    this turn's prompt, so only the new instruction is prefilled and the image is not encoded again.  Off by default: the
+    cached prefix's K/V came from the decode GEMMs, equal to a fresh prefill only within bf16 rounding, so a sampled reply can
+    differ from the one without reuse under the same seed."""
+    if not getattr(model, "reuse_kv_cache", False):
+        return {}
+    return dict(past_key_values=getattr(model, "_chat_kv_cache", None), return_dict_in_generate=True)
+
+
+def _keep_cache(model, outputs):
+    if not getattr(model, "reuse_kv_cache", False):
+        return outputs
+    model._chat_kv_cache = outputs.past_key_values
+    return outputs.sequences
+
+
 @torch.inference_mode()
 def chat(model, image, text: str, history=[], generation_config=None):
     """ref: modeling_utils.py:143-178 (same mutable-default `history` contract as the reference)."""
     enc, generation_config = _prepare(model, image, text, history, generation_config)
     outputs = model.generate(input_ids=enc.input_ids, attention_mask=enc.attention_mask, pixel_values=enc.pixel_values,
-                             generation_config=generation_config)
+                             generation_config=generation_config, **_cache_kwargs(model))
+    outputs = _keep_cache(model, outputs)
     response = model.tokenizer.decode(outputs[0], skip_special_tokens=True)
     history.append({"type": "response", "value": response})
     print("Response:", response)
@@ -157,13 +177,19 @@ class Stream:
 
     def __call__(self, input_ids, scores) -> bool:
         if self.callback_func is not None:
-            self.callback_func(input_ids[0])
+            try:
+                self.callback_func(input_ids[0])
+            except StopIteration:
+                # the consumer stopped listening (Iteratorize left its `with` block): end generation normally, so that
+                # generate() still returns -- with reuse_kv_cache, its cache handle records the tokens fed so far
+                return True
         return False
 
 
 class Iteratorize:
     """Run `func(callback=..., **kwargs)` on a worker thread and iterate over what it passes to the callback
-    (ref :415-472).  Leaving the `with` block stops generation at the next token."""
+    (ref :415-472).  Leaving the `with` block stops generation at the next token and waits for the worker to finish, so the
+    model is idle (and a chat turn's cache handle stored) when the block is left."""
 
     _END = object()
 
@@ -207,6 +233,8 @@ class Iteratorize:
 
     def __exit__(self, *exc):
         self._stop.set()
+        if self._thread is not threading.current_thread():
+            self._thread.join()
         clear_torch_cache()
 
 
@@ -222,8 +250,9 @@ def chat_in_stream(model, image, text: str, history=[], generation_config=None):
 
     def run(callback=None, **_):
         with torch.no_grad():
-            model.generate(input_ids=enc.input_ids, attention_mask=enc.attention_mask, pixel_values=enc.pixel_values,
-                           generation_config=gen_cfg, stopping_criteria=[Stream(callback_func=callback)])
+            out = model.generate(input_ids=enc.input_ids, attention_mask=enc.attention_mask, pixel_values=enc.pixel_values,
+                                 generation_config=gen_cfg, stopping_criteria=[Stream(callback_func=callback)], **_cache_kwargs(model))
+            _keep_cache(model, out)
 
     response, hist = "", history
     with Iteratorize(run) as stream:

@@ -14,6 +14,7 @@ import copy
 import glob
 import json
 import os
+import weakref
 from types import SimpleNamespace
 from typing import Dict, List, Optional, Union
 
@@ -75,9 +76,32 @@ class _SubModel:
         return self._model.get_output_embeddings()
 
 
+class VclaKVCache:
+    """What `generate(..., return_dict_in_generate=True).past_key_values` holds: a handle on the engine's resident KV cache, not the
+    tensors.  It records the token ids that are really in the cache (the prompt, then every token fed to a decode step -- with EOS
+    on the device that includes the pad steps run past EOS, never the last, unfed pick), the layout and a device copy of the pixels.
+    Passing it back with the whole conversation as `input_ids` (as with HF's `past_key_values`) lets generate() keep the longest
+    common prefix and prefill only the rest.  Any later prefill, decode, reset or weight change on the engine makes it stale, and a
+    stale handle simply means a full prefill."""
+
+    def __init__(self, engine, session: int, ids: Optional[torch.Tensor], mode: int, pixel_values: Optional[torch.Tensor]):
+        self._engine = weakref.ref(engine)
+        self.session = session
+        self.ids = ids                      # (L,) int64 on the CPU, or None when the cache cannot be reused (batch > 1, padding)
+        self.mode = mode
+        self.pixel_values = pixel_values
+
+    def is_current(self, engine) -> bool:
+        return self._engine() is engine and getattr(engine, "session", None) == self.session
+
+    def __len__(self):
+        return 0 if self.ids is None else int(self.ids.numel())
+
+
 class VisualCLAModel:
     config_class = VisualCLAConfig
     base_model_prefix = "visualcla"
+    reuse_kv_cache = False     # chat() / chat_in_stream(): keep the KV cache between turns (opt-in, see modeling_utils.chat)
 
     def __init__(self, config: VisualCLAConfig = None, vision_model=None, text_model=None, device=None,
                  max_batch: int = 8, max_seq: int = 1024, max_prefill_tokens: Optional[int] = None,
@@ -394,6 +418,7 @@ class VisualCLAModel:
     @torch.no_grad()
     def generate(self, input_ids=None, pixel_values=None, attention_mask=None, generation_config=None,
                  logits_processor=None, stopping_criteria=None, prefix_allowed_tokens_fn=None, synced_gpus=False, **kwargs):
+        past_key_values = kwargs.pop("past_key_values", None)
         gc = self._resolve_generation_config(generation_config, kwargs)
         if prefix_allowed_tokens_fn is not None:
             raise NotImplementedError("prefix_allowed_tokens_fn is not supported on the H100 path")
@@ -426,8 +451,31 @@ class VisualCLAModel:
         need_logits = sampling or len(processors) > 0 or bool(getattr(gc, "output_logits", False) or getattr(gc, "output_scores", False))
         crit = list(stopping_criteria) if stopping_criteria is not None else []
 
-        if mode != N.TEXT_ONLY:
+        reuse = self._plan_kv_reuse(past_key_values, input_ids, pixel_values, mode, rows, pads)
+        if mode != N.TEXT_ONLY and reuse is None:
             eng.vision_encode(pixel_values)
+
+        def start(want_last_logits):
+            """prefill the prompt, or keep the reusable cached prefix and extend it by the rest -> (last logits, first pick)"""
+            if reuse is None:
+                ll, first, _ = eng.prefill(input_ids, mode, rows, all_logits=False, last_logits=want_last_logits, left_pad=pads, pos_from_mask=True)
+            else:
+                keep, rest = reuse
+                eng.truncate([keep])
+                ll, first, _ = eng.extend(rest, all_logits=False, last_logits=want_last_logits)
+            return ll, first
+
+        def finish(result, fed, logits=None):
+            """the return value; with return_dict_in_generate also the cache handle (prompt + the tokens fed to decode steps)"""
+            if not getattr(gc, "return_dict_in_generate", False):
+                return result
+            ids = px = None
+            if B == 1 and pads is None:       # only such a cache can be reused: keep its ids and pixels, nothing otherwise
+                ids = torch.cat([input_ids[0].detach().to("cpu", torch.int64), fed[0].detach().to("cpu", torch.int64)])
+                px = None if pixel_values is None else pixel_values.detach().to(eng.device).clone()
+            cache = VclaKVCache(eng, getattr(eng, "session", 0), ids, mode, px)
+            return SimpleNamespace(sequences=result, logits=logits, scores=None, past_key_values=cache)
+
         dev = eng.device
         key = (B, need_logits)
         if key not in self._tok_buf:
@@ -442,16 +490,14 @@ class VisualCLAModel:
 
         spec = self._device_sampler_spec(gc, eos, pad, min_new, logits_processor, crit, processors)
         if spec is not None:
-            return self._generate_on_device(spec, input_ids, mode, rows, pads, B, max_new, eos, pad, gc, tok)
-        last, first_tok, _ = eng.prefill(input_ids, mode, rows, all_logits=False, last_logits=need_logits, left_pad=pads, pos_from_mask=True)
+            return self._generate_on_device(spec, start, finish, B, max_new, eos, tok)
+        last, first_tok = start(need_logits)
         if not need_logits and not eos and not crit:
             # pure greedy, fixed length: graph replays only; tokens come from the device-side history the graph appends to
             tok.copy_(first_tok)
             eng.decode_many(tok, max_new - 1)
             result = eng.read_history(B, max_new).t().to(torch.int64)
-            if getattr(gc, "return_dict_in_generate", False):
-                return SimpleNamespace(sequences=result, logits=None, scores=None)
-            return result
+            return finish(result, result[:, : max_new - 1])
         finished = torch.zeros(B, dtype=torch.bool, device=dev)
         n_done = 0
         for step in range(max_new):
@@ -503,6 +549,7 @@ class VisualCLAModel:
             if stop:
                 break
         result = out[:, :n_done]
+        fed = out[:, : n_done - 1]
         if eos:
             # cut at the step where the last sequence finished (what HF's per-step check would have produced)
             hit = torch.zeros(B, n_done, dtype=torch.bool, device=dev)
@@ -513,9 +560,7 @@ class VisualCLAModel:
             result = result[:, :keep]
             idx = torch.arange(keep, device=dev)[None, :]
             result = torch.where(idx < first[:, None], result, torch.full_like(result, pad))
-        if getattr(gc, "return_dict_in_generate", False):
-            return SimpleNamespace(sequences=result, logits=tuple(all_logits) if all_logits else None, scores=None)
-        return result
+        return finish(result, fed, tuple(all_logits) if all_logits else None)
 
     # ---- sampling / EOS on the device: one fused kernel per step inside the decode graph ---------------------
     def _device_sampler_spec(self, gc, eos, pad, min_new, extra_processors, crit, processors):
@@ -550,11 +595,11 @@ class VisualCLAModel:
         return eng.sampler_spec(do_sample=sampling, repetition_penalty=rp, no_repeat_ngram_size=ng, temperature=temperature, top_k=top_k or 0,
                                 top_p=top_p, min_new_tokens=min_new, eos_token_id=eos, pad_token_id=pad, seed=seed)
 
-    def _generate_on_device(self, spec, input_ids, mode, rows, pads, B, max_new, eos, pad, gc, tok):
+    def _generate_on_device(self, spec, start, finish, B, max_new, eos, tok):
         eng = self._engine
         eng.set_sampler(spec)
         try:
-            _, first_tok, _ = eng.prefill(input_ids, mode, rows, all_logits=False, last_logits=False, left_pad=pads, pos_from_mask=True)
+            _, first_tok = start(False)
             tok.copy_(first_tok)
             n_done = 1
             if not eos:
@@ -572,15 +617,43 @@ class VisualCLAModel:
             result = eng.read_history(B, n_done).t().to(torch.int64)
         finally:
             eng.set_sampler(None)
+        fed = result[:, : n_done - 1]
         if eos:
             hit = torch.zeros_like(result, dtype=torch.bool)
             for e in eos:
                 hit |= result == e
             first = torch.where(hit.any(1), hit.float().argmax(1) + 1, torch.full((B,), n_done, device=result.device))
             result = result[:, : int(first.max())]        # cut where the last sequence finished (HF's per-step check)
-        if getattr(gc, "return_dict_in_generate", False):
-            return SimpleNamespace(sequences=result, logits=None, scores=None)
-        return result
+        return finish(result, fed)
+
+    def _plan_kv_reuse(self, cache, input_ids, pixel_values, mode, rows, pads):
+        """-> (tokens to keep, (1, T) ids to extend by) when the KV cache `cache` describes can serve this prompt, else None (full
+        prefill).  Reuse needs one unpadded sequence, a current handle, the same placeholder / text-only layout and pixels, and a
+        longest common prefix (LCP) of the cached and the new ids that covers the image block.  The LCP decides, not an assumption
+        about tokenization: re-tokenized history often differs from the generated ids near the start of a reply."""
+        eng = self._engine
+        if not isinstance(cache, VclaKVCache) or cache.ids is None or not cache.is_current(eng):
+            return None
+        if input_ids.shape[0] != 1 or pads is not None or mode == N.IMAGE_AT_HEAD or cache.mode != mode:
+            return None
+        if (pixel_values is None) != (cache.pixel_values is None):
+            return None
+        if pixel_values is not None:
+            px = pixel_values.detach().to(cache.pixel_values.device)
+            if px.shape != cache.pixel_values.shape or px.dtype != cache.pixel_values.dtype or not torch.equal(px, cache.pixel_values):
+                return None
+        new = input_ids[0].detach().to("cpu", torch.int64)
+        old = cache.ids
+        n = min(new.numel(), old.numel())
+        diff = torch.nonzero(new[:n] != old[:n])
+        lcp = int(diff[0]) if diff.numel() else n
+        keep = lcp if lcp < new.numel() else new.numel() - 1        # the whole prompt is cached: recompute its last token
+        image_end = 0
+        if mode == N.IMAGE_PLACEHOLDER and rows is not None and int(rows[0]) >= 0:
+            image_end = int(rows[0]) + eng.nq + 1                     # <img> ... </img> stay whole
+        if keep < max(image_end, 1) or new.numel() - keep > getattr(eng, "max_prefill_tokens", new.numel()):
+            return None
+        return keep, new[keep:].unsqueeze(0)
 
     @staticmethod
     def _build_processors(gc, extra):
