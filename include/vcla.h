@@ -194,6 +194,44 @@ int vcla_read_finished(vcla_ctx* ctx, int32_t* dst_dev, int B, vcla_stream strea
 int vcla_op_sample(const float* logits_dev, int B, int V, const int32_t* history_dev, int L, const vcla_sampler* sampler,
                    int32_t* tok_dev, float* scores_out_dev, vcla_stream stream);
 
+/* ---- beam search without sampling (HF:generation/utils.py:2876-3395, the vectorised _beam_search; reached from the reference's
+ * generate(num_beams=...), models/visualcla/modeling_visualcla.py:382-391) ---------------------------------------------------------
+ * With beam mode set, vcla_prefill prefills each of its B prompts once, runs the first selection on the prompts' last logits and forks
+ * every prompt to K = num_beams rows (row b * K + j) that share the prompt's KV-cache pages; next_tok_dev (if not NULL) then receives
+ * the B * K first tokens.  vcla_decode_step / vcla_decode_multi step all B * K rows: per step one kernel per beam row (log_softmax,
+ * repetition penalty / no-repeat-ngram / min_new_tokens EOS mask on that beam's own history, + its running score, top-M of the row),
+ * one kernel per item (the item's top M = max(2, 1 + n_eos) * K candidates over K * V, stopping-criteria hits, the next K beams, the
+ * finished-hypothesis store, the early-stop heuristic) and, after the sequence lengths advance, the page-table reorder: a beam continues
+ * its parent's pages; only the partly filled page it writes next is copied, when several beams continue one parent.  All of it is
+ * captured in the decode graphs.  Refused: B * K > min(max_batch, 64), prompt + max_new_tokens > max_seq, the data-parallel exchange.
+ *   vcla_set_beam        NULL: off (argmax / sampler again).  early_stopping: 0 False, 1 True, 2 "never" (HF's three settings)
+ *   vcla_read_beams      synchronous copy to the host of the store of the B items: tokens [B][K][max_new_tokens] int32 (the first
+ *                        lengths[b][k] are valid), lengths [B][K] int32, scores [B][K] f32 (length-penalised, best first), done [B]
+ *                        int32 (HF's stopping condition holds for the item); any pointer may be NULL
+ *   vcla_beam_cow_bytes  bytes of K/V copied copy-on-write since the last reset (counted on the device); synchronises
+ *   vcla_op_beam_step    the two selection kernels on caller buffers (operator tests): logits (t == 0: B rows, the prompts; else B * K
+ *                        rows) f32 (rows, V); history [t][rows] int32; run_scores [rows] in (ignored at t == 0), [B * K] out; the store
+ *                        hyp_scores / hyp_lens / hyp_fin [B][K] and hyp_tokens [B][K][max_new_tokens] and item_state [B][2] = {heuristic
+ *                        unsatisfied, done} are initialised at t == 0 and updated; parent (the logits row each new beam continues), token
+ *                        [B * K]; cand (nullable) [B][M][2] = {k * V + v, hit} of the item's top M.  Synchronises. */
+typedef struct {
+  int num_beams;                /* 2..16 */
+  float length_penalty;
+  int early_stopping;           /* 0 False, 1 True, 2 "never" */
+  int max_new_tokens;
+  int n_eos;                    /* <= 4 */
+  int eos_token_id[4];
+  float repetition_penalty;     /* 1 = off */
+  int no_repeat_ngram_size;     /* 0 = off */
+  int min_new_tokens;
+} vcla_beam;
+int vcla_set_beam(vcla_ctx* ctx, const vcla_beam* beam_or_null);
+int vcla_read_beams(vcla_ctx* ctx, int32_t* tokens_host, int32_t* lengths_host, float* scores_host, int32_t* done_host);
+int vcla_beam_cow_bytes(vcla_ctx* ctx, int64_t* bytes, int reset);
+int vcla_op_beam_step(const float* logits_dev, int B, int V, const int32_t* history_dev, int t, const vcla_beam* beam, float* run_scores_dev,
+                      float* hyp_scores_dev, int32_t* hyp_lens_dev, int32_t* hyp_fin_dev, int32_t* hyp_tokens_dev, int32_t* item_state_dev,
+                      int32_t* parent_dev, int32_t* token_dev, int32_t* cand_dev, vcla_stream stream);
+
 /* ---- data parallel over the GPUs of one box (SURVEY.md section 8e; the reference has no DP of its own) ----------------
  * Requests are independent through the whole path, so each rank (one process + one context per GPU) runs a contiguous slice of
  * the batch and the ONLY exchange is one NCCL all-gather of the chosen token ids per decode step.  After vcla_nccl_init the
@@ -263,7 +301,8 @@ int vcla_op_rmsnorm(const float* x, int rows, int D, const float* w, float eps, 
 int vcla_bench_decode_gemm(vcla_ctx* ctx, int which, int B, int reps, float* avg_us, int64_t* weight_bytes, vcla_stream stream);
 /* Timeline trace for profiles/: when enabled, CTA (0,0,0) of every kernel appends {tag, t_entry, t_dependency_resolved, t_exit}
  * (%globaltimer, ns).  Tags: 1 swap-AB GEMM, 2 GEMM, 3 prefill attention, 4 decode attention, 5 layernorm, 6 rmsnorm, 7 rope+cache,
- * 8 resid+rmsnorm, 9 silu*mul, 10/11 logits+argmax, 12 advance, 13 embed, 14 sampler.  vcla_trace_read synchronises and clears. */
+ * 8 resid+rmsnorm, 9 silu*mul, 10/11 logits+argmax, 12 advance, 13 embed, 14 sampler, 15 beam step, 16 beam select, 17 beam page
+ * reorder, 18 beam page copy.  vcla_trace_read synchronises and clears. */
 int vcla_trace_enable(vcla_ctx* ctx, int max_events);
 int vcla_trace_read(vcla_ctx* ctx, uint64_t* dst_host, int max_events, int* n_events);
 /* enable/disable programmatic dependent launch for subsequently enqueued kernels (process-wide) */

@@ -608,6 +608,127 @@ int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_
   return 0;
 }
 
+// ---- beam search: rows continue their parents' pages (shared through the page table, copy-on-write for the page written next) ----
+// Pages are never shared across a row boundary of positions: a page covers positions [i * page_tokens, (i + 1) * page_tokens) and sits at
+// index i of every row that references it.  Rows that share page i also share every page before it (a fork copies the parent's row;
+// only pages created after it differ), so an old row's pages that no new row keeps are a suffix of its row.
+constexpr int kReorderThreads = 1024;
+__global__ void __launch_bounds__(kReorderThreads, 1)
+kv_beam_reorder_kernel(int rows_old, int rows_new, const int32_t* __restrict__ parent_row, const int32_t* __restrict__ new_tok, int32_t* seq_len,
+                       int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pps, int pt, int total_pages,
+                       int32_t* table_tmp, int32_t* history, const int32_t* __restrict__ step_idx, int32_t* copy_list,
+                       unsigned long long* cow_bytes, long long bytes_per_token) {
+  extern __shared__ uint32_t s_mark[];
+  __shared__ int s_np[64], s_len[64], s_par[64];
+  TraceScope trace(17);
+  trace.dep();
+  const int tid = threadIdx.x, words = (total_pages + 31) / 32;
+  if (tid < rows_old) { s_np[tid] = kv_npages[tid]; s_len[tid] = seq_len[tid]; }
+  if (tid < rows_new) s_par[tid] = parent_row[tid];
+  for (int i = tid; i < words; i += kReorderThreads) s_mark[i] = 0u;
+  __syncthreads();
+  for (int e = tid; e < rows_old * pps; e += kReorderThreads) if (e % pps < s_np[e / pps]) table_tmp[e] = page_table[e];
+  __syncthreads();
+  // mark every page a new row keeps
+  for (int e = tid; e < rows_new * pps; e += kReorderThreads) {
+    const int j = e / pps, i = e % pps, p = s_par[j];
+    if (i < s_np[p]) { const int pg = table_tmp[(size_t)p * pps + i]; atomicOr(&s_mark[pg >> 5], 1u << (pg & 31)); }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    // release the unkept suffix of every old row (marking a released page stops a sibling that shares it from releasing it again)
+    int top = kv_state[0];
+    for (int k = 0; k < rows_old; ++k) {
+      for (int i = s_np[k] - 1; i >= 0; --i) {
+        const int pg = table_tmp[(size_t)k * pps + i];
+        const uint32_t bit = 1u << (pg & 31);
+        if (s_mark[pg >> 5] & bit) break;
+        s_mark[pg >> 5] |= bit;
+        kv_free[top++] = pg;
+      }
+    }
+    kv_state[0] = top;
+  }
+  __syncthreads();
+  for (int e = tid; e < rows_new * pps; e += kReorderThreads) {
+    const int j = e / pps, i = e % pps, p = s_par[j];
+    if (i < s_np[p]) page_table[e] = table_tmp[(size_t)p * pps + i];
+  }
+  if (tid < rows_new) { kv_npages[tid] = s_np[s_par[tid]]; seq_len[tid] = s_len[s_par[tid]]; }
+  __syncthreads();
+  if (tid == 0) {
+    // copy-on-write of the page the next token is written to: the first row continuing a parent keeps it, the others get a copy
+    int top = kv_state[0], n = 0;
+    long long rows_copied = 0;
+    uint64_t seen = 0;
+    for (int j = 0; j < rows_new; ++j) {
+      const int p = s_par[j], L = s_len[p], pw = L / pt;
+      if (!((seen >> p) & 1ull)) { seen |= 1ull << p; continue; }
+      if (pw >= s_np[p]) continue;                       // no page for a next token (the sequence is at its capacity)
+      if (top <= 0) { kv_state[1] = 1; continue; }       // pool exhausted (unreachable: distinct pages <= rows * pages_per_seq)
+      const int fresh = kv_free[--top];
+      page_table[(size_t)j * pps + pw] = fresh;
+      copy_list[1 + 3 * n] = table_tmp[(size_t)p * pps + pw];
+      copy_list[2 + 3 * n] = fresh;
+      copy_list[3 + 3 * n] = L % pt;
+      rows_copied += L % pt;
+      ++n;
+    }
+    copy_list[0] = n;
+    kv_state[0] = top;
+    if (cow_bytes) *cow_bytes += (unsigned long long)(rows_copied * bytes_per_token);
+  }
+  // token history: columns gathered by parent, then this step's tokens as row t (one thread per history row: in place)
+  const int t = *step_idx - 1;
+  for (int pos = tid; pos < t; pos += kReorderThreads) {
+    int32_t tmp[64];
+    for (int j = 0; j < rows_new; ++j) tmp[j] = history[(size_t)pos * rows_old + s_par[j]];
+    for (int j = 0; j < rows_new; ++j) history[(size_t)pos * rows_new + j] = tmp[j];
+  }
+  if (tid < rows_new) history[(size_t)t * rows_new + tid] = new_tok[tid];
+  trace.done();
+}
+int kv_beam_reorder(int rows_old, int rows_new, const int32_t* parent_row, const int32_t* new_tok, int32_t* seq_len, int32_t* kv_free,
+                    int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, int total_pages,
+                    int32_t* table_tmp, int32_t* history, const int32_t* step_idx, int32_t* copy_list, unsigned long long* cow_bytes,
+                    long long bytes_per_token, cudaStream_t st) {
+  if (rows_old < 1 || rows_new < rows_old || rows_new > 64) { set_error("kv_beam_reorder: rows %d -> %d", rows_old, rows_new); return -1; }
+  const size_t smem = (size_t)((total_pages + 31) / 32) * 4;
+  if (smem > 200u * 1024u) { set_error("kv_beam_reorder: %d pages exceed the page bitmap", total_pages); return -1; }
+  static bool opted_in = false;        // the first call is vcla_prefill's fork, outside any graph capture
+  if (smem > 48u * 1024u && !opted_in) {
+    VCLA_CUDA_OK(cudaFuncSetAttribute(kv_beam_reorder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    opted_in = true;
+  }
+  kv_beam_reorder_kernel<<<1, kReorderThreads, smem, st>>>(rows_old, rows_new, parent_row, new_tok, seq_len, kv_free, kv_state, kv_npages, page_table,
+                                                            pages_per_seq, page_tokens, total_pages, table_tmp, history, step_idx, copy_list, cow_bytes,
+                                                            bytes_per_token);
+  VCLA_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+__global__ void kv_page_copy_kernel(bf16* kv_arena, size_t layer_elems, int heads, int pt, const int32_t* __restrict__ copy_list) {
+  TraceScope trace(18);
+  trace.dep();
+  const int e = blockIdx.x, layer = blockIdx.y;
+  if (e >= copy_list[0]) return;
+  const int src = copy_list[1 + 3 * e], dst = copy_list[2 + 3 * e], n = copy_list[3 + 3 * e];
+  const size_t page_elems = (size_t)2 * heads * pt * 128;
+  const uint4* s = reinterpret_cast<const uint4*>(kv_arena + layer * layer_elems + (size_t)src * page_elems);
+  uint4* d = reinterpret_cast<uint4*>(kv_arena + layer * layer_elems + (size_t)dst * page_elems);
+  const int per_plane = n * 16, plane_stride = pt * 16;           // 16 uint4 = one 128-wide bf16 row
+  for (int i = threadIdx.x; i < 2 * heads * per_plane; i += blockDim.x) {
+    const int plane = i / per_plane, off = i % per_plane;
+    d[(size_t)plane * plane_stride + off] = s[(size_t)plane * plane_stride + off];
+  }
+  trace.done();
+}
+int kv_page_copy(bf16* kv_arena, size_t layer_elems, int layers, int heads, int page_tokens, const int32_t* copy_list, int max_entries, cudaStream_t st) {
+  kv_page_copy_kernel<<<dim3(max_entries, layers), 256, 0, st>>>(kv_arena, layer_elems, heads, page_tokens, copy_list);
+  VCLA_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------------
 // weights: synthetic generator (bit-identical to oracle.hash_normal_bf16) and checkpoint repacking
 // ------------------------------------------------------------------------------------------------

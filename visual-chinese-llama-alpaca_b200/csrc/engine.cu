@@ -52,7 +52,7 @@ struct TextLayer {
 };
 
 struct GraphKey {
-  int B; const void* tok_in; const void* logits; const void* tok_out; int n_steps = 1; int dp = 0; int samp = 0;
+  int B; const void* tok_in; const void* logits; const void* tok_out; int n_steps = 1; int dp = 0; int samp = 0; int beam = 0;
   bool operator<(const GraphKey& o) const {
     if (B != o.B) return B < o.B;
     if (tok_in != o.tok_in) return tok_in < o.tok_in;
@@ -60,6 +60,7 @@ struct GraphKey {
     if (n_steps != o.n_steps) return n_steps < o.n_steps;
     if (dp != o.dp) return dp < o.dp;
     if (samp != o.samp) return samp < o.samp;
+    if (beam != o.beam) return beam < o.beam;
     return tok_out < o.tok_out;
   }
 };
@@ -110,6 +111,13 @@ struct vcla_ctx {
   cudaStream_t dp_stream = nullptr; cudaEvent_t dp_fork = nullptr, dp_join = nullptr; bool dp_pending = false;
   // device-side sampling (vcla_set_sampler): replaces the argmax by the fused logits-processor chain + draw
   SamplerParams* samp_params = nullptr; float* samp_logits = nullptr; int32_t* finished = nullptr; bool samp_on = false;
+  // beam search (vcla_set_beam): the beam kernels replace the argmax, and the K/V of the chosen beams are rearranged through the
+  // page table after every step (beam_K rows per batch item, sharing their parents' pages copy-on-write)
+  BeamParams* beam_params = nullptr; bool beam_on = false; int beam_K = 0, beam_max_new = 0;
+  float *beam_cand_val = nullptr, *beam_run = nullptr, *hyp_score = nullptr;
+  int32_t *beam_cand_tok = nullptr, *beam_parent = nullptr, *hyp_len = nullptr, *hyp_fin = nullptr, *hyp_tok = nullptr, *hyp_tmp = nullptr;
+  int32_t *beam_state = nullptr, *beam_copy = nullptr, *beam_table_tmp = nullptr;
+  unsigned long long* beam_cow_bytes = nullptr;
   int64_t len_bound = 0;   // host-side upper bound of the cached tokens per sequence (prefill S + decode steps issued since)
   int resident_b = 0;      // sequences resident since the last vcla_prefill (0 after vcla_reset)
   // vision activations
@@ -332,6 +340,20 @@ void layout_activations(vcla_ctx* c) {
   c->samp_params = a_alloc<SamplerParams>(c, 1);
   c->samp_logits = a_alloc<float>(c, Bp * (size_t)g.t_vocab);
   c->finished = a_alloc<int32_t>(c, Bp);
+  c->beam_params = a_alloc<BeamParams>(c, 1);
+  c->beam_cand_val = a_alloc<float>(c, Bp * kBeamMaxCand);
+  c->beam_cand_tok = a_alloc<int32_t>(c, Bp * kBeamMaxCand);
+  c->beam_run = a_alloc<float>(c, Bp);
+  c->beam_parent = a_alloc<int32_t>(c, Bp);
+  c->hyp_score = a_alloc<float>(c, Bp);
+  c->hyp_len = a_alloc<int32_t>(c, Bp);
+  c->hyp_fin = a_alloc<int32_t>(c, Bp);
+  c->hyp_tok = a_alloc<int32_t>(c, Bp * (size_t)g.max_seq);
+  c->hyp_tmp = a_alloc<int32_t>(c, Bp * (size_t)g.max_seq);
+  c->beam_state = a_alloc<int32_t>(c, Bp * 2);
+  c->beam_copy = a_alloc<int32_t>(c, 1 + 3 * Bp);
+  c->beam_table_tmp = a_alloc<int32_t>(c, (size_t)g.max_batch * c->pages_per_seq);
+  c->beam_cow_bytes = a_alloc<unsigned long long>(c, 1);
 }
 
 // Split-K factor of a decode GEMM (row tiles of 128 x `splits` work units on 2 persistent CTAs per SM).  A thin last wave is
@@ -380,6 +402,7 @@ int trace_set_all(void* buf, unsigned long long cap) {
   rc |= trace_set_attention_tc(buf, cap);
   rc |= trace_set_gemm_decode(buf, cap);
   rc |= trace_set_sampler(buf, cap);
+  rc |= trace_set_beam(buf, cap);
   rc |= trace_set_attention(buf, cap);
   rc |= trace_set_elementwise(buf, cap);
   return rc;
@@ -505,7 +528,7 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   cudaMemcpy(c->img_row_default, two.data(), two.size() * 4, cudaMemcpyHostToDevice);
   if (const char* e = getenv("VCLA_ATTN_PERSISTENT")) c->attn_persistent_mode = atoi(e);
   if (const char* e = getenv("VCLA_ATTN_PERSISTENT_GRID")) c->attn_persistent_grid = atoi(e);
-  if (rope_fill_tables(g.max_seq + 1, 128, g.rope_theta, c->rope_cos, c->rope_sin) || attention_init() || sampler_init() || vcla_reset(c, nullptr)) { vcla_destroy(c); return -1; }
+  if (rope_fill_tables(g.max_seq + 1, 128, g.rope_theta, c->rope_cos, c->rope_sin) || attention_init() || sampler_init() || beam_init() || vcla_reset(c, nullptr)) { vcla_destroy(c); return -1; }
   if (cudaDeviceSynchronize() != cudaSuccess) { set_error("vcla_create: device error %s", cudaGetErrorString(cudaGetLastError())); vcla_destroy(c); return -1; }
   *out = c;
   return 0;
@@ -859,6 +882,18 @@ static int logits_argmax(vcla_ctx* c, int B, float* logits, int32_t* tok, int fo
   const vcla_config& g = c->cfg;
   const int sp_lm = lm_splits > 0 ? lm_splits : c->sp_lm;     // 1: ws_lm already holds the reduced logits (cluster split-K lm_head)
   if (c->dp_on() && dp_wait(c, st)) return -1;            // the previous step's exchange must have read dp_send before it is rewritten
+  if (c->beam_on) {
+    // B rows: the prompts at the prefill (fork == 0; every item's beams are still its prompt), else B / K items of K beams
+    float* lg = logits ? logits : c->samp_logits;
+    const bool first = fork == 0;
+    const int R = first ? 1 : c->beam_K, items = B / R;
+    count(c, 3);
+    if (dec_logits_reduce(c->ws_lm, sp_lm, B, g.t_vocab, B, g.t_vocab, lg, g.t_vocab, c->cand_val, c->cand_idx, st)) return -1;
+    if (dec_beam_step(lg, g.t_vocab, g.t_vocab, B, c->tok_hist, c->step_idx, c->beam_params, first ? nullptr : c->beam_run, c->beam_cand_val,
+                      c->beam_cand_tok, st)) return -1;
+    return dec_beam_select(c->beam_params, items, R, g.t_vocab, c->step_idx, c->beam_cand_val, c->beam_cand_tok, c->tok_hist, c->beam_run,
+                           c->beam_parent, tok, c->hyp_score, c->hyp_len, c->hyp_fin, c->hyp_tok, c->hyp_tmp, c->cfg.max_seq, c->beam_state, nullptr, st);
+  }
   if (c->samp_on) {
     // logits -> [repetition penalty, no-repeat-ngram, temperature, top-k, top-p, draw] in one kernel; raw logits stay available
     float* lg = logits ? logits : c->samp_logits;
@@ -949,6 +984,8 @@ static int prefill_logits(vcla_ctx* c, int B, int S, float* logits_all, float* l
   return lm_head_last(c, B, last_logits, next_tok, st);
 }
 
+static int beam_reorder(vcla_ctx* c, int rows_old, int rows_new, const int32_t* tok, cudaStream_t st);
+
 int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, const int32_t* img_row, const int32_t* left_pad,
                  int pos_from_mask, float* logits_all, float* last_logits, int32_t* next_tok, vcla_stream stream) {
   cudaStream_t st = (cudaStream_t)stream;
@@ -960,6 +997,13 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
   if (S > g.max_seq) { set_error("prefill: sequence %d exceeds max_seq %d", S, g.max_seq); return -1; }
   if (image_mode == VCLA_IMAGE_AT_HEAD && T < 2) { set_error("prefill: image_at_head needs >= 2 text tokens"); return -1; }
   if (image_mode == VCLA_IMAGE_AT_HEAD && left_pad != nullptr) { set_error("prefill: left padding is not defined for the image_at_head layout"); return -1; }
+  if (c->beam_on) {
+    // each prompt is prefilled once and forked to K rows afterwards
+    const int rows = B * c->beam_K, cap = std::min(g.max_batch, 64);
+    if (rows > cap) { set_error("prefill: %d prompts x %d beams exceed %d rows (min(max_batch, 64))", B, c->beam_K, cap); return -1; }
+    if ((long)S + c->beam_max_new > g.max_seq) { set_error("prefill: prompt %d + %d new tokens exceed max_seq %d", S, c->beam_max_new, g.max_seq); return -1; }
+    if (c->dp_on()) { set_error("prefill: beam search is not available while the data-parallel token exchange is active"); return -1; }
+  }
   if (vcla_reset(c, stream)) return -1;
   // pages for the prompt's tokens (real tokens only: left padding is never cached)
   count(c); if (kv_reserve(c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, B, S, left_pad, st)) return -1;
@@ -971,8 +1015,9 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
   if (prefill_layers(c, B, S, left_pad, pos_from_mask, nullptr, st) || prefill_logits(c, B, S, logits_all, last_logits, next_tok, st)) return -1;
   // sequence lengths become S - pad; the page the first decoded token will be appended to is reserved here
   count(c); if (advance_seq(c->seq_len, B, S, left_pad, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st)) return -1;
+  if (c->beam_on && beam_reorder(c, B, B * c->beam_K, next_tok ? next_tok : c->d_tok, st)) return -1;
   c->len_bound = S;
-  c->resident_b = B;
+  c->resident_b = c->beam_on ? B * c->beam_K : B;
   return 0;
 }
 
@@ -983,6 +1028,7 @@ int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* lo
   if (c->resident_b <= 0) { set_error("prefill_extend: no resident sequences (call vcla_prefill first)"); return -1; }
   if (B != c->resident_b) { set_error("prefill_extend: batch %d differs from the %d resident sequences", B, c->resident_b); return -1; }
   if (c->dp_on()) { set_error("prefill_extend: not available while the data-parallel token exchange is active"); return -1; }
+  if (c->beam_on) { set_error("prefill_extend: not available in beam-search mode"); return -1; }
   if ((long)B * T > g.max_prefill_tokens) { set_error("prefill_extend: %d x %d tokens exceed max_prefill_tokens %d", B, T, g.max_prefill_tokens); return -1; }
   if (c->len_bound + T > g.max_seq) {
     set_error("prefill_extend: %lld cached tokens + %d exceed the context capacity max_seq=%d", (long long)c->len_bound, T, g.max_seq);
@@ -999,8 +1045,21 @@ int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* lo
   return 0;
 }
 
-static int advance_and_reserve(vcla_ctx* c, int B, cudaStream_t st) {
-  return advance_seq(c->seq_len, B, 1, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st);
+// Beam search: rows_new rows continue the rows_old rows (beam_parent, written by the select kernel) with the tokens `tok`; then the
+// copy-on-write rows of the pages written next are copied for every layer.
+static int beam_reorder(vcla_ctx* c, int rows_old, int rows_new, const int32_t* tok, cudaStream_t st) {
+  const vcla_config& g = c->cfg;
+  const long long bytes_per_token = (long long)g.t_layers * 2 * g.t_heads * 128 * (long long)sizeof(bf16);
+  count(c, 2);
+  if (kv_beam_reorder(rows_old, rows_new, c->beam_parent, tok, c->seq_len, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq,
+                      c->page_tokens, c->total_pages, c->beam_table_tmp, c->tok_hist, c->step_idx, c->beam_copy, c->beam_cow_bytes, bytes_per_token, st))
+    return -1;
+  return kv_page_copy(c->kv_arena, c->kv_layer_elems, g.t_layers, g.t_heads, c->page_tokens, c->beam_copy, rows_new, st);
+}
+
+static int advance_and_reserve(vcla_ctx* c, int B, const int32_t* tok, cudaStream_t st) {
+  if (advance_seq(c->seq_len, B, 1, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st)) return -1;
+  return c->beam_on ? beam_reorder(c, B, B, tok, st) : 0;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1025,7 +1084,7 @@ static int decode_enqueue_workspace(vcla_ctx* c, const int32_t* tok_in, int B, f
   count(c); if (dec_resid_norm(c->ws_d, c->sp_d, B, c->d_resid, B, TH, c->final_norm, g.t_eps, c->d_xn, st)) return -1;
   if (ws_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
   if (logits_argmax(c, B, logits, tok_out, 1, st)) return -1;
-  count(c); if (advance_and_reserve(c, B, st)) return -1;
+  count(c); if (advance_and_reserve(c, B, tok_out, st)) return -1;
   return 0;
 }
 
@@ -1078,7 +1137,7 @@ static int decode_enqueue_csk(vcla_ctx* c, const int32_t* tok_in, int B, float* 
   }
   if (csk_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
   if (logits_argmax(c, B, logits, tok_out, 1, st, 1)) return -1;
-  count(c); if (advance_and_reserve(c, B, st)) return -1;
+  count(c); if (advance_and_reserve(c, B, tok_out, st)) return -1;
   return 0;
 }
 
@@ -1087,7 +1146,7 @@ static int decode_enqueue(vcla_ctx* c, const int32_t* tok_in, int B, float* logi
 }
 
 static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, int n_steps, cudaStream_t st) {
-  GraphKey key{B, tok_in, logits, tok_out, n_steps, c->dp_on() ? 1 : 0, c->samp_on ? 1 : 0};
+  GraphKey key{B, tok_in, logits, tok_out, n_steps, c->dp_on() ? 1 : 0, c->samp_on ? 1 : 0, c->beam_on ? c->beam_K : 0};
   auto it = c->graphs.find(key);
   if (it == c->graphs.end()) {
     const int64_t before = c->launches;
@@ -1133,8 +1192,13 @@ static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits
 
 // Every decode step appends one token per sequence: refuse the call instead of running past the context capacity (the kernels
 // index the page table, the RoPE table and the token history by the sequence length).
-static int decode_capacity(vcla_ctx* c, int n_steps) {
+static int decode_capacity(vcla_ctx* c, int n_steps, int B) {
   if (c->len_bound <= 0) { set_error("decode: no prefilled sequences (call vcla_prefill first)"); return -1; }
+  if (c->beam_on && B != c->resident_b) {
+    // the beams of an item share pages: a step advances exactly the rows the prefill forked
+    set_error("decode: beam search steps all %d rows the prefill forked (got %d)", c->resident_b, B);
+    return -1;
+  }
   if (c->len_bound + n_steps > c->cfg.max_seq) {
     set_error("decode: %lld cached tokens + %d steps exceed the context capacity max_seq=%d", (long long)c->len_bound, n_steps, c->cfg.max_seq);
     return -1;
@@ -1146,7 +1210,7 @@ int vcla_decode_step(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, i
   cudaStream_t st = (cudaStream_t)stream;
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_in || !tok_out) { set_error("decode: null token buffers"); return -1; }
-  if (decode_capacity(c, 1)) return -1;
+  if (decode_capacity(c, 1, B)) return -1;
   if (decode_uses_csk(B) && csk_prepare(c, B)) return -1;      // occupancy queries: never inside a capture
   int rc = use_graph ? decode_graph(c, tok_in, B, logits, tok_out, 1, st) : decode_enqueue(c, tok_in, B, logits, tok_out, st);
   if (rc == 0 && !use_graph && c->dp_on()) rc = dp_wait(c, st);
@@ -1159,7 +1223,7 @@ int vcla_decode_multi(vcla_ctx* c, int32_t* tok_inout, int B, int n_steps, vcla_
   // every chosen token is appended to the device-side history): amortises the gap between consecutive graph launches.
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_inout || n_steps < 1 || n_steps > 64) { set_error("decode_multi: bad arguments"); return -1; }
-  if (decode_capacity(c, n_steps)) return -1;
+  if (decode_capacity(c, n_steps, B)) return -1;
   if (decode_uses_csk(B) && csk_prepare(c, B)) return -1;
   const int rc = decode_graph(c, tok_inout, B, nullptr, tok_inout, n_steps, (cudaStream_t)stream);
   if (rc == 0) c->len_bound += n_steps;
@@ -1219,6 +1283,102 @@ int vcla_op_sample(const float* logits_dev, int B, int V, const int32_t* history
   const int rc = dec_sample(logits_dev, V, V, B, history_dev, (const int32_t*)(scratch + sizeof(SamplerParams)), (const SamplerParams*)scratch, tok_dev, nullptr,
                             nullptr, nullptr, scores_out_dev, st);
   cudaStreamSynchronize(st);
+  cudaFree(scratch);
+  return rc;
+}
+
+// -------------------------------------------------------------------------------------------------
+// beam search
+// -------------------------------------------------------------------------------------------------
+static int beam_to_params(const vcla_beam* s, int V, BeamParams* p) {
+  if (s->num_beams < 2 || s->num_beams > kBeamMaxK) { set_error("beam: num_beams must be in 2..%d (got %d)", kBeamMaxK, s->num_beams); return -1; }
+  if (s->n_eos < 0 || s->n_eos > 4) { set_error("beam: at most 4 eos ids"); return -1; }
+  if (s->early_stopping < 0 || s->early_stopping > 2) { set_error("beam: early_stopping must be 0 (False), 1 (True) or 2 (\"never\")"); return -1; }
+  if (s->max_new_tokens < 1) { set_error("beam: max_new_tokens must be >= 1"); return -1; }
+  if (!(s->repetition_penalty > 0.f)) { set_error("beam: repetition_penalty must be > 0"); return -1; }
+  memset(p, 0, sizeof(*p));
+  p->K = s->num_beams;
+  p->M = std::max(2, 1 + s->n_eos) * s->num_beams;
+  if (p->M > V) { set_error("beam: %d candidates per step exceed the vocabulary %d", p->M, V); return -1; }
+  p->n_eos = s->n_eos;
+  for (int i = 0; i < s->n_eos; ++i) p->eos[i] = s->eos_token_id[i];
+  p->length_penalty = s->length_penalty; p->early_stopping = s->early_stopping; p->max_new = s->max_new_tokens;
+  p->rep_penalty = s->repetition_penalty; p->no_repeat_ngram = s->no_repeat_ngram_size > 0 ? s->no_repeat_ngram_size : 0;
+  p->min_new_tokens = s->min_new_tokens;
+  return 0;
+}
+
+int vcla_set_beam(vcla_ctx* c, const vcla_beam* s) {
+  if (!c) return -1;
+  if (s == nullptr) { c->beam_on = false; c->beam_K = 0; return 0; }
+  if (!beam_supported(c->cfg.t_vocab)) { set_error("beam: vocabulary %d does not fit the beam-step kernel", c->cfg.t_vocab); return -1; }
+  if (c->dp_on()) { set_error("beam: not available while the data-parallel token exchange is active"); return -1; }
+  BeamParams p;
+  if (beam_to_params(s, c->cfg.t_vocab, &p)) return -1;
+  if (p.K > std::min(c->cfg.max_batch, 64)) { set_error("beam: %d beams exceed min(max_batch, 64) = %d rows", p.K, std::min(c->cfg.max_batch, 64)); return -1; }
+  if (p.max_new > c->cfg.max_seq) { set_error("beam: max_new_tokens %d exceeds max_seq %d", p.max_new, c->cfg.max_seq); return -1; }
+  VCLA_CUDA_OK(cudaMemcpy(c->beam_params, &p, sizeof(p), cudaMemcpyHostToDevice));
+  c->beam_on = true; c->beam_K = p.K; c->beam_max_new = p.max_new;
+  return 0;
+}
+
+int vcla_read_beams(vcla_ctx* c, int32_t* tokens_host, int32_t* lengths_host, float* scores_host, int32_t* done_host) {
+  if (!c || !c->beam_on || c->resident_b <= 0) { set_error("vcla_read_beams: no beam search is resident (vcla_set_beam, then vcla_prefill)"); return -1; }
+  const int K = c->beam_K, items = c->resident_b / K, cap = c->cfg.max_seq;
+  VCLA_CUDA_OK(cudaDeviceSynchronize());
+  if (tokens_host) {
+    VCLA_CUDA_OK(cudaMemcpy2D(tokens_host, (size_t)c->beam_max_new * 4, c->hyp_tok, (size_t)cap * 4, (size_t)c->beam_max_new * 4, (size_t)items * K,
+                              cudaMemcpyDeviceToHost));
+  }
+  if (lengths_host) VCLA_CUDA_OK(cudaMemcpy(lengths_host, c->hyp_len, (size_t)items * K * 4, cudaMemcpyDeviceToHost));
+  if (scores_host) VCLA_CUDA_OK(cudaMemcpy(scores_host, c->hyp_score, (size_t)items * K * 4, cudaMemcpyDeviceToHost));
+  if (done_host) {
+    std::vector<int32_t> st((size_t)items * 2);
+    VCLA_CUDA_OK(cudaMemcpy(st.data(), c->beam_state, st.size() * 4, cudaMemcpyDeviceToHost));
+    for (int b = 0; b < items; ++b) done_host[b] = st[(size_t)b * 2 + 1];
+  }
+  return 0;
+}
+
+int vcla_beam_cow_bytes(vcla_ctx* c, int64_t* bytes, int reset) {
+  if (!c) return -1;
+  unsigned long long v = 0;
+  VCLA_CUDA_OK(cudaDeviceSynchronize());
+  VCLA_CUDA_OK(cudaMemcpy(&v, c->beam_cow_bytes, 8, cudaMemcpyDeviceToHost));
+  if (bytes) *bytes = (int64_t)v;
+  if (reset) VCLA_CUDA_OK(cudaMemset(c->beam_cow_bytes, 0, 8));
+  return 0;
+}
+
+int vcla_op_beam_step(const float* logits_dev, int B, int V, const int32_t* history_dev, int t, const vcla_beam* beam, float* run_scores_dev,
+                      float* hyp_scores_dev, int32_t* hyp_lens_dev, int32_t* hyp_fin_dev, int32_t* hyp_tokens_dev, int32_t* item_state_dev,
+                      int32_t* parent_dev, int32_t* token_dev, int32_t* cand_dev, vcla_stream stream) {
+  if (!logits_dev || !beam || B < 1 || V < 1 || t < 0 || (t > 0 && !history_dev) || !run_scores_dev || !hyp_scores_dev || !hyp_lens_dev ||
+      !hyp_fin_dev || !hyp_tokens_dev || !item_state_dev || !parent_dev || !token_dev) {
+    set_error("vcla_op_beam_step: bad arguments"); return -1;
+  }
+  BeamParams p;
+  if (beam_to_params(beam, V, &p) || beam_init()) return -1;
+  if (B * p.K > 64) { set_error("vcla_op_beam_step: %d x %d rows exceed 64", B, p.K); return -1; }
+  if (t >= p.max_new) { set_error("vcla_op_beam_step: step %d is past max_new_tokens %d", t, p.max_new); return -1; }
+  const int R = t == 0 ? 1 : p.K, rows = B * R;
+  const size_t n_cand = (size_t)rows * p.M, n_tmp = (size_t)B * p.K * p.max_new;
+  uint8_t* scratch = nullptr;
+  VCLA_CUDA_OK(cudaMalloc(&scratch, 256 + n_cand * 8 + n_tmp * 4));
+  BeamParams* pd = reinterpret_cast<BeamParams*>(scratch);
+  int32_t* step = reinterpret_cast<int32_t*>(scratch + 128);
+  float* cv = reinterpret_cast<float*>(scratch + 256);
+  int32_t* ct = reinterpret_cast<int32_t*>(cv + n_cand);
+  int32_t* tmp = ct + n_cand;
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = 0;
+  if (cudaMemcpyAsync(pd, &p, sizeof(p), cudaMemcpyHostToDevice, st) != cudaSuccess || cudaMemcpyAsync(step, &t, 4, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+    set_error("vcla_op_beam_step: upload failed"); rc = -1;
+  }
+  if (rc == 0) rc = dec_beam_step(logits_dev, V, V, rows, history_dev, step, pd, t == 0 ? nullptr : run_scores_dev, cv, ct, st);
+  if (rc == 0) rc = dec_beam_select(pd, B, R, V, step, cv, ct, history_dev, run_scores_dev, parent_dev, token_dev, hyp_scores_dev, hyp_lens_dev, hyp_fin_dev,
+                                    hyp_tokens_dev, tmp, p.max_new, item_state_dev, cand_dev, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_beam_step: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
   cudaFree(scratch);
   return rc;
 }

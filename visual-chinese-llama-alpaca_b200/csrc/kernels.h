@@ -238,6 +238,27 @@ int sampler_init();
 int dec_sample(const float* logits, int ld, int V, int B, const int32_t* history, const int32_t* step_idx, const SamplerParams* params_dev,
                int32_t* tok, int32_t* history_out, int32_t* dp_send, int32_t* finished, float* scores_out, cudaStream_t st);
 int dp_unpack(const int32_t* recv, int n, int32_t* hist, int32_t* dp_step, cudaStream_t st);
+// ---- beam search (beam.cu; HF:generation/utils.py:2876-3395 with decoder_prompt_len = 0) ---------------------------------------
+constexpr int kBeamMaxK = 16;
+constexpr int kBeamMaxCand = 5 * kBeamMaxK;   // M = max(2, 1 + n_eos) * K candidates per item, n_eos <= 4
+struct BeamParams {        // lives in device memory, like SamplerParams
+  int K, M;                // beams per item, candidates kept per step
+  int n_eos; int eos[4];
+  float length_penalty;
+  int early_stopping;      // 0: False, 1: True, 2: "never"
+  int max_new;             // max_new_tokens (MaxLengthCriteria)
+  float rep_penalty; int no_repeat_ngram; int min_new_tokens;
+};
+int beam_supported(int V);
+int beam_init();
+// rows beams: log_softmax + history processors + running score (null: 0) -> the row's top-M (score desc, token asc)
+int dec_beam_step(const float* logits, int ld, int V, int rows, const int32_t* history, const int32_t* step_idx, const BeamParams* params_dev,
+                  const float* run_score, float* cand_val, int32_t* cand_tok, cudaStream_t st);
+// per item: global top-M of the R rows' candidates, next K running beams (parent_row / tok / run_score of slot b*K+j), store + flags
+int dec_beam_select(const BeamParams* params_dev, int items, int R, int V, const int32_t* step_idx, const float* cand_val, const int32_t* cand_tok,
+                    const int32_t* history, float* run_score, int32_t* parent_row, int32_t* tok, float* hyp_score, int32_t* hyp_len, int32_t* hyp_fin,
+                    int32_t* hyp_tok, int32_t* hyp_tmp, int hyp_cap, int32_t* item_state, int32_t* cand_out, cudaStream_t st);
+int trace_set_beam(void* buf, unsigned long long cap);
 // decode step entry of the cluster split-K schedule: resid[b,:] = table[ids[b]] ; xw = bf16(resid * norm_w) ;
 // ssq[b][0] = sum resid^2, ssq[b][1..slots) = 0 (head of the deferred-norm chain)
 int dec_embed(const int32_t* ids, int B, int D, const bf16* table, int vocab, float* resid, const float* norm_w,
@@ -257,6 +278,20 @@ int kv_truncate(int32_t* seq_len, const int32_t* len_host, int B, cudaStream_t s
 // seq_len[b] += by - left_pad[b] ; *step_idx += 1 ; then reserve the page the NEXT token of every sequence will be appended to
 int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, int32_t* kv_free, int32_t* kv_state,
                 int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, cudaStream_t st);
+// Beam reorder, after advance_seq (so every old row's write position seq_len and its page exist).  New row j (< rows_new) continues
+// old row parent_row[j] (< rows_old): its table row, page count and length are the parent's.  Pages no new row references go back on
+// the free stack; when several rows continue one parent, every one but the first gets a fresh page for the write position plus a
+// copy-list entry {src page, dst page, rows [0, seq_len % page_tokens)} (copy_list[0] = count, then 3 ints per entry).  The token
+// history [t][rows_old] (t = *step_idx - 1) is gathered into [t][rows_new] and new_tok is appended as its row t.  One CTA; the stack
+// operations are serial, so the result is deterministic.  Scratch: table_tmp [rows_old][pages_per_seq], mark (total_pages / 32 words
+// of dynamic shared memory).  cow_bytes (nullable) accumulates copied rows * bytes_per_token.
+int kv_beam_reorder(int rows_old, int rows_new, const int32_t* parent_row, const int32_t* new_tok, int32_t* seq_len, int32_t* kv_free,
+                    int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, int total_pages,
+                    int32_t* table_tmp, int32_t* history, const int32_t* step_idx, int32_t* copy_list, unsigned long long* cow_bytes,
+                    long long bytes_per_token, cudaStream_t st);
+// copies the copy list's rows of every layer (K and V, every head) from src to dst page; fixed grid (max_entries x layers)
+int kv_page_copy(bf16* kv_arena, size_t layer_elems, int layers, int heads, int page_tokens, const int32_t* copy_list, int max_entries,
+                 cudaStream_t st);
 // fp32 RoPE tables [max_pos][head_dim/2], computed on the host the way HF does and uploaded to cos_dev / sin_dev
 int rope_fill_tables(int max_pos, int head_dim, float theta, float* cos_dev, float* sin_dev);
 

@@ -12,19 +12,13 @@
 //   TopPLogitsWarper                  ascending cumulative softmax <= 1 - top_p removed; the largest is always kept
 //   multinomial                       inverse-CDF draw with a Philox4x32-10 uniform keyed by (seed, step, sequence)
 // With inputs_embeds the processors only ever see the NEW tokens (HF starts input_ids empty), i.e. the device token history.
-#include "common.cuh"
 #include "kernels.h"
+#include "logits_chain.cuh"
 
 namespace vcla {
 
 constexpr int kSampThreads = 1024;
 constexpr int kSampMaxKeep = 1024;   // candidates surviving top-k (k plus ties at the k-th value)
-
-__device__ __forceinline__ uint32_t order_key(float x) {   // monotone: a < b  <=>  key(a) < key(b)  (NaN sorts below everything)
-  if (x != x) return 0u;
-  const uint32_t u = __float_as_uint(x);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 
 // Philox4x32-10 (Salmon et al. 2011), counter = (step, sequence, 0, 0), key = seed
 __device__ __forceinline__ float philox_uniform(unsigned long long seed, uint32_t c0, uint32_t c1) {
@@ -39,16 +33,6 @@ __device__ __forceinline__ float philox_uniform(unsigned long long seed, uint32_
     k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
   }
   return (float)(ctr[0] >> 8) * (1.0f / 16777216.0f);   // [0, 1)
-}
-
-__device__ __forceinline__ int block_count(int local, int* s_cnt) {
-  const int w = __reduce_add_sync(0xffffffffu, local);
-  __syncthreads();
-  if (threadIdx.x == 0) *s_cnt = 0;
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0 && w) atomicAdd(s_cnt, w);
-  __syncthreads();
-  return *s_cnt;
 }
 
 __global__ void __launch_bounds__(kSampThreads, 1)
@@ -82,36 +66,7 @@ dec_sample_kernel(const float* __restrict__ logits, int ld, int V, int B, const 
   if (tid == 0) { s_n = 0; s_choice = 0; s_keep = 0; s_thr = 0xFFFFFFFFu; }
   __syncthreads();
 
-  // ---- repetition penalty: once per distinct token of the history
-  if (p.rep_penalty != 1.0f) {
-    for (int i = tid; i < L; i += kSampThreads) {
-      const int t = history[(size_t)i * B + b];
-      if (t >= 0 && t < V) {
-        const uint32_t bit = 1u << (t & 31);
-        const uint32_t old = atomicOr(&s_seen[t >> 5], bit);
-        if (!(old & bit)) {
-          const float x = s_row[t];
-          s_row[t] = x < 0.f ? x * p.rep_penalty : __fdiv_rn(x, p.rep_penalty);
-        }
-      }
-    }
-    __syncthreads();
-  }
-  // ---- no-repeat-ngram: windows [i, i+n) of the history whose first n-1 tokens equal the last n-1 tokens ban their last token
-  const int n = p.no_repeat_ngram;
-  if (n > 0 && L + 1 >= n) {
-    for (int i = tid; i + n <= L; i += kSampThreads) {
-      bool same = true;
-      for (int j = 0; j < n - 1 && same; ++j) same = history[(size_t)(i + j) * B + b] == history[(size_t)(L - n + 1 + j) * B + b];
-      if (same) {
-        const int t = history[(size_t)(i + n - 1) * B + b];
-        if (t >= 0 && t < V) s_row[t] = NEG_INF;
-      }
-    }
-    __syncthreads();
-  }
-  if (tid < p.n_eos && L < p.min_new_tokens) { const int e = p.eos[tid]; if (e >= 0 && e < V) s_row[e] = NEG_INF; }
-  __syncthreads();
+  history_processors<kSampThreads>(s_row, s_seen, V, history, B, b, L, p.rep_penalty, p.no_repeat_ngram, p.n_eos, p.eos, p.min_new_tokens);
 
   int chosen = 0;
   if (!p.do_sample) {
@@ -141,55 +96,9 @@ dec_sample_kernel(const float* __restrict__ logits, int ld, int V, int B, const 
       for (int v = tid; v < V; v += kSampThreads) s_row[v] = __fdiv_rn(s_row[v], p.temperature);
       __syncthreads();
     }
-    // ---- top-k threshold = the k-th largest key.  Two levels instead of 32 counting passes over the whole row:
-    //  (1) T1 = the k-th largest of the 1024 per-thread maxima (bit search with __syncthreads_count: one barrier per bit).  At least
-    //      k elements are >= T1, so the k-th largest element of the row is >= T1: every top-k element survives the pre-filter.
-    //  (2) the (few) elements >= T1 are collected and the exact k-th largest is found among them.
-    // If the pre-filter keeps more than the candidate buffer holds (a row full of ties), the exact bit search over the row runs.
+    // ---- top-k threshold = the k-th largest key
     const int k = p.top_k < V ? p.top_k : V;
-    uint32_t my_max = 0u;
-    for (int v = tid; v < V; v += kSampThreads) { const uint32_t key = order_key(s_row[v]); my_max = key > my_max ? key : my_max; }
-    uint32_t T = 0u;
-    if (k <= kSampThreads) {
-      for (int bit = 31; bit >= 0; --bit) {
-        const uint32_t cand = T | (1u << bit);
-        if (__syncthreads_count(my_max >= cand) >= k) T = cand;
-      }
-      int c1 = 0;
-      for (int v = tid; v < V; v += kSampThreads) c1 += order_key(s_row[v]) >= T;
-      const int n1 = block_count(c1, &s_cnt);
-      if (n1 <= kSampMaxKeep) {
-        // exact k-th largest among the n1 pre-filtered elements (rank by counting)
-        for (int v = tid; v < V; v += kSampThreads) {
-          const float x = s_row[v];
-          if (order_key(x) >= T) { const int pos = atomicAdd(&s_n, 1); s_val[pos] = x; s_idx[pos] = v; }
-        }
-        __syncthreads();
-        if (tid < n1) {
-          const uint32_t kx = order_key(s_val[tid]);
-          int greater = 0;
-          for (int j = 0; j < n1; ++j) greater += order_key(s_val[j]) > kx;
-          // the k-th largest value is the smallest key that still has fewer than k strictly greater elements
-          if (greater < k) atomicMin(&s_thr, kx);
-        }
-        __syncthreads();
-        T = s_thr;
-        __syncthreads();
-        if (tid == 0) { s_n = 0; }
-        __syncthreads();
-      } else {
-        T = 0u;
-      }
-    }
-    if (T == 0u) {
-      // exact bit search over the whole row: largest T with count(key >= T) >= k
-      for (int bit = 31; bit >= 0; --bit) {
-        const uint32_t cand = T | (1u << bit);
-        int c = 0;
-        for (int v = tid; v < V; v += kSampThreads) c += order_key(s_row[v]) >= cand;
-        if (block_count(c, &s_cnt) >= k) T = cand;
-      }
-    }
+    const uint32_t T = topk_threshold<kSampThreads, kSampMaxKeep>(s_row, V, k, s_val, s_idx, &s_cnt, &s_n, &s_thr);
     // ---- candidates (k plus ties), sorted by (value desc, index asc)
     for (int v = tid; v < V; v += kSampThreads) {
       const float x = s_row[v];

@@ -28,6 +28,12 @@ class VclaSampler(C.Structure):
                 ("pad_token_id", C.c_int), ("seed", C.c_uint64)]
 
 
+class VclaBeam(C.Structure):
+    _fields_ = [("num_beams", C.c_int), ("length_penalty", C.c_float), ("early_stopping", C.c_int), ("max_new_tokens", C.c_int),
+                ("n_eos", C.c_int), ("eos_token_id", C.c_int * 4), ("repetition_penalty", C.c_float), ("no_repeat_ngram_size", C.c_int),
+                ("min_new_tokens", C.c_int)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -63,6 +69,10 @@ _SIGNATURES = [
     ("vcla_set_sampler", C.c_int, [_P, C.POINTER(VclaSampler), _P]),
     ("vcla_read_finished", C.c_int, [_P, _P, C.c_int, _P]),
     ("vcla_op_sample", C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, C.POINTER(VclaSampler), _P, _P, _P]),
+    ("vcla_set_beam", C.c_int, [_P, C.POINTER(VclaBeam)]),
+    ("vcla_read_beams", C.c_int, [_P, _P, _P, _P, _P]),
+    ("vcla_beam_cow_bytes", C.c_int, [_P, C.POINTER(C.c_int64), C.c_int]),
+    ("vcla_op_beam_step", C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, C.POINTER(VclaBeam), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     ("vcla_nccl_unique_id", C.c_int, [_P]),
     ("vcla_nccl_init", C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int]),
     ("vcla_allgather_tokens", C.c_int, [_P, _P, C.c_int, _P, _P]),

@@ -155,7 +155,7 @@ class Engine:
         S = T + self.nq if image_mode == N.IMAGE_AT_HEAD else T
         la = torch.empty(B, S, self.vocab, dtype=torch.float32, device=self.device) if all_logits else None
         ll = torch.empty(B, self.vocab, dtype=torch.float32, device=self.device) if last_logits else None
-        tok = torch.empty(B, dtype=torch.int32, device=self.device)
+        tok = torch.empty(B * (self._beam.num_beams if self._beam is not None else 1), dtype=torch.int32, device=self.device)
         rows = None if img_rows is None else img_rows.to(self.device, dtype=torch.int32).contiguous()
         pad = None if left_pad is None else left_pad.to(self.device, dtype=torch.int32).contiguous()
         self.session += 1
@@ -292,6 +292,72 @@ class Engine:
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_op_sample(N.ptr(lg), B, V, N.ptr(hist), L, C.byref(spec), N.ptr(tok), N.ptr(scores), self._stream()), "vcla_op_sample")
         return tok, scores
+
+    # ---- beam search (include/vcla.h, "beam search") --------------------------------------------------------
+    _beam = None
+
+    @staticmethod
+    def beam_spec(num_beams, max_new_tokens, length_penalty=1.0, early_stopping=False, eos_token_id=(), repetition_penalty=1.0,
+                  no_repeat_ngram_size=0, min_new_tokens=0) -> "N.VclaBeam":
+        eos = list(eos_token_id)
+        es = 2 if early_stopping == "never" else (1 if early_stopping is True else 0)
+        arr = (C.c_int * 4)(*(eos + [0] * (4 - len(eos)))[:4])
+        return N.VclaBeam(int(num_beams), float(length_penalty), es, int(max_new_tokens), len(eos), arr, float(repetition_penalty),
+                          int(no_repeat_ngram_size or 0), int(min_new_tokens or 0))
+
+    def set_beam(self, spec: Optional["N.VclaBeam"]):
+        """spec = beam_spec(...): prefill forks every prompt to num_beams rows and decode steps run the beam kernels; None: off."""
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_set_beam(self._ctx, C.byref(spec) if spec is not None else None), "vcla_set_beam")
+        self._beam = spec
+
+    def read_beams(self, items: int):
+        """-> (tokens (items, K, max_new) int32, lengths (items, K), scores (items, K) f32, done (items,)) host tensors: the finished-
+        hypothesis store of the resident beam search, best first."""
+        K, n = self._beam.num_beams, self._beam.max_new_tokens
+        tok = torch.zeros(items, K, n, dtype=torch.int32)
+        lens = torch.zeros(items, K, dtype=torch.int32)
+        scores = torch.zeros(items, K, dtype=torch.float32)
+        done = torch.zeros(items, dtype=torch.int32)
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_read_beams(self._ctx, N.ptr(tok), N.ptr(lens), N.ptr(scores), N.ptr(done)), "vcla_read_beams")
+        return tok, lens, scores, done
+
+    def read_beam_done(self, items: int) -> torch.Tensor:
+        done = torch.zeros(items, dtype=torch.int32)
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_read_beams(self._ctx, None, None, None, N.ptr(done)), "vcla_read_beams")
+        return done
+
+    def beam_cow_bytes(self, reset: bool = False) -> int:
+        v = C.c_int64()
+        N.check(self.lib.vcla_beam_cow_bytes(self._ctx, C.byref(v), 1 if reset else 0), "vcla_beam_cow_bytes")
+        return v.value
+
+    def op_beam_step(self, logits: torch.Tensor, history: Optional[torch.Tensor], t: int, spec: "N.VclaBeam", state: dict) -> dict:
+        """The two beam-selection kernels on caller data.  logits (rows, V) f32 (t == 0: the B prompts, else B * K beams); history
+        (rows, t) tokens; state: dict of CUDA tensors run (B*K,) f32, scores (B,K) f32, lens / fin (B,K) int32, tokens (B,K,max_new)
+        int32, items (B,2) int32 -- created by the call at t == 0, updated in place.  -> {parent, token (B*K,), cand (B,M,2)}."""
+        lg = logits.to(self.device, torch.float32).contiguous()
+        rows, V = lg.shape
+        K, n = spec.num_beams, spec.max_new_tokens
+        B = rows if t == 0 else rows // K
+        M = max(2, 1 + spec.n_eos) * K
+        dev = self.device
+        if t == 0:
+            state.update(run=torch.zeros(B * K, dtype=torch.float32, device=dev), scores=torch.zeros(B, K, dtype=torch.float32, device=dev),
+                         lens=torch.zeros(B, K, dtype=torch.int32, device=dev), fin=torch.zeros(B, K, dtype=torch.int32, device=dev),
+                         tokens=torch.zeros(B, K, n, dtype=torch.int32, device=dev), items=torch.zeros(B, 2, dtype=torch.int32, device=dev))
+        hist = None if t == 0 else history.to(dev, torch.int32).t().contiguous()      # kernel layout: [t][rows]
+        parent = torch.empty(B * K, dtype=torch.int32, device=dev)
+        token = torch.empty(B * K, dtype=torch.int32, device=dev)
+        cand = torch.empty(B, M, 2, dtype=torch.int32, device=dev)
+        s = state
+        with torch.cuda.device(dev):
+            N.check(self.lib.vcla_op_beam_step(N.ptr(lg), B, V, N.ptr(hist), t, C.byref(spec), N.ptr(s["run"]), N.ptr(s["scores"]), N.ptr(s["lens"]),
+                                               N.ptr(s["fin"]), N.ptr(s["tokens"]), N.ptr(s["items"]), N.ptr(parent), N.ptr(token), N.ptr(cand),
+                                               self._stream()), "vcla_op_beam_step")
+        return dict(parent=parent, token=token, cand=cand)
 
     def read_history(self, B: int, n_steps: int) -> torch.Tensor:
         """(n_steps, B) int32 CUDA tensor: tokens chosen by the prefill (row 0) and each decode step since."""

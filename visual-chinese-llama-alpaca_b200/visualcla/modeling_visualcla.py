@@ -404,8 +404,12 @@ class VisualCLAModel:
                 setattr(gc, k, unused.pop(k))
         if unused:
             raise ValueError(f"generate(): unsupported arguments {sorted(unused)}")
-        if getattr(gc, "num_beams", 1) not in (None, 1) or getattr(gc, "num_return_sequences", 1) not in (None, 1):
-            raise NotImplementedError("beam search / num_return_sequences > 1 are not on the H100 path")
+        beams = getattr(gc, "num_beams", 1) or 1
+        nrs = getattr(gc, "num_return_sequences", 1) or 1
+        if beams > 1 and nrs > beams:
+            raise ValueError(f"`num_return_sequences` ({nrs}) has to be smaller or equal to `num_beams` ({beams}).")
+        if beams == 1 and nrs != 1:
+            raise NotImplementedError("num_return_sequences > 1 without beam search is not on the H100 path")
         return gc
 
     @staticmethod
@@ -419,9 +423,13 @@ class VisualCLAModel:
     def generate(self, input_ids=None, pixel_values=None, attention_mask=None, generation_config=None,
                  logits_processor=None, stopping_criteria=None, prefix_allowed_tokens_fn=None, synced_gpus=False, **kwargs):
         past_key_values = kwargs.pop("past_key_values", None)
+        beam_request = (kwargs.get("num_beams") or getattr(generation_config, "num_beams", 1) or 1) > 1
+        streamer = kwargs.pop("streamer", None) if beam_request else None
         gc = self._resolve_generation_config(generation_config, kwargs)
         if prefix_allowed_tokens_fn is not None:
             raise NotImplementedError("prefix_allowed_tokens_fn is not supported on the H100 path")
+        if (getattr(gc, "num_beams", 1) or 1) > 1:
+            return self._generate_beams(gc, input_ids, pixel_values, attention_mask, logits_processor, stopping_criteria, streamer)
         eng = self._engine
         B = input_ids.shape[0]
         if B > eng.max_batch:
@@ -625,6 +633,89 @@ class VisualCLAModel:
             first = torch.where(hit.any(1), hit.float().argmax(1) + 1, torch.full((B,), n_done, device=result.device))
             result = result[:, : int(first.max())]        # cut where the last sequence finished (HF's per-step check)
         return finish(result, fed)
+
+    # ---- beam search: the beam kernels and copy-on-write KV pages inside the decode graphs -------------------------------------
+    def _generate_beams(self, gc, input_ids, pixel_values, attention_mask, logits_processor, stopping_criteria, streamer):
+        """generate(num_beams=K, do_sample=False) with HF 5.5 semantics (HF:generation/utils.py _beam_search; the reference forwards
+        num_beams to HF generate(inputs_embeds=...), ref modeling_visualcla.py:382-391).  Batches are split into chunks of
+        max_batch // K prompts; each chunk runs graphs of 8 steps with one host poll of the per-item done flags between them.
+        -> (B * num_return_sequences, L) int64, every row filled past its hypothesis with HF's output_fill_value."""
+        K = int(gc.num_beams)
+        nrs = int(getattr(gc, "num_return_sequences", 1) or 1)
+        if not hasattr(self._engine, "set_beam"):
+            raise NotImplementedError("this engine has no beam-search kernels")
+        if gc.do_sample:
+            raise NotImplementedError("beam sampling (do_sample=True with num_beams > 1) is not on the H100 path")
+        if logits_processor or stopping_criteria:
+            raise NotImplementedError("custom logits_processor / stopping_criteria are not supported with beam search on the H100 path")
+        if streamer is not None:
+            raise NotImplementedError("streaming is not supported with beam search")
+        if getattr(gc, "output_scores", False) or getattr(gc, "output_logits", False):
+            raise NotImplementedError("output_scores / output_logits are not supported with beam search on the H100 path")
+        if (getattr(gc, "num_beam_groups", 1) or 1) > 1 or (getattr(gc, "diversity_penalty", 0.0) or 0.0) != 0.0 \
+                or getattr(gc, "constraints", None) or getattr(gc, "force_words_ids", None):
+            raise NotImplementedError("diverse / constrained beam search is not supported on the H100 path")
+        eos = self._eos_set(gc)
+        if len(eos) > 4:
+            raise NotImplementedError("beam search supports at most 4 eos_token_id values")
+        eng = self._engine
+        if K > min(eng.max_batch, 64) or K > 16:
+            raise NotImplementedError(f"num_beams={K} exceeds this model instance (at most min(max_batch, 64) rows, 16 beams)")
+        max_new = gc.max_new_tokens if gc.max_new_tokens is not None else max(int(gc.max_length or 20), 1)
+        es = gc.early_stopping
+        spec = eng.beam_spec(K, max_new, length_penalty=gc.length_penalty if gc.length_penalty is not None else 1.0,
+                             early_stopping=es if es in (True, "never") else False, eos_token_id=eos,
+                             repetition_penalty=getattr(gc, "repetition_penalty", None) or 1.0,
+                             no_repeat_ngram_size=getattr(gc, "no_repeat_ngram_size", None) or 0,
+                             min_new_tokens=int(getattr(gc, "min_new_tokens", 0) or 0))
+        pad = gc.pad_token_id if gc.pad_token_id is not None else (eos[0] if eos else None)
+        fill = (pad if pad else eos[0]) if eos else -1                       # HF:3187 output_fill_value (operator precedence kept)
+        chunk = max(1, min(eng.max_batch, 64) // K)
+        B = input_ids.shape[0]
+        toks, lens = [], []
+        mode = None
+        for s0 in range(0, B, chunk):
+            sl = slice(s0, s0 + chunk)
+            ids = input_ids[sl]
+            px = None if pixel_values is None else pixel_values[sl]
+            mode, rows = self._image_layout(ids, px)
+            pads = self._left_pad(None if attention_mask is None else attention_mask[sl], mode)
+            S = ids.shape[1] + (eng.nq if mode == N.IMAGE_AT_HEAD else 0)
+            if S + max_new > eng.max_seq:
+                raise ValueError(f"prompt ({S}) + max_new_tokens ({max_new}) exceeds the context capacity max_seq={eng.max_seq} "
+                                 f"of this model instance")
+            if mode != N.TEXT_ONLY:
+                eng.vision_encode(px)
+            n = ids.shape[0]
+            eng.set_beam(spec)
+            try:
+                _, first, _ = eng.prefill(ids, mode, rows, all_logits=False, last_logits=False, left_pad=pads, pos_from_mask=True)
+                tok = eng.token_buffer(n * K)
+                tok.copy_(first)
+                n_done = 1
+                while n_done < max_new:
+                    if bool(eng.read_beam_done(n).bool().all()):
+                        break
+                    k = min(8, max_new - n_done)
+                    eng.decode_many(tok, k)
+                    n_done += k
+                t, ln, _, _ = eng.read_beams(n)
+            finally:
+                eng.set_beam(None)
+            toks.append(t[:, :nrs].reshape(n * nrs, -1))
+            lens.append(ln[:, :nrs].reshape(-1))
+        lens = torch.cat(lens)
+        L = int(lens.max())
+        out = torch.full((B * nrs, L), fill, dtype=torch.int64)
+        allt = torch.cat(toks).to(torch.int64)
+        for i in range(B * nrs):
+            out[i, : int(lens[i])] = allt[i, : int(lens[i])]
+        out = out.to(eng.device)
+        if not getattr(gc, "return_dict_in_generate", False):
+            return out
+        # the returned hypotheses need not be resident in any cache row: the handle records no ids, so it is never reused
+        return SimpleNamespace(sequences=out, logits=None, scores=None,
+                               past_key_values=VclaKVCache(eng, getattr(eng, "session", 0), None, mode, None))
 
     def _plan_kv_reuse(self, cache, input_ids, pixel_values, mode, rows, pads):
         """-> (tokens to keep, (1, T) ids to extend by) when the KV cache `cache` describes can serve this prompt, else None (full
