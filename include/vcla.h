@@ -55,6 +55,8 @@ typedef struct {
   int max_seq;             /* prompt + generated tokens per sequence */
   int max_prefill_tokens;  /* max B*S of one prefill call */
   int page_tokens;         /* tokens per KV-cache page (default 64 if 0) */
+  /* storage of the LLaMA projections: 0 = bf16 (default), 1 = weight-only int8 (load_in_8bit, below) */
+  int weight_format;
 } vcla_config;
 
 const char* vcla_last_error(void);
@@ -87,8 +89,22 @@ int vcla_load_weight(vcla_ctx* ctx, const char* name, const void* src, int dtype
 /* Copy one logical tensor back to host: bf16 for kind 0, f32 for kind 1 (state_dict() equivalent). */
 int vcla_read_weight(vcla_ctx* ctx, const char* name, void* dst_host, vcla_stream stream);
 /* Deterministic synthetic weights: w = mean + std * IrwinHall4(hash(name, seed, index)), bit-identical
- * to oracle/visualcla_oracle.py:hash_normal_bf16 (std/mean per tensor as in oracle weight_specs). */
+ * to oracle/visualcla_oracle.py:hash_normal_bf16 (std/mean per tensor as in oracle weight_specs).  With weight_format 1 the
+ * int8 tensors are quantised from these bf16 values. */
 int vcla_init_synthetic(vcla_ctx* ctx, uint32_t seed, vcla_stream stream);
+
+/* ---- load_in_8bit: weight-only int8 LLaMA projections (weight_format 1) -------------------------------------------------------
+ * The reference passes load_in_8bit only to LlamaForCausalLM.from_pretrained (models/visualcla/modeling_visualcla.py:151-156,
+ * :242-247), where bitsandbytes replaces the seven nn.Linear of every LLaMA layer (q, k, v, o, gate, up, down); embed_tokens,
+ * lm_head, the norms, CLIP, the Resampler and the projector stay as they are.  Here those seven tensors are stored as int8 rows with
+ * one fp32 scale per row (kind 2 in vcla_weight_info): a = max|w_row| in fp32, s = a / 127, q = clamp(rint(w * (127 / a)), -127, 127)
+ * (half to even; a zero row gives s = 0, q = 0), w = the source values in fp32.  The effective weight is q * s; activations stay
+ * bf16 with fp32 accumulation.  This is the weight half of LLM.int8 only (no activation-outlier decomposition), so results are not
+ * bit-equal to bitsandbytes.  vcla_load_weight quantises on the device; vcla_read_weight returns fp32 q * s for kind 2.
+ *   vcla_read_weight_q8  the stored int8 rows (rows x cols, host) and row scales (rows, host), exactly; synchronises
+ *   vcla_load_weight_q8  stores caller int8 rows + scales exactly (host or device pointers); synchronises */
+int vcla_read_weight_q8(vcla_ctx* ctx, const char* name, int8_t* q_host, float* scale_host, vcla_stream stream);
+int vcla_load_weight_q8(vcla_ctx* ctx, const char* name, const int8_t* q, const float* scale, int on_device, vcla_stream stream);
 
 /* ---- the hot path ----------------------------------------------------------------------------- */
 /* Drop all sequences (KV cache lengths -> 0, every KV page back on the free stack). */
@@ -276,7 +292,22 @@ int vcla_op_gemm_csk(const void* W_dev_bf16, const void* X_dev_bf16, int M, int 
                      const float* norm_w, void* xw_or_h, float* ssq_out, const float* ssq_in, int ssq_slots, float inv_dim, float eps,
                      vcla_stream stream);
 int vcla_op_gemm_csk_clusters(int B, int splits);
-/* tuning hooks: read / override the CTAs-per-cluster of the five decode GEMM shapes {qkv, o, gate_up, down, lm_head} at batch B */
+/* The int8 variant of vcla_op_gemm_csk (the decode GEMMs of weight_format 1, replacing bitsandbytes' Linear8bitLt forward behind
+ * models/visualcla/modeling_visualcla.py:151-156): Wq int8 (M, K) row-major, wscale f32 (M) (device); K % 64 == 0; B <= 64 (a 64-column
+ * batch tile serves 33..64).  The row scale is applied after the fixed-order cluster reduction: mode 0 out = rstd * s * acc, mode 1
+ * resid += s * acc, mode 2 gate and up rows each take their own scale.  Synchronises. */
+int vcla_op_gemm_csk_q8(const int8_t* Wq_dev, const float* wscale_dev, const void* X_dev_bf16, int M, int B, int K, int splits, int mode,
+                        float* out_or_resid, const float* norm_w, void* xw_or_h, float* ssq_out, const float* ssq_in, int ssq_slots,
+                        float inv_dim, float eps, vcla_stream stream);
+/* The prefill GEMM of weight_format 1 (same replacement): bf16(Wq) (N, K) int8 row-major is expanded exactly, then
+ * D = A[M,K] * bf16(Wq)^T * diag(wscale) on the wgmma path.  mode 0 store bf16, 1 fp32 (accumulate flag; with norm_w not NULL also
+ * xw = bf16(out * norm_w) (M, N) and ssq_out (M, ceil(N / tile width)) as vcla_prefill's residual GEMMs; the GEMM picks a tile width of
+ * 64, 128 or 256 from M and N), 2 SwiGLU (rows interleaved [32 gate|32 up]).
+ * Synchronises. */
+int vcla_op_gemm_q8(const void* A_dev_bf16, const int8_t* Wq_dev, const float* wscale_dev, int M, int N, int K, int mode, int accumulate,
+                    void* out_dev, int ldo, const float* norm_w, void* xw_dev, float* ssq_out, vcla_stream stream);
+/* tuning hooks: read / override the CTAs-per-cluster of the five decode GEMM shapes {qkv, o, gate_up, down, lm_head} at batch B
+ * (B <= 32; with weight_format 1 B <= 64, where at 33..64 the lm_head runs on the workspace GEMM and its entry is ignored) */
 int vcla_debug_set_csk_splits(vcla_ctx* ctx, int B, int qkv, int o, int gate_up, int down, int lm_head);
 int vcla_debug_get_csk_splits(vcla_ctx* ctx, int B, int* out5);
 /* prefill attention kernel: 0 = the mma.sync kernel everywhere, 1 (default) = wgmma flash attention (QK^T / PV on the warpgroup tensor
@@ -297,7 +328,8 @@ int vcla_op_layernorm(const float* x, int rows, int D, const float* w, const flo
 int vcla_op_rmsnorm(const float* x, int rows, int D, const float* w, float eps, void* y_bf16, vcla_stream stream);
 /* Micro-benchmark of ONE decode weight-streaming GEMM shape (which: 0 fused QKV, 1 o_proj, 2 fused gate/up, 3 down_proj,
  * 4 lm_head) over every layer's distinct weights with batch B, timed with CUDA events on `stream`; returns the mean
- * microseconds per kernel launch and the algorithmic weight bytes one launch streams.  Synchronises. */
+ * microseconds per kernel launch and the algorithmic weight bytes one launch streams (weight_format 1: the int8 kernel, one byte
+ * per weight + 4 per row scale, for shapes 0..3).  Synchronises. */
 int vcla_bench_decode_gemm(vcla_ctx* ctx, int which, int B, int reps, float* avg_us, int64_t* weight_bytes, vcla_stream stream);
 /* Timeline trace for profiles/: when enabled, CTA (0,0,0) of every kernel appends {tag, t_entry, t_dependency_resolved, t_exit}
  * (%globaltimer, ns).  Tags: 1 swap-AB GEMM, 2 GEMM, 3 prefill attention, 4 decode attention, 5 layernorm, 6 rmsnorm, 7 rope+cache,

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libvcla.so")
-SOURCES = ["gemm.cu", "attention.cu", "elementwise.cu", "engine.cu", "preprocess.cu", "sampler.cu", "beam.cu", "gemm_decode.cu", "attention_tc.cu"]
+SOURCES = ["gemm.cu", "attention.cu", "elementwise.cu", "engine.cu", "preprocess.cu", "sampler.cu", "beam.cu", "gemm_decode.cu", "attention_tc.cu", "quant.cu"]
 ARCH = "arch=compute_90a,code=sm_90a"
 HEADERS = ["common.cuh", "kernels.h", "logits_chain.cuh", "preprocess_core.h", os.path.join("..", "..", "include", "vcla.h")]
 

@@ -20,7 +20,7 @@ using namespace vcla;
 
 namespace {
 
-enum SlotKind { SLOT_MAT = 0, SLOT_VEC = 1 };
+enum SlotKind { SLOT_MAT = 0, SLOT_VEC = 1, SLOT_Q8 = 2 };   // SLOT_Q8: int8 rows + fp32 row scales (weight_format 1)
 enum SlotLayout { LAY_PLAIN = 0, LAY_INTERLEAVE32 = 1 };
 
 struct Slot {
@@ -34,6 +34,7 @@ struct Slot {
   void* dst = nullptr;     // storage (bf16 for MAT, f32 for VEC) at the slot's first row
   int ld = 0;              // storage row pitch (elements) for MAT
   void* dst2 = nullptr;    // optional second copy (resampler k/v also live in the all-layer KV weight)
+  float* scale = nullptr;  // SLOT_Q8: row scales, indexed like the stored rows
   double std = 0.0; float mean = 0.f;
 };
 
@@ -47,7 +48,9 @@ struct ResamplerLayer {
 };
 struct TextLayer {
   float *ln1, *ln2;
-  bf16 *wqkv, *wo, *wgu, *wd;
+  bf16 *wqkv, *wo, *wgu, *wd;                 // weight_format 0
+  int8_t *qqkv, *qo, *qgu, *qd;               // weight_format 1: int8 rows (k in the decode kernel's fragment order, quant.cu) ...
+  float *sqkv, *so, *sgu, *sd;                //                  ... and their fp32 scales
   bf16* kv;  // this layer's pages
 };
 
@@ -128,6 +131,7 @@ struct vcla_ctx {
   // prefill activations
   float* resid = nullptr; bf16 *xn = nullptr, *qkv = nullptr, *attn = nullptr, *hmid = nullptr;
   float* p_ssq = nullptr;    // [max_prefill_tokens][t_hidden / 64] row statistics of the deferred-RMSNorm prefill schedule
+  bf16* q8_wide = nullptr;   // weight_format 1: bf16(q) of the projection the prefill GEMM runs next (largest: gate/up)
   // decode activations
   float* d_resid = nullptr; bf16 *d_xn = nullptr, *d_attn = nullptr, *d_h = nullptr;
   float *ws_qkv = nullptr, *ws_o = nullptr, *ws_gu = nullptr, *ws_d = nullptr, *ws_lm = nullptr;
@@ -268,6 +272,29 @@ void layout_weights(vcla_ctx* c) {
     const std::string lp = tp + "layers." + std::to_string(i) + ".";
     L.ln1 = w_alloc<float>(c, T); add_slot(c, lp + "input_layernorm.weight", {T}, SLOT_VEC, L.ln1, 0, 0.1, 1.f);
     L.ln2 = w_alloc<float>(c, T); add_slot(c, lp + "post_attention_layernorm.weight", {T}, SLOT_VEC, L.ln2, 0, 0.1, 1.f);
+    if (g.weight_format == 1) {
+      // load_in_8bit: the seven projections as int8 rows + row scales (q/k/v and gate/up are quantised per slot)
+      L.wqkv = L.wo = L.wgu = L.wd = nullptr;
+      auto q8 = [&](const std::string& name, int64_t rows, int64_t cols, int8_t* q, float* sc, double std_, int layout, int which) {
+        add_slot(c, name, {rows, cols}, SLOT_Q8, q, (int)cols, std_, 0.f, layout, which);
+        if (c->w_arena != nullptr) c->slots.back().scale = sc;
+      };
+      L.qqkv = w_alloc<int8_t>(c, (size_t)3 * T * T); L.sqkv = w_alloc<float>(c, (size_t)3 * T);
+      const char* pr[3] = {"q_proj", "k_proj", "v_proj"};
+      const double sd[3] = {1.5, 1.5, 1.0};
+      for (int j = 0; j < 3; ++j)
+        q8(lp + "self_attn." + pr[j] + ".weight", T, T, L.qqkv ? L.qqkv + (size_t)j * T * T : nullptr, L.sqkv ? L.sqkv + (size_t)j * T : nullptr,
+           sd[j] / sqrt((double)T), LAY_PLAIN, 0);
+      L.qo = w_alloc<int8_t>(c, (size_t)T * T); L.so = w_alloc<float>(c, T);
+      q8(lp + "self_attn.o_proj.weight", T, T, L.qo, L.so, res_gain * 2.0 / sqrt((double)T), LAY_PLAIN, 0);
+      L.qgu = w_alloc<int8_t>(c, (size_t)2 * Ft * T); L.sgu = w_alloc<float>(c, (size_t)2 * Ft);
+      q8(lp + "mlp.gate_proj.weight", Ft, T, L.qgu, L.sgu, 1.0 / sqrt((double)T), LAY_INTERLEAVE32, 0);
+      q8(lp + "mlp.up_proj.weight", Ft, T, L.qgu, L.sgu, 1.0 / sqrt((double)T), LAY_INTERLEAVE32, 1);
+      L.qd = w_alloc<int8_t>(c, (size_t)T * Ft); L.sd = w_alloc<float>(c, T);
+      q8(lp + "mlp.down_proj.weight", T, Ft, L.qd, L.sd, res_gain * 4.0 / sqrt((double)Ft), LAY_PLAIN, 0);
+      continue;
+    }
+    L.qqkv = L.qo = L.qgu = L.qd = nullptr; L.sqkv = L.so = L.sgu = L.sd = nullptr;
     L.wqkv = w_alloc<bf16>(c, (size_t)3 * T * T);
     add_slot(c, lp + "self_attn.q_proj.weight", {T, T}, SLOT_MAT, L.wqkv, T, 1.5 / sqrt((double)T), 0.f);
     add_slot(c, lp + "self_attn.k_proj.weight", {T, T}, SLOT_MAT, L.wqkv ? L.wqkv + (size_t)T * T : nullptr, T, 1.5 / sqrt((double)T), 0.f);
@@ -308,6 +335,7 @@ void layout_activations(vcla_ctx* c) {
   c->attn = a_alloc<bf16>(c, Tk * T);
   c->hmid = a_alloc<bf16>(c, Tk * F);
   c->p_ssq = a_alloc<float>(c, Tk * ((T + 63) / 64));
+  if (g.weight_format == 1) c->q8_wide = a_alloc<bf16>(c, std::max((size_t)3 * T * T, (size_t)2 * F * T));
   const size_t Bp = 64;  // decode operand rows (batch is processed in chunks of <= 64)
   c->d_resid = a_alloc<float>(c, Bp * T);
   c->d_xn = a_alloc<bf16>(c, Bp * T);
@@ -485,6 +513,8 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   if (g.max_batch < 1 || g.max_seq < 1 || g.max_prefill_tokens < 1) return bad("capacities must be positive");
   if (g.max_seq > 1 << 20) return bad("max_seq too large");
   if (g.page_tokens > 64 || g.page_tokens % 8) return bad("page_tokens must be a multiple of 8 and <= 64");
+  if (g.weight_format != 0 && g.weight_format != 1) return bad("weight_format must be 0 (bf16) or 1 (int8 LLaMA projections)");
+  if (g.weight_format == 1 && (g.t_hidden % 64 || g.t_ffn % 64)) return bad("int8 projections need LLaMA hidden and ffn sizes that are multiples of 64");
   c->v_tokens = (g.v_image / g.v_patch) * (g.v_image / g.v_patch) + 1;
   c->kpatch = 3 * g.v_patch * g.v_patch;
   c->kpad = (c->kpatch + 63) / 64 * 64;
@@ -589,6 +619,8 @@ static int place_matrix(const Slot& s, const bf16* src, cudaStream_t st) {
   return 0;
 }
 
+static int q8_which(const Slot& s) { return s.layout == LAY_INTERLEAVE32 ? s.which : -1; }
+
 int vcla_load_weight(vcla_ctx* c, const char* name, const void* src, int dtype, int64_t numel, int on_device, vcla_stream stream) {
   cudaStream_t st = (cudaStream_t)stream;
   auto it = c->slot_index.find(name);
@@ -612,6 +644,9 @@ int vcla_load_weight(vcla_ctx* c, const char* name, const void* src, int dtype, 
   if (s.kind == SLOT_VEC) {
     if (convert_to_f32(dsrc, dtype, (int64_t)n, (float*)s.dst, st)) return -1;
     if (s.dst2 && convert_to_f32(dsrc, dtype, (int64_t)n, (float*)s.dst2, st)) return -1;
+  } else if (s.kind == SLOT_Q8) {
+    // quantised from the source values themselves (fp32 / fp16 / bf16), not from a bf16 copy
+    if (quantize_rows_q8(dsrc, dtype, (int)s.rows, (int)s.cols, q8_which(s), (int8_t*)s.dst, s.scale, st)) return -1;
   } else {
     bf16* tmp = reinterpret_cast<bf16*>((uint8_t*)c->staging + raw_bytes);
     if (convert_to_bf16(dsrc, dtype, (int64_t)n, tmp, st)) return -1;
@@ -628,6 +663,11 @@ int vcla_read_weight(vcla_ctx* c, const char* name, void* dst_host, vcla_stream 
   const Slot& s = c->slots[it->second];
   if (s.kind == SLOT_VEC) {
     VCLA_CUDA_OK(cudaMemcpyAsync(dst_host, s.dst, (size_t)s.cols * 4, cudaMemcpyDeviceToHost, st));
+  } else if (s.kind == SLOT_Q8) {
+    const size_t n = (size_t)s.rows * s.cols;
+    if (ensure_staging(c, n * 4)) return -1;
+    if (read_rows_q8((const int8_t*)s.dst, s.scale, (int)s.rows, (int)s.cols, q8_which(s), nullptr, nullptr, (float*)c->staging, st)) return -1;
+    VCLA_CUDA_OK(cudaMemcpyAsync(dst_host, c->staging, n * 4, cudaMemcpyDeviceToHost, st));
   } else if (s.layout == LAY_INTERLEAVE32) {
     for (int64_t j0 = 0; j0 < s.rows; j0 += 32) {
       const int64_t nr = (s.rows - j0) < 32 ? (s.rows - j0) : 32;
@@ -641,10 +681,51 @@ int vcla_read_weight(vcla_ctx* c, const char* name, void* dst_host, vcla_stream 
   return 0;
 }
 
+static const Slot* q8_slot(vcla_ctx* c, const char* name, const char* what) {
+  auto it = c->slot_index.find(name);
+  if (it == c->slot_index.end()) { set_error("%s: unknown tensor '%s'", what, name); return nullptr; }
+  const Slot& s = c->slots[it->second];
+  if (s.kind != SLOT_Q8) { set_error("%s: '%s' is not stored as int8 (weight_format 1 stores the LLaMA projections so)", what, name); return nullptr; }
+  return &s;
+}
+
+int vcla_read_weight_q8(vcla_ctx* c, const char* name, int8_t* q_host, float* scale_host, vcla_stream stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const Slot* s = q8_slot(c, name, "vcla_read_weight_q8");
+  if (s == nullptr) return -1;
+  const size_t n = (size_t)s->rows * s->cols, qbytes = align_up(n, 256);
+  if (ensure_staging(c, qbytes + (size_t)s->rows * 4)) return -1;
+  int8_t* q = (int8_t*)c->staging;
+  float* sc = (float*)((uint8_t*)c->staging + qbytes);
+  if (read_rows_q8((const int8_t*)s->dst, s->scale, (int)s->rows, (int)s->cols, q8_which(*s), q, sc, nullptr, st)) return -1;
+  if (q_host) VCLA_CUDA_OK(cudaMemcpyAsync(q_host, q, n, cudaMemcpyDeviceToHost, st));
+  if (scale_host) VCLA_CUDA_OK(cudaMemcpyAsync(scale_host, sc, (size_t)s->rows * 4, cudaMemcpyDeviceToHost, st));
+  VCLA_CUDA_OK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int vcla_load_weight_q8(vcla_ctx* c, const char* name, const int8_t* q, const float* scale, int on_device, vcla_stream stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const Slot* s = q8_slot(c, name, "vcla_load_weight_q8");
+  if (s == nullptr) return -1;
+  if (q == nullptr || scale == nullptr) { set_error("vcla_load_weight_q8: null source"); return -1; }
+  const size_t n = (size_t)s->rows * s->cols, qbytes = align_up(n, 256);
+  const int8_t* dq = q; const float* ds = scale;
+  if (!on_device) {
+    if (ensure_staging(c, qbytes + (size_t)s->rows * 4)) return -1;
+    VCLA_CUDA_OK(cudaMemcpyAsync(c->staging, q, n, cudaMemcpyHostToDevice, st));
+    VCLA_CUDA_OK(cudaMemcpyAsync((uint8_t*)c->staging + qbytes, scale, (size_t)s->rows * 4, cudaMemcpyHostToDevice, st));
+    dq = (const int8_t*)c->staging; ds = (const float*)((uint8_t*)c->staging + qbytes);
+  }
+  if (place_rows_q8(dq, ds, (int)s->rows, (int)s->cols, q8_which(*s), (int8_t*)s->dst, s->scale, st)) return -1;
+  VCLA_CUDA_OK(cudaStreamSynchronize(st));
+  return 0;
+}
+
 int vcla_init_synthetic(vcla_ctx* c, uint32_t seed, vcla_stream stream) {
   cudaStream_t st = (cudaStream_t)stream;
   size_t max_n = 0;
-  for (const Slot& s : c->slots) if (s.kind == SLOT_MAT) max_n = std::max(max_n, (size_t)s.rows * s.cols);
+  for (const Slot& s : c->slots) if (s.kind != SLOT_VEC) max_n = std::max(max_n, (size_t)s.rows * s.cols);
   if (ensure_staging(c, max_n * 2 + 256)) return -1;
   const double sigma = 65536.0 / sqrt(3.0);
   for (const Slot& s : c->slots) {
@@ -657,7 +738,9 @@ int vcla_init_synthetic(vcla_ctx* c, uint32_t seed, vcla_stream stream) {
     } else {
       bf16* tmp = (bf16*)c->staging;
       if (fill_hash_normal(tmp, nullptr, n, sd, mul, s.mean, st)) return -1;
-      if (place_matrix(s, tmp, st)) return -1;
+      if (s.kind == SLOT_Q8) {
+        if (quantize_rows_q8(tmp, VCLA_BF16, (int)s.rows, (int)s.cols, q8_which(s), (int8_t*)s.dst, s.scale, st)) return -1;
+      } else if (place_matrix(s, tmp, st)) return -1;
     }
   }
   VCLA_CUDA_OK(cudaStreamSynchronize(st));
@@ -793,9 +876,11 @@ int vcla_vision_encode(vcla_ctx* c, const void* pixels, int pixel_dtype, int B, 
 // -------------------------------------------------------------------------------------------------
 // decode launches (the prefill's last-position lm_head uses the workspace one too)
 // -------------------------------------------------------------------------------------------------
-// The batch size alone picks the decode schedule: up to 32 rows the cluster split-K GEMMs with fused consumers (5 kernels
+// The batch size picks the decode schedule: up to 32 rows the cluster split-K GEMMs with fused consumers (5 kernels
 // per layer); 33..64 rows split-K partials in an L2 workspace reduced by separate consumer kernels (8 kernels per layer).
-static bool decode_uses_csk(int B) { return B <= 32; }
+// int8 projections (weight_format 1) run the cluster split-K schedule at every batch: its int8 kernel has a 64-column batch tile.
+static bool decode_uses_csk(const vcla_ctx* c, int B) { return B <= 32 || c->cfg.weight_format == 1; }
+static int csk_max_batch(const vcla_ctx* c) { return c->cfg.weight_format == 1 ? 64 : 32; }
 
 // The five weight-streaming GEMMs of a decode step (numbering of vcla_bench_decode_gemm's `which`).
 enum DecodeGemm { DG_QKV = 0, DG_O = 1, DG_GATE_UP = 2, DG_DOWN = 3, DG_LM_HEAD = 4 };
@@ -826,10 +911,10 @@ static int csk_gemm(vcla_ctx* c, int which, int i, int B, cudaStream_t st) {
   const TextLayer* L = which == DG_LM_HEAD ? nullptr : &c->tl[i];
   CskCall k; k.B = B; k.inv_dim = 1.0f / (float)TH; k.eps = g.t_eps;
   switch (which) {
-    case DG_QKV: k.W = L->wqkv; k.X = c->d_xn; k.M = 3 * TH; k.K = TH; k.splits = c->csk_qkv; k.mode = CSK_OUT_F32; k.out = c->ws_qkv; break;
-    case DG_O: k.W = L->wo; k.X = c->d_attn; k.M = TH; k.K = TH; k.splits = c->csk_o; k.mode = CSK_RESID; k.norm_w = L->ln2; break;
-    case DG_GATE_UP: k.W = L->wgu; k.X = c->d_xn; k.M = 2 * F; k.K = TH; k.splits = c->csk_gu; k.mode = CSK_SWIGLU; k.h = c->d_h; break;
-    case DG_DOWN: k.W = L->wd; k.X = c->d_h; k.M = TH; k.K = F; k.splits = c->csk_d; k.mode = CSK_RESID;
+    case DG_QKV: k.W = L->wqkv; k.Wq = L->qqkv; k.wscale = L->sqkv; k.X = c->d_xn; k.M = 3 * TH; k.K = TH; k.splits = c->csk_qkv; k.mode = CSK_OUT_F32; k.out = c->ws_qkv; break;
+    case DG_O: k.W = L->wo; k.Wq = L->qo; k.wscale = L->so; k.X = c->d_attn; k.M = TH; k.K = TH; k.splits = c->csk_o; k.mode = CSK_RESID; k.norm_w = L->ln2; break;
+    case DG_GATE_UP: k.W = L->wgu; k.Wq = L->qgu; k.wscale = L->sgu; k.X = c->d_xn; k.M = 2 * F; k.K = TH; k.splits = c->csk_gu; k.mode = CSK_SWIGLU; k.h = c->d_h; break;
+    case DG_DOWN: k.W = L->wd; k.Wq = L->qd; k.wscale = L->sd; k.X = c->d_h; k.M = TH; k.K = F; k.splits = c->csk_d; k.mode = CSK_RESID;
       k.norm_w = (i + 1 < g.t_layers) ? c->tl[i + 1].ln1 : c->final_norm; break;
     default: k.W = c->lm_head; k.X = c->d_xn; k.M = g.t_vocab; k.K = TH; k.splits = c->csk_lm; k.mode = CSK_OUT_F32; k.out = c->ws_lm; break;
   }
@@ -933,10 +1018,20 @@ static int prefill_layers(vcla_ctx* c, int B, int S, const int32_t* left_pad, in
   const int slots = (TH + gemm_pick_bn(rows, TH) - 1) / gemm_pick_bn(rows, TH);
   GemmRowScale rsc; rsc.ssq = c->p_ssq; rsc.slots = slots; rsc.inv_dim = 1.0f / (float)TH; rsc.eps = g.t_eps;
   count(c); if (prenorm_rows(c->resid, rows, TH, c->tl[0].ln1, c->xn, c->p_ssq, slots, st)) return -1;
+  // int8 projections: each GEMM first expands its int8 rows to bf16(q) (exact) in q8_wide and takes the row scales as column scales,
+  // so the prefill computes sum(q x) * s like the decode kernel
+  const bool q8 = g.weight_format == 1;
+  auto weight = [&](const bf16* w, const int8_t* q, int n, int k, GemmCall& gc, const float* sc) -> int {
+    if (!q8) { gc.B = w; return 0; }
+    count(c); if (expand_rows_q8(q, n, k, 1, c->q8_wide, st)) return -1;
+    gc.B = c->q8_wide; gc.colscale = sc;
+    return 0;
+  };
   for (int i = 0; i < g.t_layers; ++i) {
     const TextLayer& L = c->tl[i];
     {
-      GemmCall gc; gc.A = c->xn; gc.B = L.wqkv; gc.M = rows; gc.N = 3 * TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_STORE_BF16; gc.out = c->qkv; gc.ldo = 3 * TH;
+      GemmCall gc; if (weight(L.wqkv, L.qqkv, 3 * TH, TH, gc, L.sqkv)) return -1;
+      gc.A = c->xn; gc.M = rows; gc.N = 3 * TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_STORE_BF16; gc.out = c->qkv; gc.ldo = 3 * TH;
       gc.rowscale = rsc;
       gc.rope.cos = c->rope_cos; gc.rope.sin = c->rope_sin; gc.rope.kv_pages = L.kv; gc.rope.page_table = c->page_table; gc.rope.pages_per_seq = c->pages_per_seq;
       gc.rope.page_tokens = c->page_tokens; gc.rope.S = S; gc.rope.T = TH; gc.rope.H = H; gc.rope.left_pad = left_pad; gc.rope.pos_from_mask = pos_from_mask;
@@ -954,17 +1049,20 @@ static int prefill_layers(vcla_ctx* c, int B, int S, const int32_t* left_pad, in
       count(c); if (attention_paged(a, st)) return -1;
     }
     {
-      GemmCall gc; gc.A = c->attn; gc.B = L.wo; gc.M = rows; gc.N = TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_ADD_F32; gc.accumulate = 1; gc.out = c->resid; gc.ldo = TH;
+      GemmCall gc; if (weight(L.wo, L.qo, TH, TH, gc, L.so)) return -1;
+      gc.A = c->attn; gc.M = rows; gc.N = TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_ADD_F32; gc.accumulate = 1; gc.out = c->resid; gc.ldo = TH;
       gc.emit.norm_w = L.ln2; gc.emit.xw = c->xn; gc.emit.ldxw = TH; gc.emit.ssq_out = c->p_ssq;
       count(c); if (gemm_tc(gc, st)) return -1;
     }
     {
-      GemmCall gc; gc.A = c->xn; gc.B = L.wgu; gc.M = rows; gc.N = 2 * F; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_SWIGLU_BF16; gc.out = c->hmid; gc.ldo = F;
+      GemmCall gc; if (weight(L.wgu, L.qgu, 2 * F, TH, gc, L.sgu)) return -1;
+      gc.A = c->xn; gc.M = rows; gc.N = 2 * F; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_SWIGLU_BF16; gc.out = c->hmid; gc.ldo = F;
       gc.rowscale = rsc;
       count(c); if (gemm_tc(gc, st)) return -1;
     }
     {
-      GemmCall gc; gc.A = c->hmid; gc.B = L.wd; gc.M = rows; gc.N = TH; gc.K = F; gc.lda = F; gc.ldb = F; gc.mode = GEMM_ADD_F32; gc.accumulate = 1; gc.out = c->resid; gc.ldo = TH;
+      GemmCall gc; if (weight(L.wd, L.qd, TH, F, gc, L.sd)) return -1;
+      gc.A = c->hmid; gc.M = rows; gc.N = TH; gc.K = F; gc.lda = F; gc.ldb = F; gc.mode = GEMM_ADD_F32; gc.accumulate = 1; gc.out = c->resid; gc.ldo = TH;
       gc.emit.norm_w = (i + 1 < g.t_layers) ? c->tl[i + 1].ln1 : c->final_norm; gc.emit.xw = c->xn; gc.emit.ldxw = TH; gc.emit.ssq_out = c->p_ssq;
       count(c); if (gemm_tc(gc, st)) return -1;
     }
@@ -1088,18 +1186,19 @@ static int decode_enqueue_workspace(vcla_ctx* c, const int32_t* tok_in, int B, f
   return 0;
 }
 
-// ---- cluster split-K schedule (batches <= 32): 5 kernels per layer, no split-K workspace, no consumer kernels ----------
+// ---- cluster split-K schedule (batches <= 32, every batch with int8 projections): 5 kernels per layer, no split-K workspace,
+// no consumer kernels ------------------------------------------------------------------------------------------------------------
 // CTAs per cluster for a [M, K] weight at batch B: the choice that keeps the largest share of the 2 x SMs CTA slots busy over whole
-// rounds of cluster-tiles (clusters are gang-scheduled: floor(slots / S) of them are resident).
-static int csk_pick(int M, int K, int B) {
-  const int tiles = (M + 127) / 128, kb = (K + 63) / 64, bn = B <= 16 ? 16 : 32;
+// rounds of cluster-tiles (clusters are gang-scheduled: floor(slots / S) of them are resident).  q8: the int8 kernel's batch tiles.
+static int csk_pick(int M, int K, int B, bool q8 = false) {
+  const int tiles = (M + 127) / 128, kb = (K + 63) / 64, bn = B <= 16 ? 16 : (B <= 32 || !q8 ? 32 : 64);
   int best = 1; double best_score = -1.0;
   for (int S = 1; S <= 8; ++S) {
     const int per = (kb + S - 1) / S;
     if ((kb + per - 1) / per != S) continue;                 // every K slice non-empty
     if (S > 1 && kb / S < 2) break;
     if (((B + S - 1) / S) * S > bn + 4) continue;            // reduce buffer columns
-    int ncl = gemm_csk_clusters(B, S);
+    int ncl = gemm_csk_clusters(B, S, q8);
     if (ncl <= 0) continue;
     if (ncl > tiles) ncl = tiles;
     const int rounds = (tiles + ncl - 1) / ncl;
@@ -1112,8 +1211,10 @@ static int csk_pick(int M, int K, int B) {
 static int csk_prepare(vcla_ctx* c, int B) {
   if (c->csk_batch == B) return 0;
   const vcla_config& g = c->cfg;
-  int v[5] = {csk_pick(3 * g.t_hidden, g.t_hidden, B), csk_pick(g.t_hidden, g.t_hidden, B), csk_pick(2 * g.t_ffn, g.t_hidden, B),
-              csk_pick(g.t_hidden, g.t_ffn, B), csk_pick(g.t_vocab, g.t_hidden, B)};
+  const bool q8 = g.weight_format == 1;
+  // the bf16 lm_head runs on the cluster kernel only up to 32 rows (beyond: the workspace GEMM, see decode_enqueue_csk)
+  int v[5] = {csk_pick(3 * g.t_hidden, g.t_hidden, B, q8), csk_pick(g.t_hidden, g.t_hidden, B, q8), csk_pick(2 * g.t_ffn, g.t_hidden, B, q8),
+              csk_pick(g.t_hidden, g.t_ffn, B, q8), B <= 32 ? csk_pick(g.t_vocab, g.t_hidden, B) : 1};
   if (const char* e = getenv("VCLA_CSK_SPLITS")) {            // tuning override: "qkv,o,gu,d,lm"
     int o[5];
     if (sscanf(e, "%d,%d,%d,%d,%d", &o[0], &o[1], &o[2], &o[3], &o[4]) == 5) for (int i = 0; i < 5; ++i) if (o[i] >= 1 && o[i] <= 8) v[i] = o[i];
@@ -1135,14 +1236,20 @@ static int decode_enqueue_csk(vcla_ctx* c, const int32_t* tok_in, int B, float* 
     count(c); if (attention_decode(decode_attn_call(c, c->tl[i], B, 1), st)) return -1;
     if (csk_gemm(c, DG_O, i, B, st) || csk_gemm(c, DG_GATE_UP, i, B, st) || csk_gemm(c, DG_DOWN, i, B, st)) return -1;
   }
-  if (csk_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
-  if (logits_argmax(c, B, logits, tok_out, 1, st, 1)) return -1;
+  if (B > 32) {
+    // int8 projections at 33..64 rows: the bf16 lm_head streams once through the workspace GEMM over the normalised rows
+    count(c); if (dec_resid_norm(nullptr, 0, B, c->d_resid, B, TH, c->final_norm, g.t_eps, c->d_xn, st)) return -1;
+    if (ws_gemm(c, DG_LM_HEAD, 0, B, st) || logits_argmax(c, B, logits, tok_out, 1, st)) return -1;
+  } else {
+    if (csk_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
+    if (logits_argmax(c, B, logits, tok_out, 1, st, 1)) return -1;
+  }
   count(c); if (advance_and_reserve(c, B, tok_out, st)) return -1;
   return 0;
 }
 
 static int decode_enqueue(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, cudaStream_t st) {
-  return decode_uses_csk(B) ? decode_enqueue_csk(c, tok_in, B, logits, tok_out, st) : decode_enqueue_workspace(c, tok_in, B, logits, tok_out, st);
+  return decode_uses_csk(c, B) ? decode_enqueue_csk(c, tok_in, B, logits, tok_out, st) : decode_enqueue_workspace(c, tok_in, B, logits, tok_out, st);
 }
 
 static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, int n_steps, cudaStream_t st) {
@@ -1211,7 +1318,7 @@ int vcla_decode_step(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, i
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_in || !tok_out) { set_error("decode: null token buffers"); return -1; }
   if (decode_capacity(c, 1, B)) return -1;
-  if (decode_uses_csk(B) && csk_prepare(c, B)) return -1;      // occupancy queries: never inside a capture
+  if (decode_uses_csk(c, B) && csk_prepare(c, B)) return -1;      // occupancy queries: never inside a capture
   int rc = use_graph ? decode_graph(c, tok_in, B, logits, tok_out, 1, st) : decode_enqueue(c, tok_in, B, logits, tok_out, st);
   if (rc == 0 && !use_graph && c->dp_on()) rc = dp_wait(c, st);
   if (rc == 0) c->len_bound += 1;
@@ -1224,7 +1331,7 @@ int vcla_decode_multi(vcla_ctx* c, int32_t* tok_inout, int B, int n_steps, vcla_
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_inout || n_steps < 1 || n_steps > 64) { set_error("decode_multi: bad arguments"); return -1; }
   if (decode_capacity(c, n_steps, B)) return -1;
-  if (decode_uses_csk(B) && csk_prepare(c, B)) return -1;
+  if (decode_uses_csk(c, B) && csk_prepare(c, B)) return -1;
   const int rc = decode_graph(c, tok_inout, B, nullptr, tok_inout, n_steps, (cudaStream_t)stream);
   if (rc == 0) c->len_bound += n_steps;
   return rc;
@@ -1472,7 +1579,7 @@ int vcla_bench_decode_gemm(vcla_ctx* c, int which, int B, int reps, float* avg_u
   cudaEvent_t e0, e1;
   VCLA_CUDA_OK(cudaEventCreate(&e0));
   VCLA_CUDA_OK(cudaEventCreate(&e1));
-  const bool csk = decode_uses_csk(B);
+  const bool csk = decode_uses_csk(c, B) && !(which == DG_LM_HEAD && B > 32);
   if (csk && csk_prepare(c, B)) return -1;
   auto run_all = [&]() -> int {
     const int layers = which == DG_LM_HEAD ? 1 : g.t_layers;
@@ -1490,7 +1597,9 @@ int vcla_bench_decode_gemm(vcla_ctx* c, int which, int B, int reps, float* avg_u
   if (avg_us) *avg_us = ms * 1000.f / (float)(reps * per);
   if (weight_bytes) {
     const int64_t n[5] = {(int64_t)3 * TH * TH, (int64_t)TH * TH, (int64_t)2 * F * TH, (int64_t)TH * F, (int64_t)g.t_vocab * TH};
-    *weight_bytes = n[which] * 2;
+    const int64_t rows[5] = {(int64_t)3 * TH, TH, (int64_t)2 * F, TH, g.t_vocab};
+    // int8 projections: one byte per weight + one fp32 scale per row
+    *weight_bytes = (g.weight_format == 1 && which != DG_LM_HEAD) ? n[which] + rows[which] * 4 : n[which] * 2;
   }
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   return 0;
@@ -1549,9 +1658,49 @@ int vcla_op_gemm_csk(const void* W, const void* X, int M, int B, int K, int spli
   else { set_error("vcla_op_gemm_csk: unknown mode %d", mode); return -1; }
   return gemm_csk(k, (cudaStream_t)stream);
 }
+int vcla_op_gemm_csk_q8(const int8_t* Wq, const float* wscale, const void* X, int M, int B, int K, int splits, int mode, float* out_or_resid,
+                        const float* norm_w, void* xw_or_h, float* ssq_out, const float* ssq_in, int ssq_slots, float inv_dim, float eps,
+                        vcla_stream stream) {
+  // caller rows are in logical order: put them into the stored (fragment) order in a scratch, run, free.  Synchronises.
+  if (!Wq || !wscale || !X || M < 1 || K < 1) { set_error("vcla_op_gemm_csk_q8: bad arguments"); return -1; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t qbytes = align_up((size_t)M * K, 256);
+  uint8_t* scratch = nullptr;
+  VCLA_CUDA_OK(cudaMalloc(&scratch, qbytes + (size_t)M * 4));
+  CskCall k; k.Wq = (const int8_t*)scratch; k.wscale = (const float*)(scratch + qbytes); k.X = (const bf16*)X; k.M = M; k.B = B; k.K = K;
+  k.splits = splits; k.mode = mode; k.ssq_in = ssq_in; k.ssq_slots = ssq_slots; k.inv_dim = inv_dim; k.eps = eps;
+  int rc = 0;
+  if (mode == CSK_OUT_F32) { k.out = out_or_resid; k.ldo = M; }
+  else if (mode == CSK_RESID) { k.resid = out_or_resid; k.norm_w = norm_w; k.xw = (bf16*)xw_or_h; k.ssq_out = ssq_out; }
+  else if (mode == CSK_SWIGLU) { k.h = (bf16*)xw_or_h; }
+  else { set_error("vcla_op_gemm_csk_q8: unknown mode %d", mode); rc = -1; }
+  if (rc == 0) rc = place_rows_q8(Wq, wscale, M, K, -1, (int8_t*)scratch, (float*)(scratch + qbytes), st);
+  if (rc == 0) rc = gemm_csk(k, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_gemm_csk_q8: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
+  cudaFree(scratch);
+  return rc;
+}
+int vcla_op_gemm_q8(const void* A, const int8_t* Wq, const float* wscale, int M, int N, int K, int mode, int accumulate, void* out, int ldo,
+                    const float* norm_w, void* xw, float* ssq_out, vcla_stream stream) {
+  // bf16(q) of the caller's logical rows into a scratch, then the prefill GEMM with the row scales as column scales.  Synchronises.
+  if (!A || !Wq || !wscale || !out || M < 1 || N < 1 || K < 1) { set_error("vcla_op_gemm_q8: bad arguments"); return -1; }
+  if (mode != GEMM_STORE_BF16 && mode != GEMM_ADD_F32 && mode != GEMM_SWIGLU_BF16) { set_error("vcla_op_gemm_q8: unknown mode %d", mode); return -1; }
+  cudaStream_t st = (cudaStream_t)stream;
+  bf16* wide = nullptr;
+  VCLA_CUDA_OK(cudaMalloc(&wide, (size_t)N * K * 2));
+  GemmCall g; g.A = (const bf16*)A; g.B = wide; g.M = M; g.N = N; g.K = K; g.lda = K; g.ldb = K; g.mode = mode; g.accumulate = accumulate;
+  g.out = out; g.ldo = ldo; g.colscale = wscale;
+  if (norm_w != nullptr) { g.emit.norm_w = norm_w; g.emit.xw = (bf16*)xw; g.emit.ldxw = N; g.emit.ssq_out = ssq_out; }
+  int rc = expand_rows_q8(Wq, N, K, 0, wide, st);
+  if (rc == 0) rc = gemm_tc(g, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_gemm_q8: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
+  cudaFree(wide);
+  return rc;
+}
 int vcla_debug_set_csk_splits(vcla_ctx* c, int B, int qkv, int o, int gu, int d, int lm) {
-  // tuning hook: CTAs per cluster of the five decode GEMM shapes at batch B (0 = keep the automatic choice); drops the captured graphs
-  if (!c || B < 1 || B > 32) { set_error("vcla_debug_set_csk_splits: bad arguments"); return -1; }
+  // tuning hook: CTAs per cluster of the five decode GEMM shapes at batch B (0 = keep the automatic choice); drops the captured graphs.
+  // Batches 33..64 run the cluster schedule only with int8 projections, whose lm_head then is the workspace GEMM (lm is ignored).
+  if (!c || B < 1 || B > csk_max_batch(c)) { set_error("vcla_debug_set_csk_splits: bad arguments"); return -1; }
   c->csk_batch = 0;
   if (csk_prepare(c, B)) return -1;
   int* dst[5] = {&c->csk_qkv, &c->csk_o, &c->csk_gu, &c->csk_d, &c->csk_lm};
@@ -1560,7 +1709,7 @@ int vcla_debug_set_csk_splits(vcla_ctx* c, int B, int qkv, int o, int gu, int d,
   return drop_graphs(c);
 }
 int vcla_debug_get_csk_splits(vcla_ctx* c, int B, int* out5) {
-  if (!c || !out5 || B < 1 || B > 32) return -1;
+  if (!c || !out5 || B < 1 || B > csk_max_batch(c)) return -1;
   if (c->csk_batch != B && csk_prepare(c, B)) return -1;
   out5[0] = c->csk_qkv; out5[1] = c->csk_o; out5[2] = c->csk_gu; out5[3] = c->csk_d; out5[4] = c->csk_lm;
   return 0;

@@ -68,6 +68,7 @@ struct GemmParams {
   GemmRowScale rowscale;
   GemmEmitNorm emit;
   GemmRope rope;
+  const float* colscale;
 };
 
 constexpr int kBlockK = 64;
@@ -258,6 +259,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       } else {
         const int col_tile = n_blk * BN;
+        if (p.colscale != nullptr) {
+          // per-column scale of int8 weights (their row scales), ahead of every epilogue
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = col_tile + 8 * j + fc + e;
+              const float cs = col < p.N ? __ldg(p.colscale + col) : 0.f;
+#pragma unroll
+              for (int h = 0; h < MH; ++h) {
+                acc[h][4 * j + e] *= cs;
+                acc[h][4 * j + 2 + e] *= cs;
+              }
+            }
+          }
+        }
 #pragma unroll
         for (int h = 0; h < MH; ++h) {
 #pragma unroll
@@ -534,10 +551,11 @@ int gemm_tc(const GemmCall& c, cudaStream_t st) {
   p.rows_per_group = c.rows_per_group; p.group_stride = c.group_stride; p.row_offset = c.row_offset;
   p.ws_rows = c.ws_rows;
   p.l2_prefetch_kb = c.l2_prefetch_kb;
-  p.rowscale = c.rowscale; p.emit = c.emit; p.rope = c.rope;
+  p.rowscale = c.rowscale; p.emit = c.emit; p.rope = c.rope; p.colscale = c.colscale;
   p.policy_a = c.weights_are_A ? kEvictFirst : kEvictLast;
   p.policy_b = c.weights_are_A ? kEvictLast : kEvictNormal;
 
+  if (c.colscale != nullptr && c.mode == GEMM_PARTIAL_F32) { set_error("gemm: colscale is not defined for split-K partials"); return -1; }
   if (c.mode == GEMM_PARTIAL_F32) {
     int splits = c.splits > 0 ? c.splits : 1;
     if (splits > p.kb_total) splits = p.kb_total;

@@ -48,11 +48,13 @@ struct CskParams {
   const float* ssq_in; int ssq_slots; float inv_dim, eps;   // deferred scale of the operand rows (null: 1)
   uint64_t policy_w, policy_x;
   int cluster_fence;           // explicit fence.acq_rel.cluster before the remote arrive (VCLA_CSK_FENCE=1; the arrive itself is release.cluster)
+  const float* wscale;         // Q8: per-row scale of the int8 weight rows
 };
 
-template <int BN, int STAGES, int NBUF>
+// Q8: the weight tile is int8 (64 B rows, no swizzle, k permuted into fragment order, see gemm_csk_kernel), the batch tile stays bf16.
+template <int BN, int STAGES, int NBUF, bool Q8 = false>
 struct CskCfg {
-  static constexpr int A_BYTES = kCskBlockM * kCskBlockK * 2;
+  static constexpr int A_BYTES = kCskBlockM * kCskBlockK * (Q8 ? 1 : 2);
   static constexpr int B_BYTES = BN * kCskBlockK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int RED_COLS = BN + 4;                                 // >= S * ceil(B / S) (checked at launch)
@@ -60,9 +62,10 @@ struct CskCfg {
   static constexpr int RED_OFF = STAGES * STAGE_BYTES;
   static constexpr int BAR_OFF = RED_OFF + NBUF * RED_BYTES;        // NBUF = 2: double-buffered reduce; 1: one buffer + a 'consumed' barrier
   static constexpr int MISC_OFF = BAR_OFF + 256;                          // rstd[BN], ssq warp partials [4][BN]
-  static constexpr int SMEM_BYTES = MISC_OFF + 1024 + 1024;              // + slack for the 1024 B alignment of the ring
+  static constexpr int MISC_BYTES = BN * 20 > 1024 ? BN * 20 : 1024;
+  static constexpr int SMEM_BYTES = MISC_OFF + MISC_BYTES + 1024;        // + slack for the 1024 B alignment of the ring
   static_assert(STAGE_BYTES % 1024 == 0, "stage must keep 1024 B alignment for SWIZZLE_128B");
-  static_assert(BN == 16 || BN == 32, "decode batch tile");
+  static_assert(BN == 16 || BN == 32 || (Q8 && BN == 64), "decode batch tile");
 };
 
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
@@ -96,10 +99,22 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-template <int BN, int STAGES, int NBUF>
+// Two bytes of an int8 word -> bf16x2, exactly: byte + 128 is placed in the mantissa of 2^23 and the bias subtracted in fp32.
+__device__ __forceinline__ uint32_t i8x2_to_bf16x2(uint32_t biased, uint32_t sel_lo, uint32_t sel_hi) {
+  const float lo = __int_as_float((int)__byte_perm(biased, 0x4B000000u, sel_lo)) - 8388736.f;
+  const float hi = __int_as_float((int)__byte_perm(biased, 0x4B000000u, sel_hi)) - 8388736.f;
+  return pack_bf16x2(lo, hi);
+}
+
+// Q8 = true: W is int8 with one fp32 scale per row (weight-only int8).  Each 64-column k-block of a weight row is stored in fragment
+// order: byte 16 q + 4 s + j holds column 16 s + 2 q + {0, 1, 8, 9}[j], so the 16 bytes at offset 16 (lane % 4) of a row are exactly the
+// A-fragment elements the thread needs for the four k16 steps (one 16-byte shared-memory load per row).  They are converted to bf16 in
+// registers (int8 is exact in bf16) and fed to register-A wgmma; the row scale commutes with the contraction and is applied after the
+// cluster reduction.
+template <int BN, int STAGES, int NBUF, bool Q8 = false>
 __global__ void __launch_bounds__(kCskThreads, 2)
 gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const CskParams p) {
-  using C = CskCfg<BN, STAGES, NBUF>;
+  using C = CskCfg<BN, STAGES, NBUF, Q8>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
@@ -198,6 +213,43 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
     for (int t = cluster_id; t < p.m_tiles; t += p.n_clusters) {
       const bool last_tile = t + p.n_clusters >= p.m_tiles;
       int prev = -1;
+      if constexpr (Q8) {
+        // One register set of A fragments: each k-block's MMAs are waited for before the next k-block is converted.  Two sets used
+        // alternately with one MMA group in flight make ptxas serialise every wgmma (C7513: non-wgmma instructions define wgmma
+        // input registers inside the pipeline stage), which is slower still.
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait_mma(full_bar(stage), phase);
+          const uint32_t sa = base + stage * C::STAGE_BYTES;
+          const uint64_t bdesc = make_desc_sw128(sa + C::A_BYTES);
+          const uint8_t* tile = base_ptr + stage * C::STAGE_BYTES;
+          uint32_t a[2][4][4];                        // [64-row block][k16 step][fragment register]
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int h2 = 0; h2 < 2; ++h2) {
+              const uint4 v = *reinterpret_cast<const uint4*>(tile + (h * 64 + fr + 8 * h2) * kCskBlockK + 16 * (lane & 3));
+              const uint32_t w[4] = {v.x ^ 0x80808080u, v.y ^ 0x80808080u, v.z ^ 0x80808080u, v.w ^ 0x80808080u};
+#pragma unroll
+              for (int s = 0; s < 4; ++s) {
+                a[h][s][h2] = i8x2_to_bf16x2(w[s], 0x7540u, 0x7541u);
+                a[h][s][2 + h2] = i8x2_to_bf16x2(w[s], 0x7542u, 0x7543u);
+              }
+            }
+          }
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kCskBlockK / 16; ++k) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) wgmma_bf16_rs<BN>(acc[h], a[h][k], bdesc + 2u * k, (kb > kb0 || k > 0) ? 1 : 0);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();                          // the A registers are rewritten by the next k-block
+          fence_regs(acc[0]);
+          fence_regs(acc[1]);
+          if (threadIdx.x == 0) mbar_arrive(empty_bar(stage));
+          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+        }
+      } else {
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait_mma(full_bar(stage), phase);
         const uint32_t sa = base + stage * C::STAGE_BYTES;
@@ -219,6 +271,7 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       fence_regs(acc[0]);
       fence_regs(acc[1]);
       if (prev >= 0 && threadIdx.x == 0) mbar_arrive(empty_bar(prev));
+      }
       if constexpr (NBUF == 1) {
         if (!first_tile) { mbar_wait_cluster(red_bar(1), freephase); freephase ^= 1u; }
         first_tile = false;
@@ -260,6 +313,7 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
         for (int cl = 0; cl < my_nc; ++cl) {
           float sum = 0.f;
           for (int s = 0; s < S; ++s) sum += red[(size_t)((s * cols_per + cl) * kCskBlockM) + row_in_tile];   // fixed order
+          if constexpr (Q8) sum *= row_ok ? __ldg(p.wscale + row) : 0.f;
           park[(size_t)cl * kCskBlockM + row_in_tile] = sum;      // source 0's value of this element was read by this thread only
         }
         asm volatile("bar.sync 1, 128;" ::: "memory");
@@ -282,6 +336,7 @@ gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
           const int b = my_c0 + cl;
           float sum = 0.f;
           for (int s = 0; s < S; ++s) sum += red[(size_t)((s * cols_per + cl) * kCskBlockM) + row_in_tile];   // fixed order
+          if constexpr (Q8) sum *= row_ok ? __ldg(p.wscale + row) : 0.f;
           if (p.mode == CSK_OUT_F32) {
             if (row_ok) p.out[(size_t)b * p.ldo + row] = sum * s_rstd[b];
           } else {   // CSK_RESID
@@ -343,39 +398,45 @@ static int csk_init() {
              cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) == cudaSuccess;
     };
     if (!prep((const void*)gemm_csk_kernel<16, 4, 2>, CskCfg<16, 4, 2>::SMEM_BYTES) || !prep((const void*)gemm_csk_kernel<32, 3, 2>, CskCfg<32, 3, 2>::SMEM_BYTES) ||
-        !prep((const void*)gemm_csk_kernel<16, 5, 1>, CskCfg<16, 5, 1>::SMEM_BYTES) || !prep((const void*)gemm_csk_kernel<32, 4, 1>, CskCfg<32, 4, 1>::SMEM_BYTES)) {
+        !prep((const void*)gemm_csk_kernel<16, 5, 1>, CskCfg<16, 5, 1>::SMEM_BYTES) || !prep((const void*)gemm_csk_kernel<32, 4, 1>, CskCfg<32, 4, 1>::SMEM_BYTES) ||
+        !prep((const void*)gemm_csk_kernel<16, 8, 2, true>, CskCfg<16, 8, 2, true>::SMEM_BYTES) ||
+        !prep((const void*)gemm_csk_kernel<32, 6, 2, true>, CskCfg<32, 6, 2, true>::SMEM_BYTES) ||
+        !prep((const void*)gemm_csk_kernel<64, 4, 1, true>, CskCfg<64, 4, 1, true>::SMEM_BYTES)) {
       set_error("gemm_csk: cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError())); g_csk_rc = -1;
     }
   });
   return g_csk_rc;
 }
 
-static int csk_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ld * 2) % 16 != 0) { set_error("gemm_csk: TMA operand alignment"); return -1; }
+// int8 = true: a byte matrix in plain (unswizzled) 64 B rows, the layout the Q8 kernel's fragment loads expect
+static int csk_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, bool int8 = false) {
+  const uint64_t esz = int8 ? 1 : 2;
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ld * esz) % 16 != 0) { set_error("gemm_csk: TMA operand alignment"); return -1; }
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * 2};
+  cuuint64_t strides[1] = {ld * esz};
   cuuint32_t box[2] = {(cuuint32_t)kCskBlockK, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = g_csk_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = g_csk_encode(m, int8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, int8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("gemm_csk: cuTensorMapEncodeTiled failed (%d)", (int)r); return -1; }
   return 0;
 }
 
 // clusters of S CTAs that can be co-resident (2 CTAs per SM, a cluster never spans GPCs), cached per (BN, S)
-template <int BN, int STAGES, int NBUF>
+template <int BN, int STAGES, int NBUF, bool Q8 = false>
 static int csk_max_clusters(int S) {
   static int cache[kCskMaxSplits + 1] = {0};
   if (cache[S] != 0) return cache[S];
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(S * 64); cfg.blockDim = dim3(kCskThreads); cfg.dynamicSmemBytes = CskCfg<BN, STAGES, NBUF>::SMEM_BYTES;
+  cfg.gridDim = dim3(S * 64); cfg.blockDim = dim3(kCskThreads); cfg.dynamicSmemBytes = CskCfg<BN, STAGES, NBUF, Q8>::SMEM_BYTES;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = S; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
   int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, gemm_csk_kernel<BN, STAGES, NBUF>, &cfg) != cudaSuccess || n <= 0) {
+  if (cudaOccupancyMaxActiveClusters(&n, gemm_csk_kernel<BN, STAGES, NBUF, Q8>, &cfg) != cudaSuccess || n <= 0) {
     (void)cudaGetLastError();
     n = (2 * num_sms()) / S * 3 / 4;                 // conservative fallback
     if (n < 1) n = 1;
@@ -383,29 +444,29 @@ static int csk_max_clusters(int S) {
   // The cluster occupancy query counts ONE CTA per SM on this driver even when two fit (shared memory, registers and the plain
   // per-SM occupancy query all allow 2): scale by the per-SM block occupancy, capped at 2 (the launch bound).
   int per_sm = 1;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_csk_kernel<BN, STAGES, NBUF>, kCskThreads, CskCfg<BN, STAGES, NBUF>::SMEM_BYTES) != cudaSuccess) { (void)cudaGetLastError(); per_sm = 1; }
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_csk_kernel<BN, STAGES, NBUF, Q8>, kCskThreads, CskCfg<BN, STAGES, NBUF, Q8>::SMEM_BYTES) != cudaSuccess) { (void)cudaGetLastError(); per_sm = 1; }
   if (per_sm > 2) per_sm = 2;
   // Both occupancy queries may answer 1 block per SM for this cluster launch while the kernel is sized for 2 CTAs per SM (launch
   // bound, <= 113 KB of shared memory each), so that is what the launch assumes; VCLA_CSK_OCC=1 restores the query's answer.
   int mult = 2;
   if (const char* e = getenv("VCLA_CSK_OCC")) { const int v = atoi(e); if (v >= 1 && v <= 2) mult = v; }
-  if (getenv("VCLA_DEBUG")) fprintf(stderr, "[vcla] gemm_csk<%d,%d> S=%d: cluster query %d, blocks/SM %d, using x%d\n", BN, STAGES, S, n, per_sm, mult);
+  if (getenv("VCLA_DEBUG")) fprintf(stderr, "[vcla] gemm_csk<%d,%d%s> S=%d: cluster query %d, blocks/SM %d, using x%d\n", BN, STAGES, Q8 ? ",q8" : "", S, n, per_sm, mult);
   n *= mult;
   cache[S] = n;
   return n;
 }
 
-template <int BN, int STAGES, int NBUF>
+template <int BN, int STAGES, int NBUF, bool Q8 = false>
 static int csk_launch(const CskCall& c, CskParams p, cudaStream_t st) {
   CUtensorMap tw, tx;
-  if (csk_tmap(&tw, c.W, c.M, c.K, c.K, kCskBlockM)) return -1;
+  if (Q8 ? csk_tmap(&tw, c.Wq, c.M, c.K, c.K, kCskBlockM, true) : csk_tmap(&tw, c.W, c.M, c.K, c.K, kCskBlockM)) return -1;
   if (csk_tmap(&tx, c.X, c.B, c.K, c.K, BN)) return -1;
-  int ncl = csk_max_clusters<BN, STAGES, NBUF>(p.splits);
+  int ncl = csk_max_clusters<BN, STAGES, NBUF, Q8>(p.splits);
   if (ncl > p.m_tiles) ncl = p.m_tiles;
   p.n_clusters = ncl;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(ncl * p.splits); cfg.blockDim = dim3(kCskThreads); cfg.dynamicSmemBytes = CskCfg<BN, STAGES, NBUF>::SMEM_BYTES; cfg.stream = st;
+  cfg.gridDim = dim3(ncl * p.splits); cfg.blockDim = dim3(kCskThreads); cfg.dynamicSmemBytes = CskCfg<BN, STAGES, NBUF, Q8>::SMEM_BYTES; cfg.stream = st;
   cudaLaunchAttribute attr[2];
   int na = 0;
   attr[na].id = cudaLaunchAttributeClusterDimension;
@@ -413,7 +474,7 @@ static int csk_launch(const CskCall& c, CskParams p, cudaStream_t st) {
   ++na;
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = attr; cfg.numAttrs = na;
-  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_csk_kernel<BN, STAGES, NBUF>, tw, tx, p));
+  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_csk_kernel<BN, STAGES, NBUF, Q8>, tw, tx, p));
   return 0;
 }
 
@@ -431,9 +492,16 @@ static bool csk_double_buffered(int B) {
   return B <= 16;
 }
 
-int gemm_csk_clusters(int B, int splits) {
+// int8 weights: half the A stage, so every batch tile is double buffered with a deeper ring, and batches 33..64 get a 64-column tile
+static int csk_q8_bn(int B) { return B <= 16 ? 16 : (B <= 32 ? 32 : 64); }
+
+int gemm_csk_clusters(int B, int splits, bool q8) {
   if (csk_init()) return -1;
   if (splits < 1 || splits > kCskMaxSplits) return -1;
+  if (q8) {
+    const int bn = csk_q8_bn(B);
+    return bn == 16 ? csk_max_clusters<16, 8, 2, true>(splits) : bn == 32 ? csk_max_clusters<32, 6, 2, true>(splits) : csk_max_clusters<64, 4, 1, true>(splits);
+  }
   if (csk_double_buffered(B)) return B <= 16 ? csk_max_clusters<16, 4, 2>(splits) : csk_max_clusters<32, 3, 2>(splits);
   return B <= 16 ? csk_max_clusters<16, 5, 1>(splits) : csk_max_clusters<32, 4, 1>(splits);
 }
@@ -441,7 +509,9 @@ int gemm_csk_clusters(int B, int splits) {
 int gemm_csk(const CskCall& c, cudaStream_t st) {
   if (csk_init()) return -1;
   if (c.M <= 0 || c.B <= 0 || c.K <= 0 || c.K % 8 != 0) { set_error("gemm_csk: bad problem (M %d B %d K %d)", c.M, c.B, c.K); return -1; }
-  if (c.B > 32) { set_error("gemm_csk: batch %d > 32 (use the split-K workspace path)", c.B); return -1; }
+  const bool q8 = c.Wq != nullptr;
+  if (q8 && (c.wscale == nullptr || c.K % kCskBlockK != 0)) { set_error("gemm_csk: int8 weights need row scales and K %% 64 == 0 (K %d)", c.K); return -1; }
+  if (c.B > (q8 ? 64 : 32)) { set_error("gemm_csk: batch %d > %d (use the split-K workspace path)", c.B, q8 ? 64 : 32); return -1; }
   if (c.splits < 1 || c.splits > kCskMaxSplits) { set_error("gemm_csk: splits %d unsupported (1..%d)", c.splits, kCskMaxSplits); return -1; }
   CskParams p;
   memset(&p, 0, sizeof(p));
@@ -455,12 +525,17 @@ int gemm_csk(const CskCall& c, cudaStream_t st) {
   p.ssq_in = c.ssq_in; p.ssq_slots = c.ssq_slots; p.inv_dim = c.inv_dim; p.eps = c.eps;
   p.policy_w = kEvictFirst; p.policy_x = kEvictLast;
   { static int fence = -1; if (fence < 0) { const char* e = getenv("VCLA_CSK_FENCE"); fence = e ? atoi(e) : 0; } p.cluster_fence = fence; }
+  p.wscale = c.wscale;
   if (c.mode == CSK_OUT_F32 && (!c.out || c.ldo < c.M)) { set_error("gemm_csk: OUT_F32 needs out / ldo"); return -1; }
   if (c.mode == CSK_RESID && (!c.resid || !c.norm_w || !c.xw || !c.ssq_out)) { set_error("gemm_csk: RESID needs resid / norm_w / xw / ssq_out"); return -1; }
   if (c.mode == CSK_SWIGLU && (!c.h || (c.M % 64) != 0)) { set_error("gemm_csk: SWIGLU needs h and rows %% 64 == 0"); return -1; }
   {
-    const int cols_per = (c.B + p.splits - 1) / p.splits, bn = c.B <= 16 ? 16 : 32;
+    const int cols_per = (c.B + p.splits - 1) / p.splits, bn = q8 ? csk_q8_bn(c.B) : (c.B <= 16 ? 16 : 32);
     if (cols_per * p.splits > bn + 4) { set_error("gemm_csk: %d splits of batch %d need %d reduce columns (max %d)", p.splits, c.B, cols_per * p.splits, bn + 4); return -1; }
+  }
+  if (q8) {
+    const int bn = csk_q8_bn(c.B);
+    return bn == 16 ? csk_launch<16, 8, 2, true>(c, p, st) : bn == 32 ? csk_launch<32, 6, 2, true>(c, p, st) : csk_launch<64, 4, 1, true>(c, p, st);
   }
   if (csk_double_buffered(c.B)) return c.B <= 16 ? csk_launch<16, 4, 2>(c, p, st) : csk_launch<32, 3, 2>(c, p, st);
   return c.B <= 16 ? csk_launch<16, 5, 1>(c, p, st) : csk_launch<32, 4, 1>(c, p, st);

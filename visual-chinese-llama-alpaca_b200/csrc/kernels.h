@@ -87,6 +87,7 @@ struct GemmCall {
   GemmRowScale rowscale;     // deferred RMSNorm scale of the A rows (STORE_BF16 / SWIGLU_BF16)
   GemmEmitNorm emit;         // ADD_F32 + accumulate: also write the next operand + row statistics
   GemmRope rope;             // STORE_BF16: RoPE + KV-cache append (runs on the 64 x 256 tile, N = 3T)
+  const float* colscale = nullptr;   // [N] or null: acc[row, col] *= colscale[col] before every epilogue (per-row scales of int8 weights)
 };
 int gemm_tc(const GemmCall& c, cudaStream_t st);
 int gemm_pick_bn(int M, int N);   // tile width gemm_tc picks for a non-swap GEMM (= the number of ssq slots per row it emits: ceil(N / bn))
@@ -105,6 +106,7 @@ enum CskMode {
 };
 struct CskCall {
   const bf16* W = nullptr; const bf16* X = nullptr;
+  const int8_t* Wq = nullptr; const float* wscale = nullptr;   // int8 weights instead of W (k in fragment order, quant.cu) + fp32 row scales
   int M = 0, B = 0, K = 0;
   int splits = 1;                       // CTAs per cluster = K slices (1..8, every slice non-empty)
   int mode = CSK_OUT_F32;
@@ -114,7 +116,7 @@ struct CskCall {
   const float* ssq_in = nullptr; int ssq_slots = 0; float inv_dim = 0.f, eps = 0.f;   // rstd[b] = rsqrt(sum_slots ssq_in[b][slot] * inv_dim + eps); null: 1
 };
 int gemm_csk(const CskCall& c, cudaStream_t st);
-int gemm_csk_clusters(int B, int splits);   // clusters of `splits` CTAs that can be co-resident (occupancy query, cached)
+int gemm_csk_clusters(int B, int splits, bool q8 = false);   // clusters of `splits` CTAs that can be co-resident (occupancy query, cached)
 int trace_set_gemm(void* buf, unsigned long long cap);
 int trace_set_attention(void* buf, unsigned long long cap);
 int trace_set_gemm_decode(void* buf, unsigned long long cap);
@@ -303,5 +305,16 @@ int convert_to_f32(const void* src, int dtype, int64_t n, float* dst, cudaStream
 int copy_rows_bf16(const bf16* src, int rows, int cols, bf16* dst, int ld, cudaStream_t st);
 // interleave gate/up rows in blocks of 32: dst[(j/32)*64 + which*32 + j%32, :] = src[j, :]
 int interleave_rows32(const bf16* src, int rows, int cols, int which, bf16* dst, cudaStream_t st);
+
+// ---- weight-only int8 (quant.cu): one fp32 scale per row, q = clamp(rint(w * (127 / absmax)), -127, 127), s = absmax / 127 ---------
+// Stored rows keep the k of each 64-column block in the decode kernel's fragment order (gemm_decode.cu); `which` >= 0 places logical row
+// r at the gate/up interleave row (r / 32) * 64 + which * 32 + r % 32, -1 at row r.
+int quantize_rows_q8(const void* src, int dtype, int rows, int cols, int which, int8_t* q, float* scale, cudaStream_t st);
+// caller's logical int8 rows + scales -> stored rows
+int place_rows_q8(const int8_t* q_src, const float* s_src, int rows, int cols, int which, int8_t* q, float* scale, cudaStream_t st);
+// stored rows -> logical order: int8 + scales, and/or fp32 q * s (any output may be null)
+int read_rows_q8(const int8_t* q, const float* scale, int rows, int cols, int which, int8_t* q_out, float* s_out, float* f32_out, cudaStream_t st);
+// bf16(q) of `rows` rows with k in logical order (permuted != 0: stored fragment order, else already logical): the prefill GEMM operand
+int expand_rows_q8(const int8_t* q, int rows, int cols, int permuted, bf16* out, cudaStream_t st);
 
 }  // namespace vcla

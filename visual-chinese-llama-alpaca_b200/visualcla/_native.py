@@ -19,6 +19,7 @@ class VclaConfig(C.Structure):
         ("t_hidden", C.c_int), ("t_layers", C.c_int), ("t_heads", C.c_int), ("t_ffn", C.c_int),
         ("t_vocab", C.c_int), ("t_eps", C.c_float), ("rope_theta", C.c_float),
         ("max_batch", C.c_int), ("max_seq", C.c_int), ("max_prefill_tokens", C.c_int), ("page_tokens", C.c_int),
+        ("weight_format", C.c_int),
     ]
 
 
@@ -54,6 +55,8 @@ _SIGNATURES = [
     ("vcla_load_weight", C.c_int, [_P, C.c_char_p, _P, C.c_int, C.c_int64, C.c_int, _P]),
     ("vcla_read_weight", C.c_int, [_P, C.c_char_p, _P, _P]),
     ("vcla_init_synthetic", C.c_int, [_P, C.c_uint32, _P]),
+    ("vcla_read_weight_q8", C.c_int, [_P, C.c_char_p, _P, _P, _P]),
+    ("vcla_load_weight_q8", C.c_int, [_P, C.c_char_p, _P, _P, C.c_int, _P]),
     ("vcla_reset", C.c_int, [_P, _P]),
     ("vcla_kv_geometry", C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("vcla_kv_read_pages", C.c_int, [_P, _P, _P, _P]),
@@ -84,6 +87,8 @@ _SIGNATURES = [
     ("vcla_op_gemm", C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     ("vcla_op_gemm_csk", C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, _P]),
     ("vcla_op_gemm_csk_clusters", C.c_int, [C.c_int, C.c_int]),
+    ("vcla_op_gemm_csk_q8", C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_float, C.c_float, _P]),
+    ("vcla_op_gemm_q8", C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P]),
     ("vcla_debug_set_csk_splits", C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     ("vcla_debug_get_csk_splits", C.c_int, [_P, C.c_int, C.POINTER(C.c_int * 5)]),
     ("vcla_set_attention_tc", None, [C.c_int]),

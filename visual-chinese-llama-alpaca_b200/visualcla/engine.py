@@ -23,8 +23,10 @@ def path_config_7b() -> Dict:
 
 
 class Engine:
+    WEIGHT_BF16, WEIGHT_INT8 = 0, 1      # weight_format: storage of the LLaMA projections (int8 = load_in_8bit, include/vcla.h)
+
     def __init__(self, path_cfg: Dict, max_batch: int = 8, max_seq: int = 512, max_prefill_tokens: Optional[int] = None,
-                 device: Optional[torch.device] = None, page_tokens: int = 64):
+                 device: Optional[torch.device] = None, page_tokens: int = 64, weight_format: int = 0):
         if not torch.cuda.is_available():
             raise N.NativeError("visualcla (H100) needs a CUDA device: there is no CPU fallback")
         self.lib = N.load()
@@ -35,7 +37,8 @@ class Engine:
         self.max_batch, self.max_seq = int(max_batch), int(max_seq)
         self.max_prefill_tokens = int(max_prefill_tokens or max_batch * max_seq)
         cfg = N.VclaConfig(**self.path_cfg, max_batch=self.max_batch, max_seq=self.max_seq,
-                           max_prefill_tokens=self.max_prefill_tokens, page_tokens=page_tokens)
+                           max_prefill_tokens=self.max_prefill_tokens, page_tokens=page_tokens, weight_format=int(weight_format))
+        self.weight_format = int(weight_format)
         self._ctx = C.c_void_p()
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_create(C.byref(cfg), C.byref(self._ctx)), "vcla_create")
@@ -70,7 +73,7 @@ class Engine:
 
     # ---- weights ----------------------------------------------------------------------------
     def weight_table(self):
-        """[(name, shape, kind)] in the reference's state-dict naming; kind 0 = bf16 matrix, 1 = f32 vector."""
+        """[(name, shape, kind)] in the reference's state-dict naming; kind 0 = bf16 matrix, 1 = f32 vector, 2 = int8 matrix + row scales."""
         if self._names is None:
             out = []
             for i in range(self.lib.vcla_weight_count(self._ctx)):
@@ -119,12 +122,33 @@ class Engine:
         return loaded, unexpected
 
     def read_weight(self, name: str) -> torch.Tensor:
-        table = {n: (s, k) for n, s, k in self.weight_table()}
-        shape, kind = table[name]
+        """Host copy of one logical tensor: bf16 for kind 0, fp32 for kind 1 and for kind 2 (the int8 rows dequantised, q * s)."""
+        shape, kind = self._table()[name]
         out = torch.empty(shape, dtype=torch.bfloat16 if kind == 0 else torch.float32)
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_read_weight(self._ctx, name.encode(), N.ptr(out), self._stream()), f"vcla_read_weight({name})")
         return out
+
+    def read_weight_q8(self, name: str) -> Tuple[torch.Tensor, torch.Tensor]:
+        """-> (q int8 (rows, cols), scale f32 (rows,)) host tensors of an int8 tensor (kind 2), exactly as stored."""
+        shape, _kind = self._table()[name]
+        q = torch.empty(shape, dtype=torch.int8)
+        s = torch.empty(shape[0], dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_read_weight_q8(self._ctx, name.encode(), N.ptr(q), N.ptr(s), self._stream()), f"vcla_read_weight_q8({name})")
+        return q, s
+
+    def load_weight_q8(self, name: str, q: torch.Tensor, scale: torch.Tensor):
+        """Store int8 rows + fp32 row scales of an int8 tensor (kind 2) exactly (no requantisation)."""
+        shape, _kind = self._table()[name]
+        if tuple(q.shape) != tuple(shape) or q.dtype != torch.int8 or tuple(scale.shape) != (shape[0],):
+            raise ValueError(f"{name}: expected int8 {tuple(shape)} and scales ({shape[0]},), got {q.dtype} {tuple(q.shape)} / {tuple(scale.shape)}")
+        q = q.detach().contiguous()
+        s = scale.detach().to(q.device, torch.float32).contiguous()
+        self.session += 1
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_load_weight_q8(self._ctx, name.encode(), N.ptr(q), N.ptr(s), 1 if q.is_cuda else 0, self._stream()),
+                    f"vcla_load_weight_q8({name})")
 
     def init_synthetic(self, seed: int = 0):
         self.session += 1

@@ -56,7 +56,11 @@ def fold(w: torch.Tensor, A: torch.Tensor, B: torch.Tensor, scaling: float, fan_
 
 
 def load_lora(model, lora_dir: str, strict: bool = True):
-    """Fold an unmerged VisualCLA LoRA checkpoint directory (adapter_config.json + adapter_model.bin) into `model`."""
+    """Fold an unmerged VisualCLA LoRA checkpoint directory (adapter_config.json + adapter_model.bin) into `model`.
+
+    On a load_in_8bit model the int8 projections are folded as quantise(q * s + scaling * B @ A): the delta is added to the
+    dequantised weight and the sum is quantised again.  PEFT instead keeps the delta unmerged beside the int8 base, so the two
+    differ by the int8 rounding of the delta."""
     with open(os.path.join(lora_dir, "adapter_config.json")) as f:
         cfg = json.load(f)
     scaling = float(cfg["lora_alpha"]) / float(cfg["r"])

@@ -105,15 +105,17 @@ class VisualCLAModel:
 
     def __init__(self, config: VisualCLAConfig = None, vision_model=None, text_model=None, device=None,
                  max_batch: int = 8, max_seq: int = 1024, max_prefill_tokens: Optional[int] = None,
-                 torch_dtype=torch.bfloat16):
+                 torch_dtype=torch.bfloat16, load_in_8bit: bool = False):
         if config is None:
             raise ValueError("VisualCLAModel needs a VisualCLAConfig")
         if vision_model is not None or text_model is not None:
             raise NotImplementedError("pre-built nn.Module sub-models are not used on the H100 path; load weights with "
                                       "from_merged_pretrained / from_vision_text_pretrained / load_state_dict")
         self.config = config
-        self._engine = Engine(config.to_path_config(), max_batch=max_batch, max_seq=max_seq,
-                              max_prefill_tokens=max_prefill_tokens, device=device)
+        # load_in_8bit: the seven LLaMA projections of every layer become weight-only int8 with per-row scales (what bitsandbytes
+        # converts in the reference, modeling_visualcla.py:151-156); everything else stays as it is
+        self._engine = Engine(config.to_path_config(), max_batch=max_batch, max_seq=max_seq, max_prefill_tokens=max_prefill_tokens,
+                              device=device, weight_format=Engine.WEIGHT_INT8 if load_in_8bit else Engine.WEIGHT_BF16)
         self.dtype = torch.bfloat16      # compute dtype of the path (bf16 operands, fp32 accumulate / residual stream)
         self.requested_dtype = torch_dtype
         self.image_at_head = True        # constructor default of the reference (:108); the loader flips it (:134)
@@ -154,6 +156,8 @@ class VisualCLAModel:
         return iter(())
 
     def state_dict(self) -> Dict[str, torch.Tensor]:
+        """Host copies of every tensor.  With load_in_8bit the int8 projections come back as fp32 q * s, so save_merged_pretrained writes
+        them twice the size of bf16; loading that checkpoint with load_in_8bit=True quantises q * s again and reproduces q."""
         return {n: self._engine.read_weight(n) for n, _s, _k in self._engine.weight_table()}
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
@@ -176,11 +180,15 @@ class VisualCLAModel:
         old = self._engine.vocab
         if new_num_tokens is None or new_num_tokens == old:
             return self.get_input_embeddings()
-        sd = self.state_dict()
+        e = self._engine
+        q8 = [n for n, _s, kind in e.weight_table() if kind == 2]
+        sd = {n: e.read_weight(n) for n, _s, kind in e.weight_table() if kind != 2}
         cfg = copy.deepcopy(self.config)
         cfg.text_config["vocab_size"] = int(new_num_tokens)
-        e = self._engine
-        new = Engine(cfg.to_path_config(), max_batch=e.max_batch, max_seq=e.max_seq, max_prefill_tokens=e.max_prefill_tokens, device=e.device)
+        new = Engine(cfg.to_path_config(), max_batch=e.max_batch, max_seq=e.max_seq, max_prefill_tokens=e.max_prefill_tokens, device=e.device,
+                     weight_format=e.weight_format)
+        for n in q8:                        # int8 tensors move as stored (quantising q * s again could change them)
+            new.load_weight_q8(n, *e.read_weight_q8(n))
         for k in ("text_model.model.embed_tokens.weight", "text_model.lm_head.weight"):
             w = sd.pop(k).float()
             grown = torch.zeros(new_num_tokens, w.shape[1])
@@ -218,7 +226,7 @@ class VisualCLAModel:
         if os.path.isdir(os.path.join(path, "text_encoder")):
             return cls.from_merged_pretrained(path, **kw, **kwargs)
         config = VisualCLAConfig.from_pretrained(path)
-        model = cls(config, device=kw["default_device"], torch_dtype=kw["torch_dtype"], **kwargs)
+        model = cls(config, device=kw["default_device"], torch_dtype=kw["torch_dtype"], load_in_8bit=kw["load_in_8bit"], **kwargs)
         model.load_state_dict(dict(_iter_checkpoint(path)))
         return model
 
@@ -232,8 +240,6 @@ class VisualCLAModel:
         default_device = kwargs.pop("default_device")
         _device_map = kwargs.pop("device_map")          # whole model lives on one GPU (14.5 GB of 180 GB); DP replicates it
         load_in_8bit = kwargs.pop("load_in_8bit")
-        if load_in_8bit:
-            raise NotImplementedError("load_in_8bit (bitsandbytes) is out of scope of the H100 path (bf16 weights)")
         config = VisualCLAConfig.from_pretrained(path)
         text_dir, vision_dir = os.path.join(path, "text_encoder"), os.path.join(path, "vision_encoder")
         with open(os.path.join(text_dir, "config.json")) as f:
@@ -241,7 +247,7 @@ class VisualCLAModel:
         with open(os.path.join(vision_dir, "config.json")) as f:
             vc = json.load(f)
             config.vision_config = vc.get("vision_config", vc) if "hidden_size" not in vc else vc
-        model = cls(config, device=default_device, torch_dtype=torch_dtype, **kwargs)
+        model = cls(config, device=default_device, torch_dtype=torch_dtype, load_in_8bit=bool(load_in_8bit), **kwargs)
         eng = model._engine
         seen = set()
         for k, v in _iter_checkpoint(text_dir):
@@ -270,8 +276,6 @@ class VisualCLAModel:
             raise ValueError("If `vision_model` is not defined as an argument, a `vision_model_name_or_path` has to be defined")
         if text_model_name_or_path is None:
             raise ValueError("If `text_model` is not defined as an argument, a `text_model_name_or_path` has to be defined")
-        if load_in_8bit:
-            raise NotImplementedError("load_in_8bit is out of scope of the H100 path")
         if isinstance(visualcla_config, str):
             visualcla_config = VisualCLAConfig.from_pretrained(visualcla_config)
         config = copy.deepcopy(visualcla_config)
@@ -280,7 +284,7 @@ class VisualCLAModel:
         with open(os.path.join(vision_model_name_or_path, "config.json")) as f:
             vc = json.load(f)
             config.vision_config = vc.get("vision_config", vc) if "hidden_size" not in vc else vc
-        model = cls(config, device=default_device, torch_dtype=torch_dtype, **kwargs)
+        model = cls(config, device=default_device, torch_dtype=torch_dtype, load_in_8bit=bool(load_in_8bit), **kwargs)
         eng = model._engine
         eng.init_synthetic(0)   # resampler + projector: fresh init, as in the reference
         known = {n for n, _s, _k in eng.weight_table()}
