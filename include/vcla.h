@@ -323,6 +323,29 @@ int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v
 int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, const int32_t* page_table, int pages_per_seq,
                             int page_tokens, const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T, float scale,
                             vcla_stream stream);
+/* The decode attention of vcla_decode_step on caller buffers (head dim 128), context-free: one new token per sequence.  In one launch
+ * it sums the fused-QKV split-K partials qkv_partial f32 [splits][B][3*H*128] (q | k | v, split order 0..splits-1), applies RoPE at
+ * position seq_len[b] to q and k, rounds k and v to bf16 and WRITES them into the pool at (page_table[b][seq_len[b] / page_tokens], slot
+ * seq_len[b] % page_tokens) -- nothing else in the pool is written --, and attends over the seq_len[b] cached rows plus the new one.
+ *   kv_pages      the layer pool [pages][K|V][H][page_tokens][128] bf16, read and written
+ *   page_table    int32 (B, pages_per_seq); only entries 0 .. seq_len[b] / page_tokens of a row are read
+ *   seq_len_dev   int32 (B): cached tokens per sequence, 0 allowed (the output is then the new token's v); not advanced by the call
+ *   out           bf16 (B, H*128)
+ *   kv_splits     1..8 CTAs per (sequence, head), combined in split order through a scratch and self-resetting counters
+ *   persistent    0 = the one-shot kernel, 1 = the persistent kernel (kv_splits must be 1) on a grid of persistent_grid CTAs (0 = default)
+ *   launches      >= 1: the kernel is enqueued that many times over the same scratch and counters, as graph replays do; the append is
+ *                 idempotent while seq_len is unchanged, so out and the pool do not depend on it.  out is filled with NaN before every
+ *                 launch: what the last launch leaves unwritten stays NaN
+ * The RoPE tables (positions 0 .. max seq_len), scratch and counters are made for the call.  Refused on the host, before any launch:
+ * seq_len[b] < 0 or seq_len[b] + 1 > pages_per_seq * page_tokens, a negative page among the entries read, page_tokens not a multiple of 8
+ * in 8..64, kv_splits outside 1..8, persistent with kv_splits > 1, B > 64.  Synchronises. */
+int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq,
+                             int page_tokens, const int32_t* seq_len_dev, void* out, int B, int H, int kv_splits, float scale,
+                             float rope_theta, int persistent, int persistent_grid, int launches, vcla_stream stream);
+/* The greedy pick of vcla_decode_step on caller buffers: logits_out f32 (B, V) or NULL = sum over splits (in split order) of partial f32
+ * [splits][B][ldp] (ldp >= V; columns >= V are not read), tok_out int32 (B) = its argmax, the smallest index among equal maxima as
+ * torch.argmax; a row that is -inf everywhere gives 0.  Synchronises. */
+int vcla_op_logits_argmax(const float* partial, int splits, int ldp, int B, int V, float* logits_out, int32_t* tok_out, vcla_stream stream);
 int vcla_op_layernorm(const float* x, int rows, int D, const float* w, const float* b, float eps, void* y_bf16, float* y_f32,
                       vcla_stream stream);
 int vcla_op_rmsnorm(const float* x, int rows, int D, const float* w, float eps, void* y_bf16, vcla_stream stream);

@@ -723,7 +723,7 @@ int attention_init() {
 
 int attention_decode(const DecodeAttnCall& c, cudaStream_t st) {
   if (c.HD != 128) { set_error("attention_decode: head dim %d unsupported (128)", c.HD); return -1; }
-  if (c.page_tokens > kDecMaxPT || c.page_tokens % 8 != 0) { set_error("attention_decode: page_tokens %d unsupported (<= %d, multiple of 8)", c.page_tokens, kDecMaxPT); return -1; }
+  if (c.page_tokens < 8 || c.page_tokens > kDecMaxPT || c.page_tokens % 8 != 0) { set_error("attention_decode: page_tokens %d unsupported (8..%d, multiple of 8)", c.page_tokens, kDecMaxPT); return -1; }
   if (c.rope_cos == nullptr || c.rope_sin == nullptr) { set_error("attention_decode: rope table not initialised"); return -1; }
   if (attention_init()) return -1;
   cudaLaunchConfig_t cfg = {};

@@ -426,8 +426,10 @@ __global__ void dec_logits_stage1(const float* __restrict__ partial, int splits,
   const int b = blockIdx.y, ch = blockIdx.x;
   const int per = (V + kArgChunks - 1) / kArgChunks;
   const int v0 = ch * per, v1 = min(V, v0 + per);
+  // a thread starts from its own first column, so a row that is -inf everywhere still yields a column of the row (index 0 after
+  // the tie rule, as torch.argmax); threads and chunks without a column keep the sentinel and lose every tie
   float best = -INFINITY;
-  int bi = 0x7fffffff;
+  int bi = (v0 + (int)threadIdx.x < v1) ? v0 + (int)threadIdx.x : 0x7fffffff;
   for (int v = v0 + threadIdx.x; v < v1; v += blockDim.x) {
     float x = 0.f;
     for (int s = 0; s < splits; ++s) x += __ldcg(partial + ((size_t)s * ws_rows + b) * (size_t)ldp + v);

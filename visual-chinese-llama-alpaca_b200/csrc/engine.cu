@@ -1754,6 +1754,65 @@ int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, c
   cudaFree(scratch);
   return rc;
 }
+int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq, int page_tokens,
+                             const int32_t* seq_len_dev, void* out, int B, int H, int kv_splits, float scale, float rope_theta, int persistent,
+                             int persistent_grid, int launches, vcla_stream stream) {
+  // operator entry for tests: goes through attention_decode() (the dispatch is under test too); the RoPE tables, the combine scratch
+  // and the arrival counters are made for the call.  Everything a kernel would index with is checked here first.  Synchronises.
+  if (!qkv_partial || !kv_pages || !page_table || !seq_len_dev || !out || splits < 1 || B < 1 || B > 64 || H < 1 || pages_per_seq < 1 ||
+      page_tokens < 1 || launches < 1 || persistent_grid < 0 || !(rope_theta > 0.f)) {
+    set_error("vcla_op_attention_decode: bad arguments"); return -1;
+  }
+  if (kv_splits < 1 || kv_splits > 8) { set_error("vcla_op_attention_decode: kv_splits %d outside 1..8", kv_splits); return -1; }
+  if (persistent != 0 && persistent != 1) { set_error("vcla_op_attention_decode: persistent must be 0 or 1"); return -1; }
+  if (persistent && kv_splits != 1) { set_error("vcla_op_attention_decode: the persistent kernel requires kv_splits == 1 (got %d)", kv_splits); return -1; }
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<int32_t> table((size_t)B * pages_per_seq), len((size_t)B);
+  VCLA_CUDA_OK(cudaStreamSynchronize(st));
+  VCLA_CUDA_OK(cudaMemcpy(table.data(), page_table, table.size() * 4, cudaMemcpyDeviceToHost));
+  VCLA_CUDA_OK(cudaMemcpy(len.data(), seq_len_dev, len.size() * 4, cudaMemcpyDeviceToHost));
+  int max_len = 0;
+  for (int b = 0; b < B; ++b) {
+    if (len[b] < 0 || (int64_t)len[b] + 1 > (int64_t)pages_per_seq * page_tokens) {
+      set_error("vcla_op_attention_decode: sequence %d (%d + 1 tokens) exceeds its table row (%d pages of %d)", b, len[b], pages_per_seq, page_tokens); return -1;
+    }
+    for (int i = 0; i <= len[b] / page_tokens; ++i) {
+      if (table[(size_t)b * pages_per_seq + i] < 0) { set_error("vcla_op_attention_decode: sequence %d has no page %d", b, i); return -1; }
+    }
+    max_len = std::max(max_len, len[b]);
+  }
+  const size_t rope_floats = (size_t)(max_len + 1) * 64, scratch_floats = (size_t)B * H * kv_splits * (128 + 2);
+  float* buf = nullptr;
+  VCLA_CUDA_OK(cudaMalloc(&buf, (2 * rope_floats + scratch_floats + (size_t)B * H) * 4));
+  DecodeAttnCall a; a.qkv_partial = qkv_partial; a.splits = splits; a.ws_rows = B; a.kv_pages = (bf16*)kv_pages; a.page_table = page_table;
+  a.pages_per_seq = pages_per_seq; a.page_tokens = page_tokens; a.seq_len = seq_len_dev; a.out = (bf16*)out; a.B = B; a.H = H; a.HD = 128;
+  a.kv_splits = kv_splits; a.scale = scale; a.rope_theta = rope_theta; a.rope_cos = buf; a.rope_sin = buf + rope_floats;
+  a.scratch = buf + 2 * rope_floats; a.counters = reinterpret_cast<int32_t*>(a.scratch + scratch_floats);
+  a.persistent_mode = persistent ? 2 : 0; a.persistent_grid = persistent_grid;
+  int rc = rope_fill_tables(max_len + 1, 128, rope_theta, buf, buf + rope_floats);
+  if (rc == 0 && cudaMemsetAsync(a.scratch, 0, (scratch_floats + (size_t)B * H) * 4, st) != cudaSuccess) { set_error("vcla_op_attention_decode: memset failed"); rc = -1; }
+  // every launch runs over the same scratch and counters, as the replays of a decode graph do; out is NaN before each, so an
+  // element the last launch did not write cannot pass for one an earlier launch wrote
+  for (int i = 0; i < launches && rc == 0; ++i) {
+    if (cudaMemsetAsync(out, 0xff, (size_t)B * H * 128 * 2, st) != cudaSuccess) { set_error("vcla_op_attention_decode: memset failed"); rc = -1; break; }
+    rc = attention_decode(a, st);
+  }
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_attention_decode: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
+  cudaFree(buf);
+  return rc;
+}
+int vcla_op_logits_argmax(const float* partial, int splits, int ldp, int B, int V, float* logits_out, int32_t* tok_out, vcla_stream stream) {
+  // operator entry for tests: dec_logits_argmax without token history or data-parallel send buffer.  Synchronises.
+  if (!partial || !tok_out || splits < 1 || B < 1 || V < 1 || ldp < V) { set_error("vcla_op_logits_argmax: bad arguments"); return -1; }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* cand = nullptr;
+  VCLA_CUDA_OK(cudaMalloc(&cand, (size_t)B * kArgmaxChunks * 8));
+  int rc = dec_logits_argmax(partial, splits, B, ldp, B, V, logits_out, V, tok_out, nullptr, nullptr, cand,
+                             reinterpret_cast<int32_t*>(cand + (size_t)B * kArgmaxChunks), nullptr, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_logits_argmax: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
+  cudaFree(cand);
+  return rc;
+}
 int vcla_op_layernorm(const float* x, int rows, int D, const float* w, const float* b, float eps, void* y_bf16, float* y_f32, vcla_stream stream) {
   return layernorm(x, rows, D, w, b, eps, (bf16*)y_bf16, y_f32, (cudaStream_t)stream);
 }

@@ -212,7 +212,7 @@ int dec_resid_norm(const float* partial, int splits, int ws_rows, float* resid, 
                    bf16* xn, cudaStream_t st);
 // h[b, j] = silu(sum_s p[s][b][g(j)]) * (sum_s p[s][b][u(j)])  with the [32 gate | 32 up] interleave
 int dec_silu_mul(const float* partial, int splits, int ws_rows, int B, int F, bf16* h, cudaStream_t st);
-// logits[b, :] = sum_s partial[s][b][:V] ; tok[b] = argmax (first max wins, like torch.argmax)
+// logits[b, :] = sum_s partial[s][b][:V] ; tok[b] = argmax (first max wins, like torch.argmax; a row that is -inf everywhere gives 0)
 // cand_val / cand_idx: [B][kArgmaxChunks] scratch owned by the context
 constexpr int kArgmaxChunks = 32;
 int dec_logits_argmax(const float* partial, int splits, int ws_rows, int ldp, int B, int V, float* logits, int ld_logits,

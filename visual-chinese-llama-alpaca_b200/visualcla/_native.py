@@ -96,6 +96,9 @@ _SIGNATURES = [
                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _P]),
     ("vcla_op_attention_paged", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_float, _P]),
+    ("vcla_op_attention_decode", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float,
+                                           C.c_float, C.c_int, C.c_int, C.c_int, _P]),
+    ("vcla_op_logits_argmax", C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     ("vcla_op_layernorm", C.c_int, [_P, C.c_int, C.c_int, _P, _P, C.c_float, _P, _P, _P]),
     ("vcla_op_rmsnorm", C.c_int, [_P, C.c_int, C.c_int, _P, C.c_float, _P, _P]),
     ("vcla_bench_decode_gemm", C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int64), _P]),
