@@ -269,6 +269,22 @@ int vcla_dp_set_active(vcla_ctx* ctx, int on);
 int vcla_dp_exchange(vcla_ctx* ctx, vcla_stream stream);
 int vcla_read_history_dp(vcla_ctx* ctx, int32_t* dst_dev, int n_steps, vcla_stream stream);
 
+/* ---- token streaming (models/visualcla/modeling_utils.py:180-247 chat_in_stream; HF generate(streamer=...)) -------------------
+ * While armed, the kernel that advances the sequence lengths after every token choice (the prefill / extend pick and every decode
+ * step, also inside the CUDA graphs) copies that step's tokens into a ring in pinned, mapped host memory and then publishes the step
+ * with a system-scope release store of its counter: the host sees each token as soon as the device has it, with no copy, graph
+ * break or synchronisation per token.  The token-choosing kernels are the same armed or not, so streaming never changes a token.
+ *   vcla_stream_arm    on != 0: allocate the ring (once), reset the published-step counter, bump the epoch; refused while earlier
+ *                      armed work is still in flight, in beam mode and while the data-parallel exchange is active.  on == 0: later
+ *                      enqueues stop publishing (graphs captured armed and disarmed are cached apart)
+ *   vcla_stream_wait   wait until at least `target` steps are published (acquire load); *published = the count seen.  Returns 0
+ *                      on success or when timeout_us (< 0: no limit) expires first (then *published < target); returns an error
+ *                      when all armed work enqueued so far has completed and the count is still below target (it never will be)
+ *   vcla_stream_read   copy published steps [from, to) of B tokens each to a host buffer ([to - from][B] int32) */
+int vcla_stream_arm(vcla_ctx* ctx, int on);
+int vcla_stream_wait(vcla_ctx* ctx, int target, int timeout_us, int* published);
+int vcla_stream_read(vcla_ctx* ctx, int from, int to, int B, int32_t* dst_host);
+
 /* number of this library's kernels launched by the context since the last call with reset != 0 */
 int64_t vcla_kernel_launches(vcla_ctx* ctx, int reset);
 

@@ -576,9 +576,15 @@ int kv_truncate(int32_t* seq_len, const int32_t* len_host, int B, cudaStream_t s
   return 0;
 }
 
+__device__ __forceinline__ void st_release_sys(int32_t* p, int32_t v) {
+  asm volatile("st.release.sys.global.b32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
+}
+
 __global__ void advance_seq_kernel(int32_t* seq_len, int B, int by, const int32_t* __restrict__ left_pad, int32_t* step_idx, int32_t* kv_free,
-                                   int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens) {
+                                   int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens,
+                                   StreamRing* ring, const int32_t* __restrict__ history) {
   __shared__ int s_tokens[64];
+  __shared__ int s_step;
   TraceScope trace(12);
   pdl_launch_dependents();   // dependents may become resident early; they block in their own griddepcontrol.wait
   pdl_wait();
@@ -589,8 +595,23 @@ __global__ void advance_seq_kernel(int32_t* seq_len, int B, int by, const int32_
     seq_len[b] = L;
     s_tokens[b] = L + 1;                 // the next token of this sequence is appended at index L
   }
-  if (step_idx != nullptr && b == 0) *step_idx += 1;
+  if (step_idx != nullptr && b == 0) {
+    const int step = *step_idx;          // this step's tokens (history row `step`) are final: their kernel precedes this one
+    if (ring != nullptr) s_step = step;
+    *step_idx = step + 1;
+  }
   __syncthreads();
+  if (ring != nullptr) {
+    // publish: tokens into the host ring, each writer's stores made visible system-wide, then one release store of the count.
+    // The ring has as many rows as the history (max_seq + 2), so any step whose history row exists has a ring row.
+    const int step = s_step;
+    if (b < B) {
+      ring->tokens[(size_t)step * 64 + b] = history[(size_t)step * B + b];
+      __threadfence_system();
+    }
+    __syncthreads();
+    if (b == 0) st_release_sys(&ring->published, step + 1);
+  }
   if (threadIdx.x == 0) {
     // fast path (every step but one in page_tokens): nobody crosses a page boundary
     bool any = false;
@@ -603,10 +624,12 @@ __global__ void advance_seq_kernel(int32_t* seq_len, int B, int by, const int32_
   }
 }
 int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, int32_t* kv_free, int32_t* kv_state,
-                int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, cudaStream_t st) {
+                int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, cudaStream_t st, StreamRing* ring,
+                const int32_t* history) {
   if (B > 64) { set_error("advance_seq: batch %d > 64", B); return -1; }
+  if (ring != nullptr && (history == nullptr || step_idx == nullptr)) { set_error("advance_seq: publishing needs the token history"); return -1; }
   VCLA_LAUNCH(advance_seq_kernel, dim3(1), dim3(64), 0, st, seq_len, B, by, left_pad, step_idx, kv_free, kv_state, kv_npages, page_table,
-              pages_per_seq, page_tokens);
+              pages_per_seq, page_tokens, ring, (const int32_t*)history);
   return 0;
 }
 

@@ -11,6 +11,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <chrono>
+#include <thread>
 #include <list>
 #include <map>
 #include <string>
@@ -56,6 +58,7 @@ struct TextLayer {
 
 struct GraphKey {
   int B; const void* tok_in; const void* logits; const void* tok_out; int n_steps = 1; int dp = 0; int samp = 0; int beam = 0;
+  int stream = 0;   // captured armed: every step publishes into the token stream ring
   bool operator<(const GraphKey& o) const {
     if (B != o.B) return B < o.B;
     if (tok_in != o.tok_in) return tok_in < o.tok_in;
@@ -64,6 +67,7 @@ struct GraphKey {
     if (dp != o.dp) return dp < o.dp;
     if (samp != o.samp) return samp < o.samp;
     if (beam != o.beam) return beam < o.beam;
+    if (stream != o.stream) return stream < o.stream;
     return tok_out < o.tok_out;
   }
 };
@@ -121,6 +125,10 @@ struct vcla_ctx {
   int32_t *beam_cand_tok = nullptr, *beam_parent = nullptr, *hyp_len = nullptr, *hyp_fin = nullptr, *hyp_tok = nullptr, *hyp_tmp = nullptr;
   int32_t *beam_state = nullptr, *beam_copy = nullptr, *beam_table_tmp = nullptr;
   unsigned long long* beam_cow_bytes = nullptr;
+  // token streaming (vcla_stream_*): ring in pinned, mapped host memory; stream_done is recorded after every armed enqueue
+  StreamRing *ring_host = nullptr, *ring_dev = nullptr; bool stream_armed = false;
+  cudaEvent_t stream_done = nullptr; bool stream_pending = false;
+  StreamRing* ring() const { return stream_armed ? ring_dev : nullptr; }
   int64_t len_bound = 0;   // host-side upper bound of the cached tokens per sequence (prefill S + decode steps issued since)
   int resident_b = 0;      // sequences resident since the last vcla_prefill (0 after vcla_reset)
   // vision activations
@@ -578,6 +586,8 @@ void vcla_destroy(vcla_ctx* c) {
   if (c->dp_join) cudaEventDestroy(c->dp_join);
   if (c->cap_stream) cudaStreamDestroy(c->cap_stream);
   if (c->trace_buf) { trace_set_all(nullptr, 0); cudaFree(c->trace_buf); }
+  if (c->ring_host) { if (c->stream_pending) cudaEventSynchronize(c->stream_done); cudaFreeHost(c->ring_host); }
+  if (c->stream_done) cudaEventDestroy(c->stream_done);
   delete c;
 }
 
@@ -1084,6 +1094,14 @@ static int prefill_logits(vcla_ctx* c, int B, int S, float* logits_all, float* l
 
 static int beam_reorder(vcla_ctx* c, int rows_old, int rows_new, const int32_t* tok, cudaStream_t st);
 
+// after every enqueue that publishes into the token stream ring: lets vcla_stream_wait tell "not yet" from "never"
+static int stream_mark(vcla_ctx* c, cudaStream_t st) {
+  if (!c->stream_armed) return 0;
+  VCLA_CUDA_OK(cudaEventRecord(c->stream_done, st));
+  c->stream_pending = true;
+  return 0;
+}
+
 int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, const int32_t* img_row, const int32_t* left_pad,
                  int pos_from_mask, float* logits_all, float* last_logits, int32_t* next_tok, vcla_stream stream) {
   cudaStream_t st = (cudaStream_t)stream;
@@ -1112,11 +1130,12 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
   }
   if (prefill_layers(c, B, S, left_pad, pos_from_mask, nullptr, st) || prefill_logits(c, B, S, logits_all, last_logits, next_tok, st)) return -1;
   // sequence lengths become S - pad; the page the first decoded token will be appended to is reserved here
-  count(c); if (advance_seq(c->seq_len, B, S, left_pad, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st)) return -1;
+  count(c); if (advance_seq(c->seq_len, B, S, left_pad, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st,
+                            c->ring(), c->tok_hist)) return -1;
   if (c->beam_on && beam_reorder(c, B, B * c->beam_K, next_tok ? next_tok : c->d_tok, st)) return -1;
   c->len_bound = S;
   c->resident_b = c->beam_on ? B * c->beam_K : B;
-  return 0;
+  return stream_mark(c, st);
 }
 
 int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* logits_all, float* last_logits, int32_t* next_tok, vcla_stream stream) {
@@ -1138,9 +1157,10 @@ int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* lo
   count(c); if (kv_reserve(c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, B, T, nullptr, st, c->seq_len)) return -1;
   count(c); if (embed_tokens(ids, B, T, T, g.t_hidden, c->embed, g.t_vocab, 0, g.r_queries, c->resid, st)) return -1;
   if (prefill_layers(c, B, T, nullptr, 1, c->seq_len, st) || prefill_logits(c, B, T, logits_all, last_logits, next_tok, st)) return -1;
-  count(c); if (advance_seq(c->seq_len, B, T, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st)) return -1;
+  count(c); if (advance_seq(c->seq_len, B, T, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st,
+                            c->ring(), c->tok_hist)) return -1;
   c->len_bound += T;
-  return 0;
+  return stream_mark(c, st);
 }
 
 // Beam search: rows_new rows continue the rows_old rows (beam_parent, written by the select kernel) with the tokens `tok`; then the
@@ -1156,7 +1176,8 @@ static int beam_reorder(vcla_ctx* c, int rows_old, int rows_new, const int32_t* 
 }
 
 static int advance_and_reserve(vcla_ctx* c, int B, const int32_t* tok, cudaStream_t st) {
-  if (advance_seq(c->seq_len, B, 1, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st)) return -1;
+  if (advance_seq(c->seq_len, B, 1, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st,
+                  c->ring(), c->tok_hist)) return -1;
   return c->beam_on ? beam_reorder(c, B, B, tok, st) : 0;
 }
 
@@ -1253,7 +1274,7 @@ static int decode_enqueue(vcla_ctx* c, const int32_t* tok_in, int B, float* logi
 }
 
 static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, int n_steps, cudaStream_t st) {
-  GraphKey key{B, tok_in, logits, tok_out, n_steps, c->dp_on() ? 1 : 0, c->samp_on ? 1 : 0, c->beam_on ? c->beam_K : 0};
+  GraphKey key{B, tok_in, logits, tok_out, n_steps, c->dp_on() ? 1 : 0, c->samp_on ? 1 : 0, c->beam_on ? c->beam_K : 0, c->stream_armed ? 1 : 0};
   auto it = c->graphs.find(key);
   if (it == c->graphs.end()) {
     const int64_t before = c->launches;
@@ -1322,7 +1343,7 @@ int vcla_decode_step(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, i
   int rc = use_graph ? decode_graph(c, tok_in, B, logits, tok_out, 1, st) : decode_enqueue(c, tok_in, B, logits, tok_out, st);
   if (rc == 0 && !use_graph && c->dp_on()) rc = dp_wait(c, st);
   if (rc == 0) c->len_bound += 1;
-  return rc;
+  return rc == 0 ? stream_mark(c, st) : rc;
 }
 
 int vcla_decode_multi(vcla_ctx* c, int32_t* tok_inout, int B, int n_steps, vcla_stream stream) {
@@ -1334,7 +1355,7 @@ int vcla_decode_multi(vcla_ctx* c, int32_t* tok_inout, int B, int n_steps, vcla_
   if (decode_uses_csk(c, B) && csk_prepare(c, B)) return -1;
   const int rc = decode_graph(c, tok_inout, B, nullptr, tok_inout, n_steps, (cudaStream_t)stream);
   if (rc == 0) c->len_bound += n_steps;
-  return rc;
+  return rc == 0 ? stream_mark(c, (cudaStream_t)stream) : rc;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1420,6 +1441,7 @@ int vcla_set_beam(vcla_ctx* c, const vcla_beam* s) {
   if (s == nullptr) { c->beam_on = false; c->beam_K = 0; return 0; }
   if (!beam_supported(c->cfg.t_vocab)) { set_error("beam: vocabulary %d does not fit the beam-step kernel", c->cfg.t_vocab); return -1; }
   if (c->dp_on()) { set_error("beam: not available while the data-parallel token exchange is active"); return -1; }
+  if (c->stream_armed) { set_error("beam: not available while token streaming is armed (vcla_stream_arm)"); return -1; }
   BeamParams p;
   if (beam_to_params(s, c->cfg.t_vocab, &p)) return -1;
   if (p.K > std::min(c->cfg.max_batch, 64)) { set_error("beam: %d beams exceed min(max_batch, 64) = %d rows", p.K, std::min(c->cfg.max_batch, 64)); return -1; }
@@ -1534,6 +1556,7 @@ int vcla_dp_set_active(vcla_ctx* c, int on) {
   // a rank-local generate() on a context that owns a communicator runs with it off
   if (!c) return -1;
   if (on && !c->comm) { set_error("vcla_dp_set_active: call vcla_nccl_init first"); return -1; }
+  if (on && c->stream_armed) { set_error("vcla_dp_set_active: not available while token streaming is armed (vcla_stream_arm)"); return -1; }
   c->dp_active = on != 0;
   return 0;
 }
@@ -1609,6 +1632,85 @@ int vcla_read_history(vcla_ctx* c, int32_t* dst_dev, int B, int n_steps, vcla_st
   // tokens chosen by the prefill (step 0) and every decode step since, as a device [n_steps, B] int32 array
   if (n_steps < 0 || n_steps > c->cfg.max_seq + 1 || B < 1 || B > 64) { set_error("vcla_read_history: bad arguments"); return -1; }
   VCLA_CUDA_OK(cudaMemcpyAsync(dst_dev, c->tok_hist, (size_t)n_steps * B * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
+}
+
+// ---- token streaming: the ring is written by advance_seq_kernel (elementwise.cu) and read here ------------------------------------
+static int stream_published(const vcla_ctx* c) { return __atomic_load_n(&c->ring_host->published, __ATOMIC_ACQUIRE); }
+
+// 1 when every armed enqueue so far has completed, 0 when some is in flight, -1 on a device error
+static int stream_drained(vcla_ctx* c) {
+  if (!c->stream_pending) return 1;
+  const cudaError_t e = cudaEventQuery(c->stream_done);
+  if (e == cudaSuccess) { c->stream_pending = false; return 1; }
+  if (e == cudaErrorNotReady) { (void)cudaGetLastError(); return 0; }
+  set_error("token stream: device error %s", cudaGetErrorString(e));
+  return -1;
+}
+
+int vcla_stream_arm(vcla_ctx* c, int on) {
+  if (!c) return -1;
+  if (!on) { c->stream_armed = false; return 0; }
+  if (c->beam_on) { set_error("vcla_stream_arm: streaming is not available with beam search"); return -1; }
+  if (c->dp_on()) { set_error("vcla_stream_arm: streaming is not available while the data-parallel token exchange is active"); return -1; }
+  const int d = stream_drained(c);
+  if (d < 0) return -1;
+  if (d == 0) { set_error("vcla_stream_arm: armed work is still in flight (wait for it before arming again)"); return -1; }
+  if (c->ring_host == nullptr) {
+    const int rows = c->cfg.max_seq + 2;      // as many rows as the device token history
+    void* p = nullptr;
+    VCLA_CUDA_OK(cudaHostAlloc(&p, stream_ring_bytes(rows), cudaHostAllocMapped | cudaHostAllocPortable));
+    memset(p, 0, stream_ring_bytes(rows));
+    void* dp = nullptr;
+    const cudaError_t e = cudaHostGetDevicePointer(&dp, p, 0);
+    if (e == cudaSuccess && c->stream_done == nullptr) {
+      const cudaError_t e2 = cudaEventCreateWithFlags(&c->stream_done, cudaEventDisableTiming);
+      if (e2 != cudaSuccess) { cudaFreeHost(p); set_error("vcla_stream_arm: %s", cudaGetErrorString(e2)); return -1; }
+    }
+    if (e != cudaSuccess) { cudaFreeHost(p); set_error("vcla_stream_arm: %s", cudaGetErrorString(e)); return -1; }
+    c->ring_host = (StreamRing*)p;
+    c->ring_dev = (StreamRing*)dp;
+    c->ring_host->rows = rows;
+  }
+  __atomic_store_n(&c->ring_host->published, 0, __ATOMIC_RELEASE);
+  c->ring_host->epoch += 1;
+  c->stream_armed = true;
+  return 0;
+}
+
+int vcla_stream_wait(vcla_ctx* c, int target, int timeout_us, int* published) {
+  if (!c || !c->ring_host) { set_error("vcla_stream_wait: streaming was never armed (vcla_stream_arm)"); return -1; }
+  if (target < 0 || target > c->ring_host->rows) { set_error("vcla_stream_wait: target %d outside 0..%d", target, c->ring_host->rows); return -1; }
+  const auto t0 = std::chrono::steady_clock::now();
+  for (long it = 0;; ++it) {
+    int p = stream_published(c);
+    if (published) *published = p;
+    if (p >= target) return 0;
+    if (it < 4096 && (it & 63) != 63) continue;          // spin briefly: a step at 7B widths is a few milliseconds
+    const int d = stream_drained(c);
+    if (d < 0) return -1;
+    if (d == 1) {
+      p = stream_published(c);                             // the event completed after the last publish: read the count again
+      if (published) *published = p;
+      if (p >= target) return 0;
+      set_error("vcla_stream_wait: step %d will never be published: all armed work has completed with %d steps published", target, p);
+      return -1;
+    }
+    if (timeout_us >= 0 &&
+        std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - t0).count() >= timeout_us)
+      return 0;
+    if (it >= 4096) std::this_thread::sleep_for(std::chrono::microseconds(20));
+  }
+}
+
+int vcla_stream_read(vcla_ctx* c, int from, int to, int B, int32_t* dst_host) {
+  if (!c || !c->ring_host) { set_error("vcla_stream_read: streaming was never armed (vcla_stream_arm)"); return -1; }
+  const int p = stream_published(c);
+  if (from < 0 || to < from || to > p || B < 1 || B > 64 || (to > from && !dst_host)) {
+    set_error("vcla_stream_read: steps [%d, %d) x %d not within the %d published steps", from, to, B, p);
+    return -1;
+  }
+  for (int s = from; s < to; ++s) memcpy(dst_host + (size_t)(s - from) * B, c->ring_host->tokens + (size_t)s * 64, (size_t)B * 4);
   return 0;
 }
 

@@ -3,6 +3,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace vcla {
@@ -277,9 +278,22 @@ int kv_reserve(int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t*
                int B, int S, const int32_t* left_pad, cudaStream_t st, const int32_t* base_len = nullptr);
 // seq_len[b] = min(seq_len[b], len[b]) for b < B <= 64 (the pages stay owned)
 int kv_truncate(int32_t* seq_len, const int32_t* len_host, int B, cudaStream_t st);
-// seq_len[b] += by - left_pad[b] ; *step_idx += 1 ; then reserve the page the NEXT token of every sequence will be appended to
+// Token stream ring (vcla_stream_*): pinned, mapped host memory the device writes and the host polls.  tokens[L][b] = token of
+// sequence b chosen at step L (row stride 64); published = steps whose tokens are final (written with a system-scope release).
+struct StreamRing {
+  int32_t published;
+  int32_t epoch;
+  int32_t rows;          // capacity in steps (= rows of the device token history)
+  int32_t pad_[29];      // tokens start on their own 128-byte line
+  int32_t tokens[1];     // [rows][64]
+};
+inline size_t stream_ring_bytes(int rows) { return offsetof(StreamRing, tokens) + (size_t)rows * 64 * sizeof(int32_t); }
+// seq_len[b] += by - left_pad[b] ; *step_idx += 1 ; then reserve the page the NEXT token of every sequence will be appended to.
+// ring (nullable, device view of the mapped ring): first publish step L = *step_idx -- history row L ([L][B]) into ring row L, a
+// system-scope fence per writer, then ring->published = L + 1 with st.release.sys.  ring == nullptr executes none of it.
 int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, int32_t* kv_free, int32_t* kv_state,
-                int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, cudaStream_t st);
+                int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, cudaStream_t st,
+                StreamRing* ring = nullptr, const int32_t* history = nullptr);
 // Beam reorder, after advance_seq (so every old row's write position seq_len and its page exist).  New row j (< rows_new) continues
 // old row parent_row[j] (< rows_old): its table row, page count and length are the parent's.  Pages no new row references go back on
 // the free stack; when several rows continue one parent, every one but the first gets a fresh page for the write position plus a

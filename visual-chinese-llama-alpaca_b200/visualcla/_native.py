@@ -82,6 +82,10 @@ _SIGNATURES = [
     ("vcla_dp_set_active", C.c_int, [_P, C.c_int]),
     ("vcla_dp_exchange", C.c_int, [_P, _P]),
     ("vcla_read_history_dp", C.c_int, [_P, _P, C.c_int, _P]),
+    # token streaming (ref: models/visualcla/modeling_utils.py:180-247 chat_in_stream; HF generate(streamer=...))
+    ("vcla_stream_arm", C.c_int, [_P, C.c_int]),
+    ("vcla_stream_wait", C.c_int, [_P, C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    ("vcla_stream_read", C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P]),
     ("vcla_kernel_launches", C.c_int64, [_P, C.c_int]),
     ("vcla_read_stage", C.c_int, [_P, C.c_char_p, C.c_int, _P, _P]),
     ("vcla_op_gemm", C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),

@@ -383,6 +383,30 @@ class Engine:
                                                self._stream()), "vcla_op_beam_step")
         return dict(parent=parent, token=token, cand=cand)
 
+    # ---- token streaming (include/vcla.h, "token streaming") ---------------------------------------------------------------
+    def stream_supported(self) -> bool:
+        return True
+
+    def stream_arm(self, on: bool):
+        """Armed, every token choice (prefill / extend pick, each decode step) publishes its step into the host ring."""
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_stream_arm(self._ctx, 1 if on else 0), "vcla_stream_arm")
+
+    def stream_wait(self, target: int, timeout_us: int = -1) -> int:
+        """-> steps published so far, >= target unless the timeout (microseconds, < 0: none) expired first.  Raises when all armed
+        work has completed and step `target` was never published.  The GIL is released while it waits."""
+        n = C.c_int()
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_stream_wait(self._ctx, int(target), int(timeout_us), C.byref(n)), "vcla_stream_wait")
+        return n.value
+
+    def stream_read(self, lo: int, hi: int, B: int) -> torch.Tensor:
+        """(hi - lo, B) int32 host tensor: the tokens of published steps lo..hi-1."""
+        out = torch.empty(hi - lo, B, dtype=torch.int32)
+        if hi > lo:
+            N.check(self.lib.vcla_stream_read(self._ctx, int(lo), int(hi), int(B), N.ptr(out)), "vcla_stream_read")
+        return out
+
     def read_history(self, B: int, n_steps: int) -> torch.Tensor:
         """(n_steps, B) int32 CUDA tensor: tokens chosen by the prefill (row 0) and each decode step since."""
         out = torch.empty(n_steps, B, dtype=torch.int32, device=self.device)

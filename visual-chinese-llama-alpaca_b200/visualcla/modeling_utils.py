@@ -240,7 +240,8 @@ class Iteratorize:
 
 @torch.inference_mode()
 def chat_in_stream(model, image, text: str, history=[], generation_config=None):
-    """Generator of (response_so_far, history) (ref: modeling_utils.py:180-247)."""
+    """Generator of (response_so_far, history) (ref: modeling_utils.py:180-247).  Its only stopping criterion is a Stream, so generate()
+    runs it on the device decode graphs with each token published as it is chosen: under the same seed it ends on chat()'s reply."""
     enc, generation_config = _prepare(model, image, text, history, generation_config)
     eos_token_id = model.tokenizer.eos_token_id
     base_history = deepcopy(history)

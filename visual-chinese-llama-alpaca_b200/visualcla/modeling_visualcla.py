@@ -427,8 +427,7 @@ class VisualCLAModel:
     def generate(self, input_ids=None, pixel_values=None, attention_mask=None, generation_config=None,
                  logits_processor=None, stopping_criteria=None, prefix_allowed_tokens_fn=None, synced_gpus=False, **kwargs):
         past_key_values = kwargs.pop("past_key_values", None)
-        beam_request = (kwargs.get("num_beams") or getattr(generation_config, "num_beams", 1) or 1) > 1
-        streamer = kwargs.pop("streamer", None) if beam_request else None
+        streamer = kwargs.pop("streamer", None)
         gc = self._resolve_generation_config(generation_config, kwargs)
         if prefix_allowed_tokens_fn is not None:
             raise NotImplementedError("prefix_allowed_tokens_fn is not supported on the H100 path")
@@ -437,6 +436,8 @@ class VisualCLAModel:
         eng = self._engine
         B = input_ids.shape[0]
         if B > eng.max_batch:
+            if streamer is not None:
+                raise NotImplementedError(f"streaming a batch of {B} > max_batch={eng.max_batch} prompts is not supported")
             outs = []
             for s in range(0, B, eng.max_batch):
                 sl = slice(s, s + eng.max_batch)
@@ -500,11 +501,21 @@ class VisualCLAModel:
         out = torch.full((B, max_new), pad, dtype=torch.int64, device=dev)
         all_logits: List[torch.Tensor] = []
 
-        spec = self._device_sampler_spec(gc, eos, pad, min_new, logits_processor, crit, processors)
+        streaming = streamer is not None or self._stream_criteria_only(crit)
+        if streaming and (not crit or self._stream_criteria_only(crit)) and os.environ.get("VCLA_HOST_SAMPLER") != "1" and getattr(eng, "stream_supported", lambda: False)():
+            # streamed on the device when the call would run there without its Stream criteria: the sampler graphs, or the
+            # pure-greedy argmax graphs (spec None); each step's tokens reach the host through the pinned ring as they are chosen
+            pure_greedy = not need_logits and not eos
+            spec = None if pure_greedy else self._device_sampler_spec(gc, eos, pad, min_new, logits_processor, [], processors)
+            if pure_greedy or spec is not None:
+                return self._generate_streamed(spec, start, finish, B, max_new, eos, tok, streamer, crit)
+        spec = None if streaming else self._device_sampler_spec(gc, eos, pad, min_new, logits_processor, crit, processors)
         if spec is not None:
             return self._generate_on_device(spec, start, finish, B, max_new, eos, tok)
+        if streamer is not None:
+            streamer.put(torch.empty(B, 0, dtype=torch.int64))    # HF generate: put(input_ids) first -- none with inputs_embeds
         last, first_tok = start(need_logits)
-        if not need_logits and not eos and not crit:
+        if not need_logits and not eos and not crit and streamer is None:
             # pure greedy, fixed length: graph replays only; tokens come from the device-side history the graph appends to
             tok.copy_(first_tok)
             eng.decode_many(tok, max_new - 1)
@@ -544,14 +555,17 @@ class VisualCLAModel:
                 tok.copy_(nxt)
             n_done = step + 1
             stop = False
+            if streamer is not None:
+                streamer.put(nxt.to("cpu", torch.int64))
             if eos:
                 is_eos = torch.zeros_like(finished)
                 for e in eos:
                     is_eos |= nxt == e
                 finished |= is_eos
                 # host poll (one sync) only every 8 steps: sequences are independent, so running a few extra
-                # steps past the last EOS cannot change any retained token (HF syncs every step)
-                if (step & 7) == 7 or step == max_new - 1:
+                # steps past the last EOS cannot change any retained token (HF syncs every step).  A streamer sees every
+                # step, so with one the loop stops where HF does.
+                if (step & 7) == 7 or step == max_new - 1 or streamer is not None:
                     stop = bool(finished.all())
             for cfn in crit:
                 r = cfn(out[:, :n_done], cur_logits if need_logits else None)
@@ -572,15 +586,93 @@ class VisualCLAModel:
             result = result[:, :keep]
             idx = torch.arange(keep, device=dev)[None, :]
             result = torch.where(idx < first[:, None], result, torch.full_like(result, pad))
+        if streamer is not None:
+            streamer.end()
         return finish(result, fed, tuple(all_logits) if all_logits else None)
+
+    # ---- streaming on the device: decode graphs publish every step into a pinned host ring (include/vcla.h, token streaming) ----
+    STREAM_CHUNK = 8      # decode steps per graph replay while streaming
+
+    @staticmethod
+    def _stream_criteria_only(crit) -> bool:
+        from .modeling_utils import Stream
+        return len(crit) > 0 and all(isinstance(c, Stream) for c in crit)
+
+    def _generate_streamed(self, spec, start, finish, B, max_new, eos, tok, streamer, crit):
+        """generate() with a streamer and / or Stream criteria, on the device.  The prefill and graphs of up to STREAM_CHUNK decode steps
+        run as without streaming (spec: the device sampler, None: the argmax graphs) while armed, so each step's tokens are published
+        to the host as soon as they are chosen.  The next graph is enqueued once the second-to-last step of the running one is
+        published, so the device never waits for the host.  Every published step goes, in order, to streamer.put and then to the
+        criteria (HF _sample's order).  Launching stops when every row has emitted an EOS id, at max_new_tokens, or when a criterion
+        returns True; the steps still running then (at most STREAM_CHUNK + 1) are drained and dropped."""
+        eng = self._engine
+        if streamer is not None:
+            streamer.put(torch.empty(B, 0, dtype=torch.int64))    # HF generate: put(input_ids) first -- none with inputs_embeds
+        rows = torch.empty(B, max_new, dtype=torch.int64)         # host copy of the published steps
+        eos_t = torch.tensor(eos, dtype=torch.int64) if eos else None
+        n_launched, n_kept = 0, 0
+        if spec is not None:
+            eng.set_sampler(spec)
+        try:
+            eng.stream_arm(True)
+            try:
+                _, first_tok = start(False)
+                tok.copy_(first_tok)
+                n_launched = 1
+
+                def launch():
+                    nonlocal n_launched
+                    k = min(self.STREAM_CHUNK, max_new - n_launched)
+                    eng.decode_many(tok, k)
+                    n_launched += k
+
+                if max_new > 1:
+                    launch()
+                finished = torch.zeros(B, dtype=torch.bool)
+                s, done = 0, False
+                while not done:
+                    seen = min(eng.stream_wait(s + 1), n_launched)
+                    new = eng.stream_read(s, seen, B).to(torch.int64)
+                    for row in new:
+                        rows[:, s] = row
+                        if eos:
+                            finished |= torch.isin(row, eos_t)
+                        last = s + 1 == max_new or (bool(eos) and bool(finished.all()))
+                        if not last and s >= n_launched - 2 and n_launched < max_new:
+                            launch()                                          # before the callbacks: keep the device busy
+                        n_kept = s + 1
+                        if streamer is not None:
+                            streamer.put(row.clone())
+                        stop = False
+                        for cfn in crit:
+                            r = cfn(rows[:, :n_kept], None)
+                            if isinstance(r, torch.Tensor):
+                                r = bool(r.all())
+                            stop = stop or bool(r)
+                        s += 1
+                        if last or stop:
+                            done = True
+                            break
+            finally:
+                if n_launched:
+                    eng.stream_wait(n_launched)                               # drain what is still running before disarming
+                eng.stream_arm(False)
+        finally:
+            if spec is not None:
+                eng.set_sampler(None)
+        if streamer is not None:
+            streamer.end()
+        result = rows[:, :n_kept].to(eng.device)                     # the device sampler already pads a finished row
+        # the cache handle records the tokens fed up to the cut; steps run past it lie beyond its length
+        return finish(result, rows[:, : n_kept - 1])
 
     # ---- sampling / EOS on the device: one fused kernel per step inside the decode graph ---------------------
     def _device_sampler_spec(self, gc, eos, pad, min_new, extra_processors, crit, processors):
         """-> a native sampler spec when this call can run entirely on the device, else None (host logits-processor path).
         On the device: greedy or sampling with repetition_penalty / no_repeat_ngram_size / temperature / top_k (1..1024) / top_p and
         up to 4 EOS ids -- the reference's DEFAULT_GENERATION_CONFIG (ref modeling_utils.py:36-47) is such a call.  Anything else
-        (custom processors, stopping criteria / streaming, TFS / Top-A / Mirostat, top_k disabled, logits or scores requested)
-        keeps the per-step host path."""
+        (custom processors, stopping criteria, TFS / Top-A / Mirostat, top_k disabled, logits or scores requested) keeps the
+        per-step host path; generate() streams on the device by calling this without its Stream criteria."""
         eng = self._engine
         if os.environ.get("VCLA_HOST_SAMPLER") == "1" or not hasattr(eng, "sampler_supported") or not eng.sampler_supported():
             return None
