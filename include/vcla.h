@@ -326,6 +326,9 @@ int vcla_op_gemm_q8(const void* A_dev_bf16, const int8_t* Wq_dev, const float* w
  * (B <= 32; with weight_format 1 B <= 64, where at 33..64 the lm_head runs on the workspace GEMM and its entry is ignored) */
 int vcla_debug_set_csk_splits(vcla_ctx* ctx, int B, int qkv, int o, int gate_up, int down, int lm_head);
 int vcla_debug_get_csk_splits(vcla_ctx* ctx, int B, int* out5);
+/* test hook: resident CTAs per SM (occupancy query) of the two decode kernels a step at batch B launches with this context's weights and
+ * cache: out2[0] the cluster split-K GEMM, out2[1] decode attention */
+int vcla_debug_decode_ctas_per_sm(vcla_ctx* ctx, int B, int* out2);
 /* prefill attention kernel: 0 = the mma.sync kernel everywhere, 1 (default) = wgmma flash attention (QK^T / PV on the warpgroup tensor
  * cores, S and O in registers, TMA operands) at head dim 128 (LLaMA prefill) and mma.sync at head dim 64 (ViT / Resampler), 2 = wgmma everywhere */
 void vcla_set_attention_tc(int mode);

@@ -235,21 +235,25 @@ int attention_prefill_mma(const AttnCall& c, cudaStream_t st) {
 // decode (hd = 128): grid (kv_splits, H, B), 128 threads
 // =================================================================================================
 constexpr int kDecWarps = 8;        // 256 threads
-#ifndef VCLA_DEC_STAGES
-#define VCLA_DEC_STAGES 3
-#endif
-constexpr int kDecStages = VCLA_DEC_STAGES;   // KV pages in flight per CTA: 3 x 32 KB at 64 tokens/page -> 2 CTAs per SM (2 stages / 3 CTAs measured slower: B=32 37 vs 34 us per layer)
+// KV pages in flight per CTA (32 KB each at 64 tokens/page).  3 stages -> 2 CTAs per SM: the persistent kernel, and the one-shot kernel
+// when its grid needs more than one wave at two CTAs per SM (2 stages with 3 CTAs per SM measured slower at B=32 on B200, 37 vs 34 us
+// per layer, with the grid filling all three slots).  A one-shot grid of at most two CTAs per SM (small batches: B = 1..8 at 32 heads)
+// runs 2 stages, so a third CTA fits per SM; that free slot is where the O-projection GEMM becomes resident and starts streaming
+// weights while attention drains.
+constexpr int kDecStages = 3;
+constexpr int kDecStagesSmallBatch = 2;
 constexpr int kDecMaxPT = 64;       // page_tokens supported by the smem ring
 
 // One CTA per (kv split, head, sequence).  The cached K/V rows of a head are contiguous per page (page_tokens x 128 bf16 =
-// 16 KB), so whole pages are streamed with TMA bulk copies (cp.async.bulk, mbarrier completion) into a 3-stage shared-memory
+// 16 KB), so whole pages are streamed with TMA bulk copies (cp.async.bulk, mbarrier completion) into a 2- or 3-stage shared-memory
 // ring and the dot products / PV accumulation run out of shared memory: the kernel is bandwidth- instead of latency-bound
 // (the register-prefetch version had one DRAM round trip per 32 tokens per CTA).
-__global__ void __launch_bounds__(kDecWarps * 32, kDecStages == 2 ? 3 : 2) attn_decode_kernel(const DecodeAttnCall c, const float* __restrict__ rope_cos,
-                                                                     const float* __restrict__ rope_sin) {
+template <int STAGES>
+__global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_decode_kernel(const DecodeAttnCall c, const float* __restrict__ rope_cos,
+                                                                                  const float* __restrict__ rope_sin) {
   constexpr int HD = 128;
-  extern __shared__ __align__(128) uint8_t dsm[];      // [kDecStages][2][PT][HD] bf16
-  __shared__ __align__(8) uint64_t s_bar[kDecStages];
+  extern __shared__ __align__(128) uint8_t dsm[];      // [STAGES][2][PT][HD] bf16
+  __shared__ __align__(8) uint64_t s_bar[STAGES];
   __shared__ float s_q[HD];
   __shared__ float s_k[HD];
   __shared__ float s_v[HD];
@@ -264,7 +268,7 @@ __global__ void __launch_bounds__(kDecWarps * 32, kDecStages == 2 ? 3 : 2) attn_
   TraceScope trace(4);
 
   if (tid == 0) {
-    for (int s = 0; s < kDecStages; ++s) mbar_init(smem_u32(&s_bar[s]), 1);
+    for (int s = 0; s < STAGES; ++s) mbar_init(smem_u32(&s_bar[s]), 1);
     fence_barrier_init();
   }
   pdl_launch_dependents();
@@ -283,8 +287,8 @@ __global__ void __launch_bounds__(kDecWarps * 32, kDecStages == 2 ? 3 : 2) attn_
   const int p0 = t_begin / PT;
   const int npages = c_end > t_begin ? (c_end - t_begin + PT - 1) / PT : 0;
 
-  auto issue_page = [&](int i) {                      // thread 0: request page i of this CTA into stage i % kDecStages
-    const int stage = i % kDecStages;
+  auto issue_page = [&](int i) {                      // thread 0: request page i of this CTA into stage i % STAGES
+    const int stage = i % STAGES;
     const int page = __ldg(c.page_table + (size_t)b * c.pages_per_seq + p0 + i);
     const int ntok = min(PT, c_end - (t_begin + i * PT));
     const uint32_t bytes = (uint32_t)ntok * HD * 2;
@@ -297,7 +301,7 @@ __global__ void __launch_bounds__(kDecWarps * 32, kDecStages == 2 ? 3 : 2) attn_
     bulk_load_1d(dst + (uint32_t)PT * HD * 2, vsrc, bytes, bar);
   };
   if (tid == 0) {
-    for (int i = 0; i < npages && i < kDecStages; ++i) issue_page(i);   // the KV stream starts before the q reduction below
+    for (int i = 0; i < npages && i < STAGES; ++i) issue_page(i);   // the KV stream starts before the q reduction below
   }
 
   // ---- reduce the split-K partials of this head's q (and k, v if this CTA owns the new token); RoPE
@@ -353,8 +357,8 @@ __global__ void __launch_bounds__(kDecWarps * 32, kDecStages == 2 ? 3 : 2) attn_
   for (int i = 0; i < 16; ++i) acc[i] = 0.f;
 
   for (int i = 0; i < npages; ++i) {
-    const int stage = i % kDecStages;
-    const uint32_t parity = (uint32_t)((i / kDecStages) & 1);
+    const int stage = i % STAGES;
+    const uint32_t parity = (uint32_t)((i / STAGES) & 1);
     mbar_wait(smem_u32(&s_bar[stage]), parity);
     const int ntok = min(PT, c_end - (t_begin + i * PT));
     const uint8_t* kbase = dsm + (size_t)stage * stage_bytes;
@@ -388,7 +392,7 @@ __global__ void __launch_bounds__(kDecWarps * 32, kDecStages == 2 ? 3 : 2) attn_
       }
     }
     __syncthreads();                                   // every warp is done with this stage
-    if (tid == 0 && i + kDecStages < npages) issue_page(i + kDecStages);
+    if (tid == 0 && i + STAGES < npages) issue_page(i + STAGES);
   }
   __syncwarp();
   // the new token (from smem), handled by warp 0 group 0 of the owning CTA
@@ -712,13 +716,32 @@ int attention_init() {
   static int rc = 0;
   std::call_once(once, [] {
     auto set = [](const void* fn, int bytes) { return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess ? 0 : -1; };
-    rc |= set((const void*)attn_decode_kernel, kDecStages * kDecMaxPT * 128 * 2 * 2);
+    rc |= set((const void*)attn_decode_kernel<kDecStages>, kDecStages * kDecMaxPT * 128 * 2 * 2);
+    rc |= set((const void*)attn_decode_kernel<kDecStagesSmallBatch>, kDecStagesSmallBatch * kDecMaxPT * 128 * 2 * 2);
     rc |= set((const void*)attn_decode_persistent_kernel, kDecStages * kDecMaxPT * 128 * 2 * 2);
     rc |= set((const void*)attn_prefill_kernel<128>, 5 * 64 * 128 * 2);
     rc |= set((const void*)attn_prefill_kernel<64>, 5 * 64 * 64 * 2);
     if (rc) set_error("attention_init: cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
   });
   return rc;
+}
+
+// The decode kernel attention_decode launches for c: the persistent kernel (-> its grid in *persistent_ctas) or the one-shot kernel with
+// a 2- or 3-stage ring.
+enum DecodeKernel { kDecPersistent, kDecOneShot2, kDecOneShot3 };
+static DecodeKernel decode_kernel_pick(const DecodeAttnCall& c, int* persistent_ctas) {
+  const int n_items = c.B * c.H;
+  int slots = 2 * num_sms();
+  // persistent_mode: 0 = never, 1 (default) = when items outnumber the resident CTAs, 2 = whenever kv_splits == 1 (tests);
+  // persistent_grid caps the persistent grid (tests: several items per CTA on small problems).  Both are read from the
+  // environment once per context (vcla_create), not per launch.
+  if (c.persistent_grid > 0 && c.persistent_grid < slots) slots = c.persistent_grid;
+  if (c.kv_splits == 1 && ((c.persistent_mode == 1 && n_items > slots) || c.persistent_mode == 2)) {
+    *persistent_ctas = n_items < slots ? n_items : slots;   // more (sequence, head) items than resident CTAs
+    return kDecPersistent;
+  }
+  // one wave at two CTAs per SM: the small ring leaves a third slot free
+  return c.kv_splits * n_items <= 2 * num_sms() ? kDecOneShot2 : kDecOneShot3;
 }
 
 int attention_decode(const DecodeAttnCall& c, cudaStream_t st) {
@@ -733,21 +756,41 @@ int attention_decode(const DecodeAttnCall& c, cudaStream_t st) {
   int na = 0;
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = attr; cfg.numAttrs = na;
-  const int n_items = c.B * c.H;
-  int slots = 2 * num_sms();
-  // persistent_mode: 0 = never, 1 (default) = when items outnumber the resident CTAs, 2 = whenever kv_splits == 1 (tests);
-  // persistent_grid caps the persistent grid (tests: several items per CTA on small problems).  Both are read from the
-  // environment once per context (vcla_create), not per launch.
-  if (c.persistent_grid > 0 && c.persistent_grid < slots) slots = c.persistent_grid;
-  if (c.kv_splits == 1 && ((c.persistent_mode == 1 && n_items > slots) || c.persistent_mode == 2)) {
-    // more (sequence, head) items than resident CTAs: persistent, warp-specialised variant
-    cfg.gridDim = dim3(n_items < slots ? n_items : slots);
-    cfg.blockDim = dim3((kDecWarps + 2) * 32);
-    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_persistent_kernel, c, c.rope_cos, c.rope_sin, n_items));
-    return 0;
+  int persistent_ctas = 0;
+  switch (decode_kernel_pick(c, &persistent_ctas)) {
+    case kDecPersistent:
+      cfg.gridDim = dim3(persistent_ctas);
+      cfg.blockDim = dim3((kDecWarps + 2) * 32);
+      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_persistent_kernel, c, c.rope_cos, c.rope_sin, c.B * c.H));
+      break;
+    case kDecOneShot2:
+      cfg.dynamicSmemBytes = (size_t)kDecStagesSmallBatch * c.page_tokens * 128 * 2 * 2;
+      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch>, c, c.rope_cos, c.rope_sin));
+      break;
+    case kDecOneShot3:
+      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStages>, c, c.rope_cos, c.rope_sin));
+      break;
   }
-  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel, c, c.rope_cos, c.rope_sin));
   return 0;
+}
+
+int attention_decode_ctas_per_sm(const DecodeAttnCall& c) {
+  if (attention_init()) return -1;
+  int persistent_ctas = 0, n = 0;
+  cudaError_t e = cudaSuccess;
+  switch (decode_kernel_pick(c, &persistent_ctas)) {
+    case kDecPersistent:
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_persistent_kernel, (kDecWarps + 2) * 32, (size_t)kDecStages * c.page_tokens * 128 * 2 * 2);
+      break;
+    case kDecOneShot2:
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStagesSmallBatch>, kDecWarps * 32, (size_t)kDecStagesSmallBatch * c.page_tokens * 128 * 2 * 2);
+      break;
+    case kDecOneShot3:
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStages>, kDecWarps * 32, (size_t)kDecStages * c.page_tokens * 128 * 2 * 2);
+      break;
+  }
+  if (e != cudaSuccess) { set_error("attention_decode_ctas_per_sm: %s", cudaGetErrorString(e)); (void)cudaGetLastError(); return -1; }
+  return n;
 }
 
 }  // namespace vcla

@@ -1816,6 +1816,12 @@ int vcla_debug_get_csk_splits(vcla_ctx* c, int B, int* out5) {
   out5[0] = c->csk_qkv; out5[1] = c->csk_o; out5[2] = c->csk_gu; out5[3] = c->csk_d; out5[4] = c->csk_lm;
   return 0;
 }
+int vcla_debug_decode_ctas_per_sm(vcla_ctx* c, int B, int* out2) {
+  if (!c || !out2 || B < 1 || B > csk_max_batch(c)) { set_error("vcla_debug_decode_ctas_per_sm: bad arguments"); return -1; }
+  out2[0] = gemm_csk_ctas_per_sm(B, c->cfg.weight_format == 1);
+  out2[1] = attention_decode_ctas_per_sm(decode_attn_call(c, c->tl[0], B, 1));
+  return out2[0] > 0 && out2[1] > 0 ? 0 : -1;
+}
 int vcla_op_gemm_csk_clusters(int B, int splits) { return gemm_csk_clusters(B, splits); }
 void vcla_set_attention_tc(int on) { attention_set_tc(on); }
 int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v0, int kv0_stride, int n0, const void* k1, const void* v1,

@@ -18,13 +18,17 @@
 //
 // Reduce buffering (template NBUF): 2 = double buffered (tile t+1's partials may arrive while tile t is being summed; the hand-shake
 // is one remote arrive per peer and tile), 1 = one buffer + a second 'consumed' barrier, which frees shared memory for a deeper TMA
-// ring (used for the 32-column batch tile).  Two CTAs per SM; the launch assumes that occupancy (see csk_max_clusters).
+// ring.  The 16-column batch tile (B <= 16) runs 3 stages + one reduce buffer (66 KB), small enough for a THIRD CTA per SM: where the
+// grid leaves a slot free (o_proj, down_proj: 32 tiles), the next kernel's first CTAs become resident there under PDL and start their
+// weight TMAs while this kernel's last tiles reduce and exit; the larger GEMMs deal their tiles evenly over the clusters resident at
+// three CTAs per SM (csk_launch).
 //
 // Per CTA (160 threads): warp 4 = TMA producer (weight tiles are requested BEFORE griddepcontrol.wait: they never depend on the
 // previous kernel), warps 0..3 = one wgmma warpgroup: MMAs (2 x m64nBNk16 per k step) -> peers' smem -> reduce -> consumer.
 #include "common.cuh"
 #include "kernels.h"
 
+#include <algorithm>
 #include <mutex>
 #include <stdio.h>
 #include <stdlib.h>
@@ -36,6 +40,7 @@ constexpr int kCskThreads = 160;
 constexpr int kCskBlockM = 128;
 constexpr int kCskBlockK = 64;
 constexpr int kCskMaxSplits = 8;
+constexpr int kCskGridSmem = 96 * 1024;   // shared memory per CTA the grid is sized with: two such CTAs fit an SM, three do not
 
 struct CskParams {
   int M, B, K;                 // output features, batch rows, reduction length
@@ -64,6 +69,8 @@ struct CskCfg {
   static constexpr int MISC_OFF = BAR_OFF + 256;                          // rstd[BN], ssq warp partials [4][BN]
   static constexpr int MISC_BYTES = BN * 20 > 1024 ? BN * 20 : 1024;
   static constexpr int SMEM_BYTES = MISC_OFF + MISC_BYTES + 1024;        // + slack for the 1024 B alignment of the ring
+  // CTAs per SM the shared memory allows (228 KB per SM, 1 KB of it reserved per CTA); the launch bound asks for registers to match
+  static constexpr int CTAS_PER_SM = 3 * (SMEM_BYTES + 1024) <= 228 * 1024 ? 3 : 2;
   static_assert(STAGE_BYTES % 1024 == 0, "stage must keep 1024 B alignment for SWIZZLE_128B");
   static_assert(BN == 16 || BN == 32 || (Q8 && BN == 64), "decode batch tile");
 };
@@ -112,7 +119,7 @@ __device__ __forceinline__ uint32_t i8x2_to_bf16x2(uint32_t biased, uint32_t sel
 // registers (int8 is exact in bf16) and fed to register-A wgmma; the row scale commutes with the contraction and is applied after the
 // cluster reduction.
 template <int BN, int STAGES, int NBUF, bool Q8 = false>
-__global__ void __launch_bounds__(kCskThreads, 2)
+__global__ void __launch_bounds__(kCskThreads, CskCfg<BN, STAGES, NBUF, Q8>::CTAS_PER_SM)
 gemm_csk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const CskParams p) {
   using C = CskCfg<BN, STAGES, NBUF, Q8>;
   extern __shared__ uint8_t smem_raw[];
@@ -391,14 +398,15 @@ static int csk_init() {
       set_error("cuTensorMapEncodeTiled not available"); g_csk_rc = -1; return;
     }
     g_csk_encode = reinterpret_cast<PFN_encodeTiled>(fn);
-    // two CTAs per SM need (almost) the whole 228 KB of an SM as shared memory: ask for the maximum carve-out explicitly (the occupancy
-    // query for cluster launches otherwise assumes a carve-out that holds only one CTA)
+    // two or three CTAs per SM need (almost) the whole 228 KB of an SM as shared memory: ask for the maximum carve-out explicitly (the
+    // occupancy query for cluster launches otherwise assumes a carve-out that holds only one CTA).  The opt-in covers kCskGridSmem, the
+    // footprint csk_max_clusters sizes the grid with.
     auto prep = [](const void* fn, int bytes) {
-      return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess &&
+      return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, std::max(bytes, kCskGridSmem)) == cudaSuccess &&
              cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) == cudaSuccess;
     };
-    if (!prep((const void*)gemm_csk_kernel<16, 4, 2>, CskCfg<16, 4, 2>::SMEM_BYTES) || !prep((const void*)gemm_csk_kernel<32, 3, 2>, CskCfg<32, 3, 2>::SMEM_BYTES) ||
-        !prep((const void*)gemm_csk_kernel<16, 5, 1>, CskCfg<16, 5, 1>::SMEM_BYTES) || !prep((const void*)gemm_csk_kernel<32, 4, 1>, CskCfg<32, 4, 1>::SMEM_BYTES) ||
+    if (!prep((const void*)gemm_csk_kernel<16, 3, 1>, CskCfg<16, 3, 1>::SMEM_BYTES) || !prep((const void*)gemm_csk_kernel<32, 3, 2>, CskCfg<32, 3, 2>::SMEM_BYTES) ||
+        !prep((const void*)gemm_csk_kernel<32, 4, 1>, CskCfg<32, 4, 1>::SMEM_BYTES) ||
         !prep((const void*)gemm_csk_kernel<16, 8, 2, true>, CskCfg<16, 8, 2, true>::SMEM_BYTES) ||
         !prep((const void*)gemm_csk_kernel<32, 6, 2, true>, CskCfg<32, 6, 2, true>::SMEM_BYTES) ||
         !prep((const void*)gemm_csk_kernel<64, 4, 1, true>, CskCfg<64, 4, 1, true>::SMEM_BYTES)) {
@@ -423,14 +431,17 @@ static int csk_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t col
   return 0;
 }
 
-// clusters of S CTAs that can be co-resident (2 CTAs per SM, a cluster never spans GPCs), cached per (BN, S)
+// Upper bound on the clusters of S CTAs per launch, cached per (BN, S); csk_pick's split counts are chosen from it.  The query is asked
+// about a CTA of at least kCskGridSmem bytes of shared memory, which admits two per SM, so a configuration small enough for a third CTA
+// gets the bound (and hence the split counts, which fix the summation order) of the two-per-SM configurations.
 template <int BN, int STAGES, int NBUF, bool Q8 = false>
 static int csk_max_clusters(int S) {
   static int cache[kCskMaxSplits + 1] = {0};
   if (cache[S] != 0) return cache[S];
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(S * 64); cfg.blockDim = dim3(kCskThreads); cfg.dynamicSmemBytes = CskCfg<BN, STAGES, NBUF, Q8>::SMEM_BYTES;
+  cfg.gridDim = dim3(S * 64); cfg.blockDim = dim3(kCskThreads);
+  cfg.dynamicSmemBytes = std::max(CskCfg<BN, STAGES, NBUF, Q8>::SMEM_BYTES, kCskGridSmem);
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = S; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
@@ -450,8 +461,32 @@ static int csk_max_clusters(int S) {
   // bound, <= 113 KB of shared memory each), so that is what the launch assumes; VCLA_CSK_OCC=1 restores the query's answer.
   int mult = 2;
   if (const char* e = getenv("VCLA_CSK_OCC")) { const int v = atoi(e); if (v >= 1 && v <= 2) mult = v; }
-  if (getenv("VCLA_DEBUG")) fprintf(stderr, "[vcla] gemm_csk<%d,%d%s> S=%d: cluster query %d, blocks/SM %d, using x%d\n", BN, STAGES, Q8 ? ",q8" : "", S, n, per_sm, mult);
+  if (getenv("VCLA_DEBUG")) fprintf(stderr, "[vcla] gemm_csk<%d,%d,%d%s> S=%d: cluster query %d, blocks/SM %d, using x%d\n", BN, STAGES, NBUF, Q8 ? ",q8" : "", S, n, per_sm, mult);
   n *= mult;
+  cache[S] = n;
+  return n;
+}
+
+// clusters of S CTAs the cluster occupancy query finds co-resident at the configuration's own shared memory, cached per (BN, S)
+template <int BN, int STAGES, int NBUF, bool Q8 = false>
+static int csk_resident_clusters(int S) {
+  static int cache[kCskMaxSplits + 1] = {0};
+  if (cache[S] != 0) return cache[S];
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(S * 64); cfg.blockDim = dim3(kCskThreads);
+  cfg.dynamicSmemBytes = CskCfg<BN, STAGES, NBUF, Q8>::SMEM_BYTES;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = S; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, gemm_csk_kernel<BN, STAGES, NBUF, Q8>, &cfg) != cudaSuccess || n <= 0) {
+    (void)cudaGetLastError();
+    n = (2 * num_sms()) / S;                         // two CTAs per SM
+    if (n < 1) n = 1;
+  }
+  if (getenv("VCLA_DEBUG")) fprintf(stderr, "[vcla] gemm_csk<%d,%d,%d%s> S=%d: %d clusters resident\n", BN, STAGES, NBUF, Q8 ? ",q8" : "", S, n);
   cache[S] = n;
   return n;
 }
@@ -463,6 +498,14 @@ static int csk_launch(const CskCall& c, CskParams p, cudaStream_t st) {
   if (csk_tmap(&tx, c.X, c.B, c.K, c.K, BN)) return -1;
   int ncl = csk_max_clusters<BN, STAGES, NBUF, Q8>(p.splits);
   if (ncl > p.m_tiles) ncl = p.m_tiles;
+  if constexpr (CskCfg<BN, STAGES, NBUF, Q8>::CTAS_PER_SM == 3) {
+    // Tiles are dealt to clusters round-robin (t = cluster, cluster + n_clusters, ...), and clusters beyond those resident start only
+    // when a resident one exits: with more clusters than fit at once, the late ones run their whole share in a tail of their own.
+    // Deal the tiles evenly over the rounds the resident clusters need instead.  Which cluster reduces a tile changes no arithmetic.
+    const int res = std::min(ncl, csk_resident_clusters<BN, STAGES, NBUF, Q8>(p.splits));
+    const int rounds = (p.m_tiles + res - 1) / res;
+    ncl = (p.m_tiles + rounds - 1) / rounds;
+  }
   p.n_clusters = ncl;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -478,18 +521,13 @@ static int csk_launch(const CskCall& c, CskParams p, cudaStream_t st) {
   return 0;
 }
 
-// Reduce buffering: batch <= 16 (16-column tile): double-buffered reduce + 4 TMA stages; batch 17..32 (32-column tile): ONE buffer
-// + 'consumed' barrier, which frees the shared memory for a 4th TMA stage.  VCLA_CSK_NBUF = 1 / 2 forces one scheme for both.
-static int csk_nbuf_env() {
+// Configurations: batch <= 16 (16-column tile): 3 TMA stages + one reduce buffer (three CTAs fit per SM, see the top of this file);
+// batch 17..32 (32-column tile): ONE buffer + 'consumed' barrier, which frees the shared memory for a 4th TMA stage, or with
+// VCLA_CSK_NBUF = 2 a double-buffered reduce + 3 stages.
+static bool csk_double_buffered_32() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("VCLA_CSK_NBUF"); v = e != nullptr ? atoi(e) : 0; }
-  return v;
-}
-static bool csk_double_buffered(int B) {
-  const int f = csk_nbuf_env();
-  if (f == 1) return false;
-  if (f == 2) return true;
-  return B <= 16;
+  return v == 2;
 }
 
 // int8 weights: half the A stage, so every batch tile is double buffered with a deeper ring, and batches 33..64 get a 64-column tile
@@ -502,8 +540,26 @@ int gemm_csk_clusters(int B, int splits, bool q8) {
     const int bn = csk_q8_bn(B);
     return bn == 16 ? csk_max_clusters<16, 8, 2, true>(splits) : bn == 32 ? csk_max_clusters<32, 6, 2, true>(splits) : csk_max_clusters<64, 4, 1, true>(splits);
   }
-  if (csk_double_buffered(B)) return B <= 16 ? csk_max_clusters<16, 4, 2>(splits) : csk_max_clusters<32, 3, 2>(splits);
-  return B <= 16 ? csk_max_clusters<16, 5, 1>(splits) : csk_max_clusters<32, 4, 1>(splits);
+  if (B <= 16) return csk_max_clusters<16, 3, 1>(splits);
+  return csk_double_buffered_32() ? csk_max_clusters<32, 3, 2>(splits) : csk_max_clusters<32, 4, 1>(splits);
+}
+
+template <int BN, int STAGES, int NBUF, bool Q8 = false>
+static int csk_ctas_per_sm() {
+  int n = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, gemm_csk_kernel<BN, STAGES, NBUF, Q8>, kCskThreads, CskCfg<BN, STAGES, NBUF, Q8>::SMEM_BYTES);
+  if (e != cudaSuccess) { set_error("gemm_csk_ctas_per_sm: %s", cudaGetErrorString(e)); (void)cudaGetLastError(); return -1; }
+  return n;
+}
+
+int gemm_csk_ctas_per_sm(int B, bool q8) {
+  if (csk_init()) return -1;
+  if (q8) {
+    const int bn = csk_q8_bn(B);
+    return bn == 16 ? csk_ctas_per_sm<16, 8, 2, true>() : bn == 32 ? csk_ctas_per_sm<32, 6, 2, true>() : csk_ctas_per_sm<64, 4, 1, true>();
+  }
+  if (B <= 16) return csk_ctas_per_sm<16, 3, 1>();
+  return csk_double_buffered_32() ? csk_ctas_per_sm<32, 3, 2>() : csk_ctas_per_sm<32, 4, 1>();
 }
 
 int gemm_csk(const CskCall& c, cudaStream_t st) {
@@ -537,8 +593,8 @@ int gemm_csk(const CskCall& c, cudaStream_t st) {
     const int bn = csk_q8_bn(c.B);
     return bn == 16 ? csk_launch<16, 8, 2, true>(c, p, st) : bn == 32 ? csk_launch<32, 6, 2, true>(c, p, st) : csk_launch<64, 4, 1, true>(c, p, st);
   }
-  if (csk_double_buffered(c.B)) return c.B <= 16 ? csk_launch<16, 4, 2>(c, p, st) : csk_launch<32, 3, 2>(c, p, st);
-  return c.B <= 16 ? csk_launch<16, 5, 1>(c, p, st) : csk_launch<32, 4, 1>(c, p, st);
+  if (c.B <= 16) return csk_launch<16, 3, 1>(c, p, st);
+  return csk_double_buffered_32() ? csk_launch<32, 3, 2>(c, p, st) : csk_launch<32, 4, 1>(c, p, st);
 }
 
 }  // namespace vcla

@@ -118,6 +118,7 @@ struct CskCall {
 };
 int gemm_csk(const CskCall& c, cudaStream_t st);
 int gemm_csk_clusters(int B, int splits, bool q8 = false);   // clusters of `splits` CTAs that can be co-resident (occupancy query, cached)
+int gemm_csk_ctas_per_sm(int B, bool q8 = false);            // resident CTAs per SM of the kernel batch B runs (occupancy query)
 int trace_set_gemm(void* buf, unsigned long long cap);
 int trace_set_attention(void* buf, unsigned long long cap);
 int trace_set_gemm_decode(void* buf, unsigned long long cap);
@@ -181,6 +182,7 @@ struct DecodeAttnCall {
   int persistent_grid = 0;             // VCLA_ATTN_PERSISTENT_GRID
 };
 int attention_decode(const DecodeAttnCall& c, cudaStream_t st);
+int attention_decode_ctas_per_sm(const DecodeAttnCall& c);     // resident CTAs per SM of the kernel attention_decode picks for c
 int attention_init();          // sets the dynamic-smem attributes and reads the VCLA_ATTN_* switches once (call outside graph capture)
 
 // ------------------------------------------------------------------------------------------

@@ -95,6 +95,7 @@ _SIGNATURES = [
     ("vcla_op_gemm_q8", C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P]),
     ("vcla_debug_set_csk_splits", C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     ("vcla_debug_get_csk_splits", C.c_int, [_P, C.c_int, C.POINTER(C.c_int * 5)]),
+    ("vcla_debug_decode_ctas_per_sm", C.c_int, [_P, C.c_int, C.POINTER(C.c_int * 2)]),
     ("vcla_set_attention_tc", None, [C.c_int]),
     ("vcla_op_attention", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, C.c_int,
                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _P]),
