@@ -210,6 +210,33 @@ int vcla_read_finished(vcla_ctx* ctx, int32_t* dst_dev, int B, vcla_stream strea
 int vcla_op_sample(const float* logits_dev, int B, int V, const int32_t* history_dev, int L, const vcla_sampler* sampler,
                    int32_t* tok_dev, float* scores_out_dev, vcla_stream stream);
 
+/* ---- prompt lookup decoding (HF GenerationConfig.prompt_lookup_num_tokens / max_matching_ngram_size) ------------------------------
+ * One resident sequence (B = 1).  With a lookup set, every step of vcla_decode_multi is a verification step: k + 1 rows -- the last
+ * emitted token and up to k tokens copied from earlier text -- run through one decode step (the split counts of a one-row step, so
+ * each row's logits are bit-identical to a one-token step at that position), each row is picked by the argmax or, with a sampler set,
+ * by the sampler at that row's length (draw counter (length, 0), history extended by the drafts it verifies), and the picks up to and
+ * including the first one that differs from the next draft are emitted (HF:generation/utils.py _assisted_decoding), stopping after an
+ * EOS id and at max_new history rows.  The next drafts follow HF:generation/candidate_generator.py
+ * PromptLookupCandidateGenerator.get_candidates over prompt_ids ++ the emitted tokens: for g = min(n, len - 1) .. 1 the leftmost
+ * earlier window equal to the last g tokens, up to k tokens of its continuation, clamped to max_new - emitted - 1.  A step emits 1 to
+ * k + 1 tokens, the same tokens one-token decoding emits; steps after the end emit nothing.  The first decode call after a prefill
+ * reserves pages and drafts the first step.  k is clamped to 15 and further to the rows the one-row split counts can reduce together.
+ * With the token stream armed, each verification step publishes the tokens it emits (vcla_stream_wait counts history rows).
+ * vcla_set_lookup refuses beam search, the data-parallel exchange and more than one resident sequence; vcla_decode_multi refuses
+ * B != 1 and prefill length + max_new + k > max_seq.  n above 16 is searched as 16 (drafts only).  prompt_ids is copied.
+ * Restates HF:generation/utils.py:3603-3620 and HF:generation/candidate_generator.py:1057-1149.  NULL: off (plain decode steps). */
+typedef struct {
+  int k;                        /* drafted tokens per step, >= 1 */
+  int n;                        /* largest n-gram matched, >= 1 (HF default 2) */
+  int max_new;                  /* max_new_tokens: history rows after which steps emit nothing */
+  const int64_t* prompt_ids;    /* device int64 (prompt_len): the text searched before the emitted tokens */
+  int prompt_len;
+} vcla_lookup;
+int vcla_set_lookup(vcla_ctx* ctx, const vcla_lookup* lookup_or_null, vcla_stream stream);
+/* Synchronises.  out[0] = history rows (emitted tokens incl. the prefill's pick), out[1] = finished flag, out[2] = verification steps
+ * that emitted, out[3] = drafts offered, out[4] = drafts emitted (counters since vcla_set_lookup), out[5] = rows per verification step. */
+int vcla_read_lookup_stats(vcla_ctx* ctx, int64_t* out6_host, vcla_stream stream);
+
 /* ---- beam search without sampling (HF:generation/utils.py:2876-3395, the vectorised _beam_search; reached from the reference's
  * generate(num_beams=...), models/visualcla/modeling_visualcla.py:382-391) ---------------------------------------------------------
  * With beam mode set, vcla_prefill prefills each of its B prompts once, runs the first selection on the prompts' last logits and forks
@@ -290,7 +317,9 @@ int64_t vcla_kernel_launches(vcla_ctx* ctx, int reset);
 
 /* ---- introspection for parity tests ---------------------------------------------------------- */
 /* Copy an internal fp32 activation to the host (synchronises): "vit_out" (B,tokens,v_hidden), "post_ln",
- * "resampler_out" (B,nq,r_hidden), "projector_out" (B,nq,t_hidden), "inputs_embeds" n/a after prefill. */
+ * "resampler_out" (B,nq,r_hidden), "projector_out" (B,nq,t_hidden), "inputs_embeds" n/a after prefill; "step_logits" (B,V): the
+ * logits rows of the last decode or verification step on the cluster split-K schedule (B <= 32 rows); "lookup_tokens" (B): the int32
+ * input tokens (bit patterns in the f32 buffer) of the next prompt lookup verification step. */
 int vcla_read_stage(vcla_ctx* ctx, const char* stage, int B, float* dst_host, vcla_stream stream);
 
 /* ---- operator-level entry points (kernel parity tests, micro-benchmarks) ---------------------- */
@@ -361,6 +390,12 @@ int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, c
 int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq,
                              int page_tokens, const int32_t* seq_len_dev, void* out, int B, int H, int kv_splits, float scale,
                              float rope_theta, int persistent, int persistent_grid, int launches, vcla_stream stream);
+/* Operator entry of the verification attention (tests): rows (2..16) query rows of ONE sequence of length seq_len_dev[0] cached tokens;
+ * row r at position seq_len + r appends its K/V, then attends over keys [0, seq_len + r] with the one-token kernel's arithmetic at
+ * length seq_len + r + 1 and kv_splits splits.  qkv_partial [splits][rows][3 * H * 128], out [rows][H * 128].  Synchronises. */
+int vcla_op_attention_decode_lookup(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq,
+                                    int page_tokens, const int32_t* seq_len_dev, void* out, int rows, int H, int kv_splits, float scale,
+                                    float rope_theta, vcla_stream stream);
 /* The greedy pick of vcla_decode_step on caller buffers: logits_out f32 (B, V) or NULL = sum over splits (in split order) of partial f32
  * [splits][B][ldp] (ldp >= V; columns >= V are not read), tok_out int32 (B) = its argmax, the smallest index among equal maxima as
  * torch.argmax; a row that is -inf everywhere gives 0.  Synchronises. */

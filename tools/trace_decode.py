@@ -14,7 +14,7 @@ pdl = int(sys.argv[2]) if len(sys.argv) > 2 else 1
 out_path = sys.argv[3] if len(sys.argv) > 3 else None
 N.load().vcla_set_pdl(pdl)
 TAGS = {1: "gemm_swap", 2: "gemm", 3: "attn_prefill", 4: "attn_decode", 5: "layernorm", 6: "rmsnorm", 7: "rope_cache", 8: "resid_norm",
-        9: "silu_mul", 10: "logits1", 11: "logits2", 12: "advance", 13: "embed", 14: "sampler"}
+        9: "silu_mul", 10: "logits1", 11: "logits2", 12: "advance", 13: "embed", 14: "sampler", 19: "attn_lookup_append", 20: "lookup_accept"}
 m = visualcla.VisualCLAModel.from_synthetic("7b", seed=0, max_batch=B, max_seq=400, max_prefill_tokens=B * 128)
 m.image_at_head = True
 eng = m._engine

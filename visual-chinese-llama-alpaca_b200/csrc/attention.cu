@@ -248,7 +248,13 @@ constexpr int kDecMaxPT = 64;       // page_tokens supported by the smem ring
 // 16 KB), so whole pages are streamed with TMA bulk copies (cp.async.bulk, mbarrier completion) into a 2- or 3-stage shared-memory
 // ring and the dot products / PV accumulation run out of shared memory: the kernel is bandwidth- instead of latency-bound
 // (the register-prefetch version had one DRAM round trip per 32 tokens per CTA).
-template <int STAGES>
+//
+// Prompt lookup verification (MODE != kDecPlain): blockIdx.z is query row r of sequence 0, the token at position seq_len[0] + r.  Row r
+// runs exactly the arithmetic of the one-token kernel at length seq_len[0] + r + 1.  Rows read keys that lower rows append, and CTAs
+// of one launch cannot rely on each other's stores, so a verification step launches this kernel twice: kDecAppend (grid (1, H, R), no
+// KV stream) writes the RoPE'd K and V of all R rows, then kDecAttend attends without writing the cache.
+constexpr int kDecPlain = 0, kDecAttend = 1, kDecAppend = 2;
+template <int STAGES, int MODE = kDecPlain>
 __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_decode_kernel(const DecodeAttnCall c, const float* __restrict__ rope_cos,
                                                                                   const float* __restrict__ rope_sin) {
   constexpr int HD = 128;
@@ -265,7 +271,8 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int T = c.H * HD, PT = c.page_tokens;
   const uint32_t stage_bytes = (uint32_t)PT * HD * 2 * 2;      // K page + V page
-  TraceScope trace(4);
+  TraceScope trace(MODE == kDecAppend ? 19 : 4);
+  const int sb = MODE == kDecPlain ? b : 0;   // the sequence whose pages and length this CTA reads
 
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) mbar_init(smem_u32(&s_bar[s]), 1);
@@ -276,20 +283,20 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
   trace.dep();
   __syncthreads();
 
-  const int L = c.seq_len[b];          // tokens already cached; the new token gets index L
+  const int L = c.seq_len[sb] + (MODE == kDecPlain ? 0 : b);   // tokens already cached; the new token gets index L
   const int n = L + 1;
   int chunk = (n + c.kv_splits - 1) / c.kv_splits;
   chunk = (chunk + PT - 1) / PT * PT;                 // splits own whole pages
   const int t_begin = split * chunk;
   const int t_end = min(n, t_begin + chunk);
-  const bool owns_new = (t_begin <= L) && (L < t_end);
+  const bool owns_new = MODE == kDecAppend || ((t_begin <= L) && (L < t_end));
   const int c_end = min(t_end, L);                    // cached tokens of this CTA: [t_begin, c_end)
   const int p0 = t_begin / PT;
-  const int npages = c_end > t_begin ? (c_end - t_begin + PT - 1) / PT : 0;
+  const int npages = (MODE != kDecAppend && c_end > t_begin) ? (c_end - t_begin + PT - 1) / PT : 0;
 
   auto issue_page = [&](int i) {                      // thread 0: request page i of this CTA into stage i % STAGES
     const int stage = i % STAGES;
-    const int page = __ldg(c.page_table + (size_t)b * c.pages_per_seq + p0 + i);
+    const int page = __ldg(c.page_table + (size_t)sb * c.pages_per_seq + p0 + i);
     const int ntok = min(PT, c_end - (t_begin + i * PT));
     const uint32_t bytes = (uint32_t)ntok * HD * 2;
     const uint32_t bar = smem_u32(&s_bar[stage]);
@@ -333,16 +340,19 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
         const bf16 kb = __float2bfloat16(kr), vb = __float2bfloat16(vv);
         s_k[d] = __bfloat162float(kb);
         s_v[d] = __bfloat162float(vb);
-        const int page = c.page_table[(size_t)b * c.pages_per_seq + L / PT];
-        const int slot = L % PT;
-        bf16* kdst = c.kv_pages + ((((size_t)page * 2 + 0) * c.H + h) * PT + slot) * HD;
-        bf16* vdst = c.kv_pages + ((((size_t)page * 2 + 1) * c.H + h) * PT + slot) * HD;
-        kdst[d] = kb;
-        vdst[d] = vb;
+        if (MODE != kDecAttend) {
+          const int page = c.page_table[(size_t)sb * c.pages_per_seq + L / PT];
+          const int slot = L % PT;
+          bf16* kdst = c.kv_pages + ((((size_t)page * 2 + 0) * c.H + h) * PT + slot) * HD;
+          bf16* vdst = c.kv_pages + ((((size_t)page * 2 + 1) * c.H + h) * PT + slot) * HD;
+          kdst[d] = kb;
+          vdst[d] = vb;
+        }
       }
     }
     __syncthreads();
   }
+  if constexpr (MODE == kDecAppend) { trace.done(); return; }
 
   // ---- attention over the cached tokens, page by page out of shared memory.  8 lanes per token; lane `sub` owns the 16 B
   //      chunks `sub` and `sub + 8` of a 256 B row (dims [8 sub, 8 sub + 8) and [64 + 8 sub, 64 + 8 sub + 8)): a quarter warp
@@ -719,6 +729,8 @@ int attention_init() {
     rc |= set((const void*)attn_decode_kernel<kDecStages>, kDecStages * kDecMaxPT * 128 * 2 * 2);
     rc |= set((const void*)attn_decode_kernel<kDecStagesSmallBatch>, kDecStagesSmallBatch * kDecMaxPT * 128 * 2 * 2);
     rc |= set((const void*)attn_decode_persistent_kernel, kDecStages * kDecMaxPT * 128 * 2 * 2);
+    rc |= set((const void*)attn_decode_kernel<kDecStages, kDecAttend>, kDecStages * kDecMaxPT * 128 * 2 * 2);
+    rc |= set((const void*)attn_decode_kernel<kDecStagesSmallBatch, kDecAttend>, kDecStagesSmallBatch * kDecMaxPT * 128 * 2 * 2);
     rc |= set((const void*)attn_prefill_kernel<128>, 5 * 64 * 128 * 2);
     rc |= set((const void*)attn_prefill_kernel<64>, 5 * 64 * 64 * 2);
     if (rc) set_error("attention_init: cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -770,6 +782,31 @@ int attention_decode(const DecodeAttnCall& c, cudaStream_t st) {
     case kDecOneShot3:
       VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStages>, c, c.rope_cos, c.rope_sin));
       break;
+  }
+  return 0;
+}
+
+int attention_decode_lookup(const DecodeAttnCall& c, cudaStream_t st) {
+  if (c.HD != 128) { set_error("attention_decode_lookup: head dim %d unsupported (128)", c.HD); return -1; }
+  if (c.page_tokens < 8 || c.page_tokens > kDecMaxPT || c.page_tokens % 8 != 0) { set_error("attention_decode_lookup: page_tokens %d unsupported (8..%d, multiple of 8)", c.page_tokens, kDecMaxPT); return -1; }
+  if (c.rope_cos == nullptr || c.rope_sin == nullptr) { set_error("attention_decode_lookup: rope table not initialised"); return -1; }
+  if (c.kv_splits < 1 || c.kv_splits > 8 || c.B < 1 || c.B > 16) { set_error("attention_decode_lookup: %d rows x %d KV splits unsupported", c.B, c.kv_splits); return -1; }
+  if (attention_init()) return -1;
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  int na = 0;
+  if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
+  cfg.attrs = attr; cfg.numAttrs = na; cfg.stream = st; cfg.blockDim = dim3(kDecWarps * 32);
+  cfg.gridDim = dim3(1, c.H, c.B); cfg.dynamicSmemBytes = 0;
+  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch, kDecAppend>, c, c.rope_cos, c.rope_sin));
+  // the ring depth changes no arithmetic; the one-token rule picks it from the grid size
+  cfg.gridDim = dim3(c.kv_splits, c.H, c.B);
+  if (c.kv_splits * c.B * c.H <= 2 * num_sms()) {
+    cfg.dynamicSmemBytes = (size_t)kDecStagesSmallBatch * c.page_tokens * 128 * 2 * 2;
+    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch, kDecAttend>, c, c.rope_cos, c.rope_sin));
+  } else {
+    cfg.dynamicSmemBytes = (size_t)kDecStages * c.page_tokens * 128 * 2 * 2;
+    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStages, kDecAttend>, c, c.rope_cos, c.rope_sin));
   }
   return 0;
 }

@@ -633,6 +633,93 @@ int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_
   return 0;
 }
 
+// ---- prompt lookup decoding: accept, advance and draft (one CTA, B = 1) ---------------------------------------------------------
+__global__ void __launch_bounds__(256) lookup_accept_kernel(const LookupCall c, int prime) {
+  __shared__ int s_done, s_prod, s_best;
+  TraceScope trace(20);
+  pdl_launch_dependents();
+  pdl_wait();
+  trace.dep();
+  const int tid = threadIdx.x;
+  const int max_new = c.state->max_new;
+  if (tid == 0) {
+    int produced = *c.step_idx;
+    bool done = produced >= max_new || c.finished[0] != 0;
+    if (!prime && !done) {
+      // HF _assisted_decoding: n_matches = leading drafts equal to the model's picks; the picks of rows 0..n_matches are emitted
+      const int nd = c.state->nd;
+      int a = 0;
+      while (a < nd && c.pick[a] == c.tok[a + 1]) ++a;
+      int cnt = 0, fin = 0;
+      for (int j = 0; j <= a && produced + cnt < max_new && !fin; ++j) {
+        const int t = c.pick[j];
+        c.history[produced + cnt] = t;
+        ++cnt;
+        if (c.samp) for (int e = 0; e < c.samp->n_eos; ++e) fin |= t == c.samp->eos[e];   // plain decoding stops at the EOS too
+      }
+      if (fin) c.finished[0] = 1;
+      c.seq_len[0] += cnt;                    // row 0 and the accepted drafts before the last emitted token are cached now
+      if (c.ring != nullptr) {
+        // the ring has as many rows as the history (max_seq + 2): every emitted row has a ring row
+        for (int j = 0; j < cnt; ++j) c.ring->tokens[(size_t)(produced + j) * 64] = c.history[produced + j];
+        __threadfence_system();
+        st_release_sys(&c.ring->published, produced + cnt);
+      }
+      produced += cnt;
+      *c.step_idx = produced;
+      c.state->steps += 1; c.state->drafted += nd; c.state->accepted += cnt - 1;
+      done = produced >= max_new || fin;
+    }
+    // pages for the R rows the next step appends (idle steps after the end append there too, beyond seq_len)
+    int need = c.seq_len[0] + c.R;
+    int np = (need + c.page_tokens - 1) / c.page_tokens;
+    if (np > c.pages_per_seq) np = c.pages_per_seq;
+    if (np > c.kv_npages[0]) { int tokens[1] = {need}; kv_reserve_serial(c.kv_free, c.kv_state, c.kv_npages, c.page_table, c.pages_per_seq, c.page_tokens, 1, tokens); }
+    s_done = done; s_prod = produced; s_best = 0x7fffffff;
+  }
+  __syncthreads();
+  if (s_done) { trace.done(); return; }
+  // HF PromptLookupCandidateGenerator.get_candidates over text = prompt ids ++ emitted tokens: for g = min(n, N - 1) .. 1, the leftmost
+  // earlier window equal to the last g tokens whose continuation is non-empty (every window but the tail itself); draft = up to R - 1
+  // tokens of that continuation, clamped so that produced + drafts + 1 <= max_new
+  const int produced = s_prod, P = c.state->prompt_len, N = P + produced;
+  auto at = [&](int i) -> int { return i < P ? (int)c.prompt[i] : c.history[i - P]; };
+  int start = -1;
+  for (int g = min(c.state->n, N - 1); g >= 1; --g) {
+    for (int i = tid; i < N - g; i += blockDim.x) {
+      bool same = true;
+      for (int j = 0; j < g && same; ++j) same = at(i + j) == at(N - g + j);
+      if (same) atomicMin(&s_best, i);
+    }
+    __syncthreads();
+    const int best = s_best;
+    __syncthreads();                          // every thread has read s_best before the next n-gram size may lower it
+    if (best != 0x7fffffff) { start = best + g; break; }
+  }
+  if (tid == 0) {
+    int nd = 0;
+    if (start >= 0) nd = min(min(c.R - 1, N - start), max_new - produced - 1);
+    if (nd < 0) nd = 0;
+    const int last = c.history[produced - 1];
+    c.tok[0] = last;
+    for (int j = 1; j < c.R; ++j) {
+      const int t = j <= nd ? at(start + j - 1) : last;
+      c.tok[j] = t;
+      c.history[produced + j - 1] = t;        // provisional: row j's sampler reads the history extended by drafts 1..j-1
+    }
+    c.state->nd = nd;
+  }
+  trace.done();
+}
+int lookup_accept(const LookupCall& c, int prime, cudaStream_t st) {
+  if (c.R < 2 || c.R > 16 || !c.prompt || !c.tok || !c.pick || !c.history || !c.step_idx || !c.seq_len ||
+      !c.finished || !c.state) {
+    set_error("lookup_accept: bad arguments"); return -1;
+  }
+  VCLA_LAUNCH(lookup_accept_kernel, dim3(1), dim3(256), 0, st, c, prime);
+  return 0;
+}
+
 // ---- beam search: rows continue their parents' pages (shared through the page table, copy-on-write for the page written next) ----
 // Pages are never shared across a row boundary of positions: a page covers positions [i * page_tokens, (i + 1) * page_tokens) and sits at
 // index i of every row that references it.  Rows that share page i also share every page before it (a fork copies the parent's row;

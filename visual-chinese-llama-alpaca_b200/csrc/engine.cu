@@ -59,7 +59,9 @@ struct TextLayer {
 struct GraphKey {
   int B; const void* tok_in; const void* logits; const void* tok_out; int n_steps = 1; int dp = 0; int samp = 0; int beam = 0;
   int stream = 0;   // captured armed: every step publishes into the token stream ring
+  int lookup = 0;   // prompt lookup: rows per verification step (0: plain decode steps)
   bool operator<(const GraphKey& o) const {
+    if (lookup != o.lookup) return lookup < o.lookup;
     if (B != o.B) return B < o.B;
     if (tok_in != o.tok_in) return tok_in < o.tok_in;
     if (logits != o.logits) return logits < o.logits;
@@ -129,6 +131,9 @@ struct vcla_ctx {
   StreamRing *ring_host = nullptr, *ring_dev = nullptr; bool stream_armed = false;
   cudaEvent_t stream_done = nullptr; bool stream_pending = false;
   StreamRing* ring() const { return stream_armed ? ring_dev : nullptr; }
+  // prompt lookup decoding (vcla_set_lookup): verification steps of lk_rows rows replace the decode steps of the one resident sequence
+  bool lk_on = false, lk_primed = false; int lk_rows = 0, lk_max_new = 0;
+  int64_t* lk_prompt = nullptr; int32_t *lk_tok = nullptr, *lk_pick = nullptr; LookupState* lk_state = nullptr;
   int64_t len_bound = 0;   // host-side upper bound of the cached tokens per sequence (prefill S + decode steps issued since)
   int resident_b = 0;      // sequences resident since the last vcla_prefill (0 after vcla_reset)
   // vision activations
@@ -390,6 +395,10 @@ void layout_activations(vcla_ctx* c) {
   c->beam_copy = a_alloc<int32_t>(c, 1 + 3 * Bp);
   c->beam_table_tmp = a_alloc<int32_t>(c, (size_t)g.max_batch * c->pages_per_seq);
   c->beam_cow_bytes = a_alloc<unsigned long long>(c, 1);
+  c->lk_prompt = a_alloc<int64_t>(c, (size_t)g.max_seq);
+  c->lk_tok = a_alloc<int32_t>(c, 16);
+  c->lk_pick = a_alloc<int32_t>(c, 16);
+  c->lk_state = a_alloc<LookupState>(c, 1);
 }
 
 // Split-K factor of a decode GEMM (row tiles of 128 x `splits` work units on 2 persistent CTAs per SM).  A thin last wave is
@@ -1135,6 +1144,7 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
   if (c->beam_on && beam_reorder(c, B, B * c->beam_K, next_tok ? next_tok : c->d_tok, st)) return -1;
   c->len_bound = S;
   c->resident_b = c->beam_on ? B * c->beam_K : B;
+  c->lk_primed = false;
   return stream_mark(c, st);
 }
 
@@ -1160,6 +1170,7 @@ int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* lo
   count(c); if (advance_seq(c->seq_len, B, T, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st,
                             c->ring(), c->tok_hist)) return -1;
   c->len_bound += T;
+  c->lk_primed = false;
   return stream_mark(c, st);
 }
 
@@ -1273,8 +1284,43 @@ static int decode_enqueue(vcla_ctx* c, const int32_t* tok_in, int B, float* logi
   return decode_uses_csk(c, B) ? decode_enqueue_csk(c, tok_in, B, logits, tok_out, st) : decode_enqueue_workspace(c, tok_in, B, logits, tok_out, st);
 }
 
+static LookupCall lookup_call(vcla_ctx* c) {
+  LookupCall k; k.R = c->lk_rows; k.prompt = c->lk_prompt;
+  k.tok = c->lk_tok; k.pick = c->lk_pick; k.history = c->tok_hist; k.step_idx = c->step_idx; k.seq_len = c->seq_len; k.finished = c->finished;
+  k.samp = c->samp_on ? c->samp_params : nullptr; k.state = c->lk_state;
+  k.kv_free = c->kv_free; k.kv_state = c->kv_state; k.kv_npages = c->kv_npages; k.page_table = c->page_table;
+  k.pages_per_seq = c->pages_per_seq; k.page_tokens = c->page_tokens; k.ring = c->ring();
+  return k;
+}
+
+// Prompt lookup verification step of the one resident sequence: the cluster split-K schedule over R = lk_rows rows with the split
+// counts of a one-row step (csk_prepare(c, 1)), so every row's logits are those of a one-token step; attention in its multi-query
+// mode with the one-row KV split count; the picks of all rows; then accept / advance / draft in place of advance_seq.
+static int decode_enqueue_lookup(vcla_ctx* c, cudaStream_t st) {
+  const vcla_config& g = c->cfg;
+  const int TH = g.t_hidden, V = g.t_vocab, R = c->lk_rows;
+  count(c); if (dec_embed(c->lk_tok, R, TH, c->embed, V, c->d_resid, c->tl[0].ln1, c->d_xn, c->d_ssq, (TH + 127) / 128, st)) return -1;
+  for (int i = 0; i < g.t_layers; ++i) {
+    if (csk_gemm(c, DG_QKV, i, R, st)) return -1;
+    DecodeAttnCall a = decode_attn_call(c, c->tl[i], 1, 1);
+    a.B = R; a.ws_rows = R;
+    count(c, 2); if (attention_decode_lookup(a, st)) return -1;
+    if (csk_gemm(c, DG_O, i, R, st) || csk_gemm(c, DG_GATE_UP, i, R, st) || csk_gemm(c, DG_DOWN, i, R, st)) return -1;
+  }
+  if (csk_gemm(c, DG_LM_HEAD, 0, R, st)) return -1;
+  count(c, 2);
+  if (c->samp_on) {
+    if (dec_logits_reduce(c->ws_lm, 1, R, V, R, V, c->samp_logits, V, c->cand_val, c->cand_idx, st) ||
+        dec_sample_lookup(c->samp_logits, V, V, R, c->tok_hist, c->step_idx, c->samp_params, c->lk_pick, st)) return -1;
+  } else {
+    if (dec_logits_argmax(c->ws_lm, 1, R, V, R, V, nullptr, V, c->lk_pick, nullptr, nullptr, c->cand_val, c->cand_idx, nullptr, st)) return -1;
+  }
+  count(c); return lookup_accept(lookup_call(c), 0, st);
+}
+
 static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, int n_steps, cudaStream_t st) {
-  GraphKey key{B, tok_in, logits, tok_out, n_steps, c->dp_on() ? 1 : 0, c->samp_on ? 1 : 0, c->beam_on ? c->beam_K : 0, c->stream_armed ? 1 : 0};
+  GraphKey key{B, tok_in, logits, tok_out, n_steps, c->dp_on() ? 1 : 0, c->samp_on ? 1 : 0, c->beam_on ? c->beam_K : 0, c->stream_armed ? 1 : 0,
+               c->lk_on ? c->lk_rows : 0};
   auto it = c->graphs.find(key);
   if (it == c->graphs.end()) {
     const int64_t before = c->launches;
@@ -1282,7 +1328,8 @@ static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits
     if (!c->cap_stream) VCLA_CUDA_OK(cudaStreamCreateWithFlags(&c->cap_stream, cudaStreamNonBlocking));
     VCLA_CUDA_OK(cudaStreamBeginCapture(c->cap_stream, cudaStreamCaptureModeThreadLocal));
     int rc = 0;
-    for (int i = 0; i < n_steps && rc == 0; ++i) rc = decode_enqueue(c, tok_in, B, logits, tok_out, c->cap_stream);
+    for (int i = 0; i < n_steps && rc == 0; ++i)
+      rc = c->lk_on ? decode_enqueue_lookup(c, c->cap_stream) : decode_enqueue(c, tok_in, B, logits, tok_out, c->cap_stream);
     if (rc == 0 && c->dp_on()) rc = dp_wait(c, c->cap_stream);      // a captured graph must join its forked exchange branch
     cudaError_t e = cudaStreamEndCapture(c->cap_stream, &graph);
     if (rc != 0) { if (graph) cudaGraphDestroy(graph); (void)cudaGetLastError(); return -1; }
@@ -1338,6 +1385,7 @@ int vcla_decode_step(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, i
   cudaStream_t st = (cudaStream_t)stream;
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_in || !tok_out) { set_error("decode: null token buffers"); return -1; }
+  if (c->lk_on) { set_error("decode: prompt lookup verification steps run through vcla_decode_multi"); return -1; }
   if (decode_capacity(c, 1, B)) return -1;
   if (decode_uses_csk(c, B) && csk_prepare(c, B)) return -1;      // occupancy queries: never inside a capture
   int rc = use_graph ? decode_graph(c, tok_in, B, logits, tok_out, 1, st) : decode_enqueue(c, tok_in, B, logits, tok_out, st);
@@ -1351,6 +1399,25 @@ int vcla_decode_multi(vcla_ctx* c, int32_t* tok_inout, int B, int n_steps, vcla_
   // every chosen token is appended to the device-side history): amortises the gap between consecutive graph launches.
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_inout || n_steps < 1 || n_steps > 64) { set_error("decode_multi: bad arguments"); return -1; }
+  if (c->lk_on) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (c->len_bound <= 0) { set_error("decode: no prefilled sequences (call vcla_prefill first)"); return -1; }
+    if (B != 1 || c->resident_b != 1) { set_error("decode: prompt lookup steps one resident sequence (got B=%d, %d resident)", B, c->resident_b); return -1; }
+    if (csk_prepare(c, 1)) return -1;
+    if (!c->lk_primed) {
+      // right after the prefill: history rows = the prefill's pick, seq_len = the prompt
+      if (c->len_bound + c->lk_max_new + c->lk_rows - 1 > c->cfg.max_seq) {
+        set_error("decode: %lld cached tokens + max_new %d + %d drafts exceed the context capacity max_seq=%d", (long long)c->len_bound,
+                  c->lk_max_new, c->lk_rows - 1, c->cfg.max_seq);
+        return -1;
+      }
+      count(c); if (lookup_accept(lookup_call(c), 1, st)) return -1;
+      c->lk_primed = true;
+      c->len_bound += c->lk_max_new - 1;     // upper bound: at most max_new - 1 decoded tokens are cached
+    }
+    const int rc = decode_graph(c, tok_inout, 1, nullptr, tok_inout, n_steps, st);
+    return rc == 0 ? stream_mark(c, st) : rc;
+  }
   if (decode_capacity(c, n_steps, B)) return -1;
   if (decode_uses_csk(c, B) && csk_prepare(c, B)) return -1;
   const int rc = decode_graph(c, tok_inout, B, nullptr, tok_inout, n_steps, (cudaStream_t)stream);
@@ -1416,6 +1483,63 @@ int vcla_op_sample(const float* logits_dev, int B, int V, const int32_t* history
 }
 
 // -------------------------------------------------------------------------------------------------
+// prompt lookup decoding
+// -------------------------------------------------------------------------------------------------
+// Rows a verification step may run: k + 1 <= 16 (the 16-column batch tile), and every one-row split count S must reduce the rows
+// together: S * ceil(rows / S) <= 20 reduce-buffer columns of that tile (gemm_csk).  Fewer rows change the speed, never the tokens.
+static int lookup_rows(vcla_ctx* c, int k) {
+  if (csk_prepare(c, 1)) return -1;
+  const int splits[5] = {c->csk_qkv, c->csk_o, c->csk_gu, c->csk_d, c->csk_lm};
+  int rows = std::min(k, 15) + 1;
+  for (; rows > 2; --rows) {
+    bool ok = true;
+    for (int s : splits) ok = ok && ((rows + s - 1) / s) * s <= 20;
+    if (ok) break;
+  }
+  return rows;
+}
+
+int vcla_set_lookup(vcla_ctx* c, const vcla_lookup* lk, vcla_stream stream) {
+  if (!c) return -1;
+  if (lk == nullptr) {
+    c->lk_on = false;
+    return 0;
+  }
+  if (lk->k < 1 || lk->n < 1 || lk->max_new < 1 || lk->prompt_len < 0 || lk->prompt_len > c->cfg.max_seq || (lk->prompt_len > 0 && !lk->prompt_ids)) {
+    set_error("vcla_set_lookup: bad arguments (k >= 1, n >= 1, max_new >= 1, 0 <= prompt_len <= max_seq)"); return -1;
+  }
+  if (c->beam_on) { set_error("vcla_set_lookup: not available in beam-search mode"); return -1; }
+  if (c->dp_on()) { set_error("vcla_set_lookup: not available while the data-parallel token exchange is active"); return -1; }
+  if (c->resident_b > 1) { set_error("vcla_set_lookup: prompt lookup decodes one sequence (%d resident)", c->resident_b); return -1; }
+  const int rows = lookup_rows(c, lk->k);
+  if (rows < 0) return -1;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (lk->prompt_len > 0) VCLA_CUDA_OK(cudaMemcpyAsync(c->lk_prompt, lk->prompt_ids, (size_t)lk->prompt_len * 8, cudaMemcpyDeviceToDevice, st));
+  LookupState init;
+  memset(&init, 0, sizeof(init));
+  // n-grams longer than 16 are searched as 16: the one-CTA search costs ~n^2 * len / 256 per step, and n changes the drafts only
+  init.n = std::min(lk->n, 16); init.max_new = lk->max_new; init.prompt_len = lk->prompt_len;
+  // pageable source: staged by the driver before the call returns
+  VCLA_CUDA_OK(cudaMemcpyAsync(c->lk_state, &init, sizeof(init), cudaMemcpyHostToDevice, st));
+  c->lk_rows = rows; c->lk_max_new = lk->max_new;
+  c->lk_on = true; c->lk_primed = false;
+  return 0;
+}
+
+int vcla_read_lookup_stats(vcla_ctx* c, int64_t* out, vcla_stream stream) {
+  if (!c || !out) { set_error("vcla_read_lookup_stats: null argument"); return -1; }
+  cudaStream_t st = (cudaStream_t)stream;
+  int32_t step = 0, fin = 0;
+  LookupState s;
+  VCLA_CUDA_OK(cudaMemcpyAsync(&step, c->step_idx, 4, cudaMemcpyDeviceToHost, st));
+  VCLA_CUDA_OK(cudaMemcpyAsync(&fin, c->finished, 4, cudaMemcpyDeviceToHost, st));
+  VCLA_CUDA_OK(cudaMemcpyAsync(&s, c->lk_state, sizeof(s), cudaMemcpyDeviceToHost, st));
+  VCLA_CUDA_OK(cudaStreamSynchronize(st));
+  out[0] = step; out[1] = fin; out[2] = (int64_t)s.steps; out[3] = (int64_t)s.drafted; out[4] = (int64_t)s.accepted; out[5] = c->lk_rows;
+  return 0;
+}
+
+// -------------------------------------------------------------------------------------------------
 // beam search
 // -------------------------------------------------------------------------------------------------
 static int beam_to_params(const vcla_beam* s, int V, BeamParams* p) {
@@ -1442,6 +1566,7 @@ int vcla_set_beam(vcla_ctx* c, const vcla_beam* s) {
   if (!beam_supported(c->cfg.t_vocab)) { set_error("beam: vocabulary %d does not fit the beam-step kernel", c->cfg.t_vocab); return -1; }
   if (c->dp_on()) { set_error("beam: not available while the data-parallel token exchange is active"); return -1; }
   if (c->stream_armed) { set_error("beam: not available while token streaming is armed (vcla_stream_arm)"); return -1; }
+  if (c->lk_on) { set_error("beam: not available while prompt lookup is set (vcla_set_lookup)"); return -1; }
   BeamParams p;
   if (beam_to_params(s, c->cfg.t_vocab, &p)) return -1;
   if (p.K > std::min(c->cfg.max_batch, 64)) { set_error("beam: %d beams exceed min(max_batch, 64) = %d rows", p.K, std::min(c->cfg.max_batch, 64)); return -1; }
@@ -1557,6 +1682,7 @@ int vcla_dp_set_active(vcla_ctx* c, int on) {
   if (!c) return -1;
   if (on && !c->comm) { set_error("vcla_dp_set_active: call vcla_nccl_init first"); return -1; }
   if (on && c->stream_armed) { set_error("vcla_dp_set_active: not available while token streaming is armed (vcla_stream_arm)"); return -1; }
+  if (on && c->lk_on) { set_error("vcla_dp_set_active: not available while prompt lookup is set (vcla_set_lookup)"); return -1; }
   c->dp_active = on != 0;
   return 0;
 }
@@ -1586,6 +1712,8 @@ int vcla_read_stage(vcla_ctx* c, const char* stage, int B, float* dst, vcla_stre
   else if (!strcmp(stage, "post_ln")) { src = c->v_postln_f32; n = (size_t)B * c->v_tokens * g.v_hidden; }
   else if (!strcmp(stage, "resampler_out")) { src = c->r_hidden; n = (size_t)B * g.r_queries * g.r_hidden; }
   else if (!strcmp(stage, "projector_out")) { src = c->img_embeds; n = (size_t)B * g.r_queries * g.t_hidden; }
+  else if (!strcmp(stage, "step_logits")) { src = c->ws_lm; n = (size_t)B * g.t_vocab; }   // B <= 32 rows of the last one-split lm_head
+  else if (!strcmp(stage, "lookup_tokens")) { src = reinterpret_cast<const float*>(c->lk_tok); n = (size_t)B; }   // int32 bits
   else { set_error("vcla_read_stage: unknown stage '%s'", stage); return -1; }
   VCLA_CUDA_OK(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToHost, st));
   VCLA_CUDA_OK(cudaStreamSynchronize(st));
@@ -1906,6 +2034,41 @@ int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_page
     rc = attention_decode(a, st);
   }
   if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_attention_decode: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
+  cudaFree(buf);
+  return rc;
+}
+int vcla_op_attention_decode_lookup(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq,
+                                    int page_tokens, const int32_t* seq_len_dev, void* out, int rows, int H, int kv_splits, float scale,
+                                    float rope_theta, vcla_stream stream) {
+  // operator entry for tests: attention_decode_lookup on caller buffers; the RoPE tables, scratch and counters are made for the call.
+  if (!qkv_partial || !kv_pages || !page_table || !seq_len_dev || !out || splits < 1 || rows < 2 || rows > 16 || H < 1 || pages_per_seq < 1 ||
+      page_tokens < 1 || !(rope_theta > 0.f)) {
+    set_error("vcla_op_attention_decode_lookup: bad arguments"); return -1;
+  }
+  if (kv_splits < 1 || kv_splits > 8) { set_error("vcla_op_attention_decode_lookup: kv_splits %d outside 1..8", kv_splits); return -1; }
+  cudaStream_t st = (cudaStream_t)stream;
+  std::vector<int32_t> table((size_t)pages_per_seq);
+  int32_t len = 0;
+  VCLA_CUDA_OK(cudaStreamSynchronize(st));
+  VCLA_CUDA_OK(cudaMemcpy(table.data(), page_table, table.size() * 4, cudaMemcpyDeviceToHost));
+  VCLA_CUDA_OK(cudaMemcpy(&len, seq_len_dev, 4, cudaMemcpyDeviceToHost));
+  if (len < 0 || (int64_t)len + rows > (int64_t)pages_per_seq * page_tokens) {
+    set_error("vcla_op_attention_decode_lookup: %d + %d tokens exceed the table row (%d pages of %d)", len, rows, pages_per_seq, page_tokens); return -1;
+  }
+  for (int i = 0; i <= (len + rows - 1) / page_tokens; ++i) {
+    if (table[i] < 0) { set_error("vcla_op_attention_decode_lookup: no page %d", i); return -1; }
+  }
+  const size_t rope_floats = (size_t)(len + rows) * 64, scratch_floats = (size_t)rows * H * kv_splits * (128 + 2);
+  float* buf = nullptr;
+  VCLA_CUDA_OK(cudaMalloc(&buf, (2 * rope_floats + scratch_floats + (size_t)rows * H) * 4));
+  DecodeAttnCall a; a.qkv_partial = qkv_partial; a.splits = splits; a.ws_rows = rows; a.kv_pages = (bf16*)kv_pages; a.page_table = page_table;
+  a.pages_per_seq = pages_per_seq; a.page_tokens = page_tokens; a.seq_len = seq_len_dev; a.out = (bf16*)out; a.B = rows; a.H = H; a.HD = 128;
+  a.kv_splits = kv_splits; a.scale = scale; a.rope_theta = rope_theta; a.rope_cos = buf; a.rope_sin = buf + rope_floats;
+  a.scratch = buf + 2 * rope_floats; a.counters = reinterpret_cast<int32_t*>(a.scratch + scratch_floats);
+  int rc = rope_fill_tables(len + rows, 128, rope_theta, buf, buf + rope_floats);
+  if (rc == 0 && cudaMemsetAsync(a.scratch, 0, (scratch_floats + (size_t)rows * H) * 4, st) != cudaSuccess) { set_error("vcla_op_attention_decode_lookup: memset failed"); rc = -1; }
+  if (rc == 0) rc = attention_decode_lookup(a, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_attention_decode_lookup: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
   cudaFree(buf);
   return rc;
 }

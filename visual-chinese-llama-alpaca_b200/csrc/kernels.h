@@ -182,6 +182,10 @@ struct DecodeAttnCall {
   int persistent_grid = 0;             // VCLA_ATTN_PERSISTENT_GRID
 };
 int attention_decode(const DecodeAttnCall& c, cudaStream_t st);
+// Prompt lookup verification over c.B <= 16 query rows of sequence 0 (row r at position seq_len[0] + r, qkv / out row r): two launches,
+// the K/V append of every row, then each row's attention over keys [0, seq_len[0] + r] with the one-token kernel's arithmetic at that
+// length (c.kv_splits must be the split count the one-token call of sequence 0 uses).  scratch / counters are indexed by row.
+int attention_decode_lookup(const DecodeAttnCall& c, cudaStream_t st);
 int attention_decode_ctas_per_sm(const DecodeAttnCall& c);     // resident CTAs per SM of the kernel attention_decode picks for c
 int attention_init();          // sets the dynamic-smem attributes and reads the VCLA_ATTN_* switches once (call outside graph capture)
 
@@ -242,6 +246,10 @@ int sampler_init();
 // history: [L][B] int32 with L = *step_idx; writes tok[b], history_out[L][b], dp_send[b]; finished[b] (nullable): sticky EOS flag
 int dec_sample(const float* logits, int ld, int V, int B, const int32_t* history, const int32_t* step_idx, const SamplerParams* params_dev,
                int32_t* tok, int32_t* history_out, int32_t* dp_send, int32_t* finished, float* scores_out, cudaStream_t st);
+// prompt lookup verification (B = 1): row r < R scores logits row r with the history column of length *step_idx + r and draws with
+// counter (*step_idx + r, 0); tok[r] = pick.  No history, finished or send-buffer writes.
+int dec_sample_lookup(const float* logits, int ld, int V, int R, const int32_t* history, const int32_t* step_idx, const SamplerParams* params_dev,
+                      int32_t* tok, cudaStream_t st);
 int dp_unpack(const int32_t* recv, int n, int32_t* hist, int32_t* dp_step, cudaStream_t st);
 // ---- beam search (beam.cu; HF:generation/utils.py:2876-3395 with decoder_prompt_len = 0) ---------------------------------------
 constexpr int kBeamMaxK = 16;
@@ -296,6 +304,33 @@ inline size_t stream_ring_bytes(int rows) { return offsetof(StreamRing, tokens) 
 int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, int32_t* kv_free, int32_t* kv_state,
                 int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, cudaStream_t st,
                 StreamRing* ring = nullptr, const int32_t* history = nullptr);
+// ---- prompt lookup decoding (one sequence): a verification step runs R = k + 1 rows -- the last emitted token and k drafts -- through
+// the decode step; lookup_accept then replaces advance_seq.  Restates HF:generation/utils.py:3603-3620 (_assisted_decoding, greedy
+// and sampled without an assistant: n_matches = leading drafts equal to the model's picks, valid_tokens = picks[: n_matches + 1],
+// streamer.put(valid_tokens)) and HF:generation/candidate_generator.py:1057-1149 (PromptLookupCandidateGenerator.get_candidates, the
+// draft rule, without its forbidden-token and EOS cropping).
+struct LookupState {          // device memory: graphs captured once serve every call
+  int32_t nd;                 // drafts in rows 1..nd of the current step
+  int32_t n, max_new, prompt_len;   // largest n-gram, max_new_tokens (history rows), prompt ids searched
+  unsigned long long steps, drafted, accepted;   // verification steps that advanced, drafts offered, drafts emitted
+};
+struct LookupCall {
+  int R = 0;                                    // rows
+  const int64_t* prompt = nullptr;
+  int32_t* tok = nullptr;                       // [R] inputs of the next step: row 0 = last emitted token, rows 1..R-1 drafts
+  const int32_t* pick = nullptr;                // [R] pick of each row of the step that just ran
+  int32_t* history = nullptr; int32_t* step_idx = nullptr; int32_t* seq_len = nullptr; int32_t* finished = nullptr;
+  const SamplerParams* samp = nullptr;          // nullable: the EOS ids
+  LookupState* state = nullptr;
+  int32_t *kv_free = nullptr, *kv_state = nullptr, *kv_npages = nullptr, *page_table = nullptr; int pages_per_seq = 0, page_tokens = 0;
+  StreamRing* ring = nullptr;                   // nullable: publish the emitted tokens (as advance_seq does)
+};
+// prime != 0: no acceptance (right after the prefill): reserve pages for R rows and draft the first step.  Otherwise, unless the row is
+// finished or max_new tokens exist: accept the leading matching drafts, emit the picks up to and including the first mismatch (stopping
+// after an EOS id, clamped to max_new) into the history, advance seq_len and the step counter by the emitted count, publish them to the
+// ring (tokens, a system-scope fence, then the count with st.release.sys).  Then reserve pages for the next R rows and write the next
+// step's inputs (drafts also provisionally into the history after the emitted tokens).
+int lookup_accept(const LookupCall& c, int prime, cudaStream_t st);
 // Beam reorder, after advance_seq (so every old row's write position seq_len and its page exist).  New row j (< rows_new) continues
 // old row parent_row[j] (< rows_old): its table row, page count and length are the parent's.  Pages no new row references go back on
 // the free stack; when several rows continue one parent, every one but the first gets a fresh page for the write position plus a

@@ -35,6 +35,10 @@ __device__ __forceinline__ float philox_uniform(unsigned long long seed, uint32_
   return (float)(ctr[0] >> 8) * (1.0f / 16777216.0f);   // [0, 1)
 }
 
+// LOOKUP (prompt lookup verification, B = 1): CTA r scores query row r, whose history is column 0 with length *step_idx + r (the drafts
+// being verified sit provisionally at rows *step_idx ..), and draws with counter (*step_idx + r, 0): exactly the draw one-token decoding
+// makes at that length.  finished is neither read nor written (the accept kernel owns it); tok[r] receives the pick.
+template <bool LOOKUP = false>
 __global__ void __launch_bounds__(kSampThreads, 1)
 dec_sample_kernel(const float* __restrict__ logits, int ld, int V, int B, const int32_t* __restrict__ history, const int32_t* __restrict__ step_idx,
                   const SamplerParams* __restrict__ pp, int32_t* __restrict__ tok, int32_t* __restrict__ history_out, int32_t* __restrict__ dp_send,
@@ -56,17 +60,18 @@ dec_sample_kernel(const float* __restrict__ logits, int ld, int V, int B, const 
   pdl_launch_dependents();
   pdl_wait();
   trace.dep();
-  const int b = blockIdx.x, tid = threadIdx.x;
+  const int b = LOOKUP ? 0 : blockIdx.x, tid = threadIdx.x;
+  const int row = blockIdx.x;
   const SamplerParams p = *pp;
-  const int L = *step_idx;                          // tokens generated so far = rows of the history
+  const int L = *step_idx + (LOOKUP ? row : 0);     // tokens generated so far = rows of the history
   const float NEG_INF = -INFINITY;
 
-  for (int v = tid; v < V; v += kSampThreads) s_row[v] = logits[(size_t)b * ld + v];
+  for (int v = tid; v < V; v += kSampThreads) s_row[v] = logits[(size_t)row * ld + v];
   for (int i = tid; i < vpad / 32; i += kSampThreads) s_seen[i] = 0u;
   if (tid == 0) { s_n = 0; s_choice = 0; s_keep = 0; s_thr = 0xFFFFFFFFu; }
   __syncthreads();
 
-  history_processors<kSampThreads>(s_row, s_seen, V, history, B, b, L, p.rep_penalty, p.no_repeat_ngram, p.n_eos, p.eos, p.min_new_tokens);
+  history_processors<kSampThreads>(s_row, s_seen, V, history, LOOKUP ? 1 : B, b, L, p.rep_penalty, p.no_repeat_ngram, p.n_eos, p.eos, p.min_new_tokens);
 
   int chosen = 0;
   if (!p.do_sample) {
@@ -88,7 +93,7 @@ dec_sample_kernel(const float* __restrict__ logits, int ld, int V, int B, const 
       if (tid == 0) s_choice = (bi == 0x7fffffff) ? 0 : bi;
     }
     __syncthreads();
-    if (scores_out) for (int v = tid; v < V; v += kSampThreads) scores_out[(size_t)b * V + v] = s_row[v];
+    if (scores_out) for (int v = tid; v < V; v += kSampThreads) scores_out[(size_t)row * V + v] = s_row[v];
     chosen = s_choice;
   } else {
     // ---- temperature
@@ -137,11 +142,15 @@ dec_sample_kernel(const float* __restrict__ logits, int ld, int V, int B, const 
     }
     __syncthreads();
     if (scores_out) {
-      for (int v = tid; v < V; v += kSampThreads) scores_out[(size_t)b * V + v] = NEG_INF;
+      for (int v = tid; v < V; v += kSampThreads) scores_out[(size_t)row * V + v] = NEG_INF;
       __syncthreads();
-      if (tid < s_keep) scores_out[(size_t)b * V + s_sidx[tid]] = s_sval[tid];
+      if (tid < s_keep) scores_out[(size_t)row * V + s_sidx[tid]] = s_sval[tid];
     }
     chosen = s_choice;
+  }
+  if (LOOKUP) {
+    if (tid == 0) tok[row] = chosen;
+    return;
   }
   if (tid == 0) {
     int t = chosen;
@@ -172,7 +181,21 @@ int dec_sample(const float* logits, int ld, int V, int B, const int32_t* history
   int na = 0;
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = attr; cfg.numAttrs = na;
-  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, dec_sample_kernel, logits, ld, V, B, history, step_idx, params_dev, tok, history_out, dp_send, finished, scores_out));
+  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, dec_sample_kernel<false>, logits, ld, V, B, history, step_idx, params_dev, tok, history_out, dp_send, finished, scores_out));
+  return 0;
+}
+
+int dec_sample_lookup(const float* logits, int ld, int V, int R, const int32_t* history, const int32_t* step_idx, const SamplerParams* params_dev,
+                      int32_t* tok, cudaStream_t st) {
+  if (!sampler_supported(V)) { set_error("device sampler: vocabulary %d does not fit one CTA's shared memory", V); return -1; }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(R); cfg.blockDim = dim3(kSampThreads); cfg.dynamicSmemBytes = sampler_smem_bytes(V); cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  int na = 0;
+  if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
+  cfg.attrs = attr; cfg.numAttrs = na;
+  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, dec_sample_kernel<true>, logits, ld, V, 1, history, step_idx, params_dev, tok, (int32_t*)nullptr,
+                                  (int32_t*)nullptr, (int32_t*)nullptr, (float*)nullptr));
   return 0;
 }
 
@@ -181,7 +204,8 @@ int sampler_init() {
   static bool done = false;
   if (done) return 0;
   done = true;
-  VCLA_CUDA_OK(cudaFuncSetAttribute(dec_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024 - 1024)));
+  VCLA_CUDA_OK(cudaFuncSetAttribute(dec_sample_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024 - 1024)));
+  VCLA_CUDA_OK(cudaFuncSetAttribute(dec_sample_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024 - 1024)));
   return 0;
 }
 

@@ -35,6 +35,10 @@ class VclaBeam(C.Structure):
                 ("min_new_tokens", C.c_int)]
 
 
+class VclaLookup(C.Structure):
+    _fields_ = [("k", C.c_int), ("n", C.c_int), ("max_new", C.c_int), ("prompt_ids", C.c_void_p), ("prompt_len", C.c_int)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -72,6 +76,9 @@ _SIGNATURES = [
     ("vcla_set_sampler", C.c_int, [_P, C.POINTER(VclaSampler), _P]),
     ("vcla_read_finished", C.c_int, [_P, _P, C.c_int, _P]),
     ("vcla_op_sample", C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, C.POINTER(VclaSampler), _P, _P, _P]),
+    # prompt lookup decoding (HF:generation/candidate_generator.py PromptLookupCandidateGenerator, HF:generation/utils.py _assisted_decoding)
+    ("vcla_set_lookup", C.c_int, [_P, C.POINTER(VclaLookup), _P]),
+    ("vcla_read_lookup_stats", C.c_int, [_P, _P, _P]),
     ("vcla_set_beam", C.c_int, [_P, C.POINTER(VclaBeam)]),
     ("vcla_read_beams", C.c_int, [_P, _P, _P, _P, _P]),
     ("vcla_beam_cow_bytes", C.c_int, [_P, C.POINTER(C.c_int64), C.c_int]),
@@ -103,6 +110,8 @@ _SIGNATURES = [
                                           C.c_float, _P]),
     ("vcla_op_attention_decode", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float,
                                            C.c_float, C.c_int, C.c_int, C.c_int, _P]),
+    ("vcla_op_attention_decode_lookup", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float,
+                                                  C.c_float, _P]),
     ("vcla_op_logits_argmax", C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     ("vcla_op_layernorm", C.c_int, [_P, C.c_int, C.c_int, _P, _P, C.c_float, _P, _P, _P]),
     ("vcla_op_rmsnorm", C.c_int, [_P, C.c_int, C.c_int, _P, C.c_float, _P, _P]),

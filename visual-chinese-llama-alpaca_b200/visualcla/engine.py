@@ -299,6 +299,30 @@ class Engine:
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_set_sampler(self._ctx, C.byref(spec) if spec is not None else None, self._stream()), "vcla_set_sampler")
 
+    def set_lookup(self, prompt_ids: Optional[torch.Tensor], k: int = 0, n: int = 2, max_new: int = 0):
+        """Prompt lookup decoding of the one resident sequence (include/vcla.h): decode_many then runs verification steps of up to k
+        drafts copied from prompt_ids ++ the emitted tokens (n-grams of up to n tokens).  None: plain decode steps."""
+        with torch.cuda.device(self.device):
+            if prompt_ids is None:
+                N.check(self.lib.vcla_set_lookup(self._ctx, None, self._stream()), "vcla_set_lookup")
+                return
+            ids = prompt_ids.reshape(-1).to(self.device, torch.int64).contiguous()
+            spec = N.VclaLookup(k=int(k), n=int(n), max_new=int(max_new), prompt_ids=ids.data_ptr(), prompt_len=ids.numel())
+            N.check(self.lib.vcla_set_lookup(self._ctx, C.byref(spec), self._stream()), "vcla_set_lookup")
+
+    def lookup_stats(self) -> Tuple[int, bool, int, int, int, int]:
+        """-> (history rows, finished, verification steps that emitted, drafts offered, drafts emitted, rows per step).  Synchronises."""
+        out = (C.c_int64 * 6)()
+        with torch.cuda.device(self.device):
+            N.check(self.lib.vcla_read_lookup_stats(self._ctx, out, self._stream()), "vcla_read_lookup_stats")
+        return int(out[0]), bool(out[1]), int(out[2]), int(out[3]), int(out[4]), int(out[5])
+
+    def record_event(self):
+        """A CUDA event recorded on this engine's stream after the work enqueued so far (.query() is True once it has run)."""
+        e = torch.cuda.Event()
+        e.record(torch.cuda.current_stream(self.device))
+        return e
+
     def read_finished(self, B: int) -> torch.Tensor:
         out = torch.empty(B, dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
@@ -468,7 +492,8 @@ class Engine:
         shapes = {"vit_out": (B, (c["v_image"] // c["v_patch"]) ** 2 + 1, c["v_hidden"]),
                   "post_ln": (B, (c["v_image"] // c["v_patch"]) ** 2 + 1, c["v_hidden"]),
                   "resampler_out": (B, c["r_queries"], c["r_hidden"]),
-                  "projector_out": (B, c["r_queries"], c["t_hidden"])}
+                  "projector_out": (B, c["r_queries"], c["t_hidden"]),
+                  "step_logits": (B, c["t_vocab"]), "lookup_tokens": (B,)}
         out = torch.empty(shapes[stage], dtype=torch.float32)
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_read_stage(self._ctx, stage.encode(), B, N.ptr(out), self._stream()), f"vcla_read_stage({stage})")

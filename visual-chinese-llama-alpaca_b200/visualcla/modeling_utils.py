@@ -259,6 +259,12 @@ def chat_in_stream(model, image, text: str, history=[], generation_config=None):
     with Iteratorize(run) as stream:
         for ids in stream:
             if len(ids) and int(ids[-1]) == eos_token_id:
+                # prompt lookup decoding publishes several tokens per step: the ones before the EOS are still part of the reply
+                if len(ids) > 1 and model.tokenizer.decode(ids[:-1], skip_special_tokens=True) != response:
+                    response = model.tokenizer.decode(ids[:-1], skip_special_tokens=True)
+                    hist = deepcopy(base_history)
+                    hist.append({"type": "response", "value": response})
+                    yield response, hist
                 break
             response = model.tokenizer.decode(ids, skip_special_tokens=True)
             hist = deepcopy(base_history)

@@ -508,14 +508,23 @@ class VisualCLAModel:
             pure_greedy = not need_logits and not eos
             spec = None if pure_greedy else self._device_sampler_spec(gc, eos, pad, min_new, logits_processor, [], processors)
             if pure_greedy or spec is not None:
+                k = self._lookup_tokens(gc, B, S, max_new)
+                if k:
+                    n = int(getattr(gc, "max_matching_ngram_size", None) or 2)
+                    return self._generate_lookup_streamed(spec, start, finish, max_new, eos, tok, input_ids[0], k, n, streamer, crit)
                 return self._generate_streamed(spec, start, finish, B, max_new, eos, tok, streamer, crit)
         spec = None if streaming else self._device_sampler_spec(gc, eos, pad, min_new, logits_processor, crit, processors)
+        pure_greedy = not need_logits and not eos and not crit and streamer is None
+        k = self._lookup_tokens(gc, B, S, max_new) if (spec is not None or pure_greedy) and not streaming else 0
+        if k:
+            n = int(getattr(gc, "max_matching_ngram_size", None) or 2)
+            return self._generate_lookup(spec, start, finish, max_new, eos, tok, input_ids[0], k, n)
         if spec is not None:
             return self._generate_on_device(spec, start, finish, B, max_new, eos, tok)
         if streamer is not None:
             streamer.put(torch.empty(B, 0, dtype=torch.int64))    # HF generate: put(input_ids) first -- none with inputs_embeds
         last, first_tok = start(need_logits)
-        if not need_logits and not eos and not crit and streamer is None:
+        if pure_greedy:
             # pure greedy, fixed length: graph replays only; tokens come from the device-side history the graph appends to
             tok.copy_(first_tok)
             eng.decode_many(tok, max_new - 1)
@@ -721,14 +730,121 @@ class VisualCLAModel:
             result = eng.read_history(B, n_done).t().to(torch.int64)
         finally:
             eng.set_sampler(None)
-        fed = result[:, : n_done - 1]
-        if eos:
-            hit = torch.zeros_like(result, dtype=torch.bool)
-            for e in eos:
-                hit |= result == e
-            first = torch.where(hit.any(1), hit.float().argmax(1) + 1, torch.full((B,), n_done, device=result.device))
-            result = result[:, : int(first.max())]        # cut where the last sequence finished (HF's per-step check)
-        return finish(result, fed)
+        return finish(self._cut_at_eos(result, eos), result[:, : n_done - 1])
+
+    @staticmethod
+    def _cut_at_eos(result, eos):
+        """history rows -> the returned rows: cut where the last sequence finished (HF's per-step check); the device sampler already
+        pads a finished row"""
+        if not eos:
+            return result
+        hit = torch.zeros_like(result, dtype=torch.bool)
+        for e in eos:
+            hit |= result == e
+        first = torch.where(hit.any(1), hit.float().argmax(1) + 1, torch.full((result.shape[0],), result.shape[1], device=result.device))
+        return result[:, : int(first.max())]
+
+    # ---- prompt lookup decoding (HF GenerationConfig.prompt_lookup_num_tokens): verification steps inside the decode graphs ----------
+    LOOKUP_MAX_TOKENS = 15   # k + 1 rows fill at most the 16-column batch tile of the decode GEMMs
+    LOOKUP_CHUNK = 8         # verification steps per graph replay
+
+    LOOKUP_STREAM_CHUNK = 4  # verification steps per graph replay while streaming (two in flight: at most 8 run past a stop)
+
+    def _lookup_tokens(self, gc, B, S, max_new) -> int:
+        """-> drafted tokens per verification step of a call that runs on the device (argmax graphs, device sampler, or either of them
+        streamed), or 0 when it ignores prompt_lookup_num_tokens and runs as without it: batches above one (HF refuses assisted
+        generation there), VCLA_HOST_SAMPLER=1, and calls whose prompt + max_new_tokens + k exceed the context capacity.  Calls on the
+        host path, beam search and generate_dp never ask."""
+        k = int(getattr(gc, "prompt_lookup_num_tokens", None) or 0)
+        if k < 1 or B != 1 or max_new < 2 or os.environ.get("VCLA_HOST_SAMPLER") == "1":
+            return 0
+        k = min(k, self.LOOKUP_MAX_TOKENS)              # speed only: the tokens are those of one-token decoding
+        if S + max_new + k > self._engine.max_seq:
+            return 0
+        return k
+
+    def _generate_lookup(self, spec, start, finish, max_new, eos, tok, prompt_ids, k, n):
+        """generate() of one prompt by prompt lookup decoding on the device (spec: the device sampler, None: argmax): graphs of
+        LOOKUP_CHUNK verification steps, one host poll of the emitted count and the finished flag between them.  Each step emits the
+        tokens one-token decoding would emit there, so the result, the EOS cut and the cache handle are those of the call without it."""
+        eng = self._engine
+        if spec is not None:
+            eng.set_sampler(spec)
+        try:
+            _, first_tok = start(False)
+            tok.copy_(first_tok)
+            eng.set_lookup(prompt_ids, k, n, max_new)
+            try:
+                while True:
+                    n_done, fin = eng.lookup_stats()[:2]
+                    if n_done >= max_new or fin:
+                        break
+                    eng.decode_many(tok, self.LOOKUP_CHUNK)
+            finally:
+                eng.set_lookup(None)
+            result = eng.read_history(1, n_done).t().to(torch.int64)
+        finally:
+            if spec is not None:
+                eng.set_sampler(None)
+        # steps after the end emit nothing: every history row was fed except the last
+        return finish(self._cut_at_eos(result, eos), result[:, : n_done - 1])
+
+    def _generate_lookup_streamed(self, spec, start, finish, max_new, eos, tok, prompt_ids, k, n, streamer, crit):
+        """_generate_lookup with a streamer and / or Stream criteria: the verification steps run armed, so the tokens each step emits
+        reach the host through the ring.  Every wait that returns new tokens makes ONE streamer.put of them as a (1, n) int64 tensor
+        (HF _assisted_decoding's streamer.put(valid_tokens.cpu())), then runs the criteria once.  Graphs of LOOKUP_STREAM_CHUNK steps are
+        kept two deep: while the older one has not finished the newer one has not started, so a wait for one more token always has a
+        step that will emit it until every row is final.  Launching stops at an EOS, at max_new_tokens or when a criterion returns True;
+        the steps still running then (at most 2 x LOOKUP_STREAM_CHUNK) are drained and dropped."""
+        eng = self._engine
+        if streamer is not None:
+            streamer.put(torch.empty(1, 0, dtype=torch.int64))    # HF generate: put(input_ids) first -- none with inputs_embeds
+        rows = torch.empty(1, max_new, dtype=torch.int64)
+        eos_t = torch.tensor(eos, dtype=torch.int64) if eos else None
+        n_kept = 0
+        pending = []
+        if spec is not None:
+            eng.set_sampler(spec)
+        try:
+            eng.stream_arm(True)
+            try:
+                _, first_tok = start(False)
+                tok.copy_(first_tok)
+                eng.set_lookup(prompt_ids, k, n, max_new)
+                done = False
+                while not done:
+                    pending = [e for e in pending if not e.query()]
+                    while len(pending) < 2:
+                        eng.decode_many(tok, self.LOOKUP_STREAM_CHUNK)
+                        pending.append(eng.record_event())
+                    seen = min(eng.stream_wait(n_kept + 1), max_new)
+                    new = eng.stream_read(n_kept, seen, 1).to(torch.int64).t()      # (1, n)
+                    if eos:
+                        hit = torch.isin(new[0], eos_t)
+                        if bool(hit.any()):                       # the device stops at the EOS; nothing follows it
+                            done = True
+                    rows[:, n_kept:seen] = new
+                    n_kept = seen
+                    done = done or n_kept >= max_new
+                    if streamer is not None:
+                        streamer.put(new.clone())
+                    for cfn in crit:
+                        r = cfn(rows[:, :n_kept], None)
+                        if isinstance(r, torch.Tensor):
+                            r = bool(r.all())
+                        done = done or bool(r)
+            finally:
+                for e in pending:
+                    e.synchronize()                                           # drain what is still running before disarming
+                eng.stream_arm(False)
+                eng.set_lookup(None)
+        finally:
+            if spec is not None:
+                eng.set_sampler(None)
+        if streamer is not None:
+            streamer.end()
+        result = rows[:, :n_kept].to(eng.device)
+        return finish(result, rows[:, : n_kept - 1])
 
     # ---- beam search: the beam kernels and copy-on-write KV pages inside the decode graphs -------------------------------------
     def _generate_beams(self, gc, input_ids, pixel_values, attention_mask, logits_processor, stopping_criteria, streamer):
