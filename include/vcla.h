@@ -187,7 +187,17 @@ int vcla_read_history(vcla_ctx* ctx, int32_t* dst_dev, int B, int n_steps, vcla_
  * device token history (with inputs_embeds HF's processors only see the new tokens), inside the captured CUDA graph: no logits
  * leave the device, no host work per token.  do_sample = 0 takes the argmax of the processed scores (greedy + penalties).
  * A sequence that emitted an EOS id keeps producing pad_token_id (sticky per-sequence flag, vcla_read_finished).
- * The parameters live in device memory: changing them does not re-capture graphs. */
+ * The parameters live in device memory: changing them does not re-capture graphs.
+ * The draw (do_sample = 1), for sequence b after L generated tokens (L = 0 at the prefill's pick):
+ *   x0   = word 0 of Philox4x32-10 (Random123) with counter words (L, b, 0, 0) and key words (seed & 0xffffffff, seed >> 32)
+ *   u    = (x0 >> 8) * 2^-24, a 24-bit uniform in [0, 1)
+ *   the candidates -- the top-k set, every tie at the k-th value included -- sorted by (score descending, token id ascending); top-p
+ *   keeps ranks 0 .. keep-1 (rank r >= 1 goes when the fp32 sum of the probabilities of ranks r .. last is <= 1 - top_p)
+ *   e_r  = expf(s_r - s_0), tot = e_0 + ... + e_{keep-1} (fp32, in rank order)
+ *   pick = the first rank r with e_0 + ... + e_r > u * tot, else rank keep-1
+ * Prompt lookup verification (vcla_lookup) draws row r of a step that starts at L generated tokens with counter (L + r, 0): the draw
+ * one-token decoding makes at that length.  The candidate buffer holds 1024 entries: a row with more than 1024 tokens tied at the
+ * k-th value draws among 1024 of them, which ones and in which order undefined. */
 typedef struct {
   int do_sample;
   float repetition_penalty;     /* 1 = off */
@@ -199,7 +209,7 @@ typedef struct {
   int n_eos;                    /* <= 4 */
   int eos_token_id[4];
   int pad_token_id;
-  uint64_t seed;                /* draw = Philox4x32-10(key = seed, counter = (step, sequence)) */
+  uint64_t seed;                /* the Philox key: the draw above */
 } vcla_sampler;
 int vcla_sampler_supported(const vcla_ctx* ctx);   /* 1 when the vocabulary row fits one CTA's shared memory */
 int vcla_set_sampler(vcla_ctx* ctx, const vcla_sampler* sampler_or_null, vcla_stream stream);   /* NULL: back to greedy argmax */
