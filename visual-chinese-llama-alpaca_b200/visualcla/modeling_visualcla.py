@@ -10,13 +10,14 @@ hand-written sm_90a kernels behind the C ABI in include/vcla.h (see engine.py / 
 """
 from __future__ import annotations
 
+import contextlib
 import copy
 import glob
 import json
 import os
 import weakref
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Union
+from typing import Dict, List, NamedTuple, Optional, Tuple, Union
 
 import torch
 
@@ -96,6 +97,13 @@ class VclaKVCache:
 
     def __len__(self):
         return 0 if self.ids is None else int(self.ids.numel())
+
+
+class _DevicePlan(NamedTuple):
+    """how a generate() call runs on the decode graphs (VisualCLAModel._device_plan)"""
+    spec: Optional["N.VclaSampler"]     # the device sampler, or None: the argmax graphs
+    lookup: Optional[Tuple[int, int]]   # prompt lookup decoding's (k, n), or None
+    streamed: bool                      # tokens reach a streamer / Stream criteria through the ring as they are chosen
 
 
 class VisualCLAModel:
@@ -498,38 +506,20 @@ class VisualCLAModel:
                 self._tok_buf[key] = (torch.zeros(B, dtype=torch.int32, device=dev),
                                       torch.empty(B, eng.vocab, dtype=torch.float32, device=dev) if need_logits else None)
         tok, logits = self._tok_buf[key]
+
+        plan = self._device_plan(gc, B, S, max_new, eos, pad, min_new, need_logits, logits_processor, processors, crit, streamer)
+        if plan is not None:
+            lookup = (input_ids[0], *plan.lookup, max_new) if plan.lookup else None
+            if plan.streamed:
+                return self._generate_streamed(plan.spec, lookup, start, finish, B, max_new, eos, tok, streamer, crit)
+            return self._generate_graphs(plan.spec, lookup, start, finish, B, max_new, eos, tok)
+
+        # the per-step host loop: HF logits processors / sampling / criteria on the logits of every step
         out = torch.full((B, max_new), pad, dtype=torch.int64, device=dev)
         all_logits: List[torch.Tensor] = []
-
-        streaming = streamer is not None or self._stream_criteria_only(crit)
-        if streaming and (not crit or self._stream_criteria_only(crit)) and os.environ.get("VCLA_HOST_SAMPLER") != "1" and getattr(eng, "stream_supported", lambda: False)():
-            # streamed on the device when the call would run there without its Stream criteria: the sampler graphs, or the
-            # pure-greedy argmax graphs (spec None); each step's tokens reach the host through the pinned ring as they are chosen
-            pure_greedy = not need_logits and not eos
-            spec = None if pure_greedy else self._device_sampler_spec(gc, eos, pad, min_new, logits_processor, [], processors)
-            if pure_greedy or spec is not None:
-                k = self._lookup_tokens(gc, B, S, max_new)
-                if k:
-                    n = int(getattr(gc, "max_matching_ngram_size", None) or 2)
-                    return self._generate_lookup_streamed(spec, start, finish, max_new, eos, tok, input_ids[0], k, n, streamer, crit)
-                return self._generate_streamed(spec, start, finish, B, max_new, eos, tok, streamer, crit)
-        spec = None if streaming else self._device_sampler_spec(gc, eos, pad, min_new, logits_processor, crit, processors)
-        pure_greedy = not need_logits and not eos and not crit and streamer is None
-        k = self._lookup_tokens(gc, B, S, max_new) if (spec is not None or pure_greedy) and not streaming else 0
-        if k:
-            n = int(getattr(gc, "max_matching_ngram_size", None) or 2)
-            return self._generate_lookup(spec, start, finish, max_new, eos, tok, input_ids[0], k, n)
-        if spec is not None:
-            return self._generate_on_device(spec, start, finish, B, max_new, eos, tok)
         if streamer is not None:
             streamer.put(torch.empty(B, 0, dtype=torch.int64))    # HF generate: put(input_ids) first -- none with inputs_embeds
         last, first_tok = start(need_logits)
-        if pure_greedy:
-            # pure greedy, fixed length: graph replays only; tokens come from the device-side history the graph appends to
-            tok.copy_(first_tok)
-            eng.decode_many(tok, max_new - 1)
-            result = eng.read_history(B, max_new).t().to(torch.int64)
-            return finish(result, result[:, : max_new - 1])
         finished = torch.zeros(B, dtype=torch.bool, device=dev)
         n_done = 0
         for step in range(max_new):
@@ -576,104 +566,175 @@ class VisualCLAModel:
                 # step, so with one the loop stops where HF does.
                 if (step & 7) == 7 or step == max_new - 1 or streamer is not None:
                     stop = bool(finished.all())
-            for cfn in crit:
-                r = cfn(out[:, :n_done], cur_logits if need_logits else None)
-                if isinstance(r, torch.Tensor):
-                    r = bool(r.all())
-                stop = stop or bool(r)
-            if stop:
+            if self._criteria_stop(crit, out[:, :n_done], cur_logits if need_logits else None) or stop:
                 break
-        result = out[:, :n_done]
-        fed = out[:, : n_done - 1]
-        if eos:
-            # cut at the step where the last sequence finished (what HF's per-step check would have produced)
-            hit = torch.zeros(B, n_done, dtype=torch.bool, device=dev)
-            for e in eos:
-                hit |= result == e
-            first = torch.where(hit.any(1), hit.float().argmax(1) + 1, torch.full((B,), n_done, device=dev))
-            keep = int(first.max())
-            result = result[:, :keep]
-            idx = torch.arange(keep, device=dev)[None, :]
-            result = torch.where(idx < first[:, None], result, torch.full_like(result, pad))
         if streamer is not None:
             streamer.end()
-        return finish(result, fed, tuple(all_logits) if all_logits else None)
+        # a finished row already holds pad after its EOS
+        return finish(self._cut_at_eos(out[:, :n_done], eos), out[:, : n_done - 1], tuple(all_logits) if all_logits else None)
+
+    def _device_plan(self, gc, B, S, max_new, eos, pad, min_new, need_logits, logits_processor, processors, crit, streamer):
+        """-> how this call runs on the decode graphs, or None: the per-step host loop.  Plain greedy without EOS runs the argmax
+        graphs; anything else needs a device sampler spec (_device_sampler_spec draws its seed).  A call with a streamer or only Stream
+        criteria streams on the device when the engine has the token ring and the call would run there without its Stream criteria;
+        any other criterion, or VCLA_HOST_SAMPLER=1, keeps it on the host loop (VCLA_HOST_SAMPLER=1 leaves a non-streamed plain greedy
+        call on the argmax graphs)."""
+        from .modeling_utils import Stream
+        stream_only = all(isinstance(c, Stream) for c in crit)
+        streamed = streamer is not None or (len(crit) > 0 and stream_only)
+        if streamed and (not stream_only or os.environ.get("VCLA_HOST_SAMPLER") == "1"
+                         or not getattr(self._engine, "stream_supported", lambda: False)()):
+            return None
+        greedy = not need_logits and not eos and (streamed or not crit)
+        spec = None
+        if not (streamed and greedy):
+            spec = self._device_sampler_spec(gc, eos, pad, min_new, logits_processor, [] if streamed else crit, processors)
+            if spec is None and not greedy:
+                return None
+        k = self._lookup_tokens(gc, B, S, max_new)
+        return _DevicePlan(spec, (k, int(getattr(gc, "max_matching_ngram_size", None) or 2)) if k else None, streamed)
+
+    @staticmethod
+    def _criteria_stop(crit, ids, scores) -> bool:
+        """HF's stopping criteria on the tokens so far: every criterion runs; one returning a tensor stops only when all of it is True"""
+        stop = False
+        for cfn in crit:
+            r = cfn(ids, scores)
+            if isinstance(r, torch.Tensor):
+                r = bool(r.all())
+            stop = stop or bool(r)
+        return stop
+
+    # ---- the decode graphs: argmax, the device sampler, prompt lookup, each optionally streamed ------------------------------------
+    @contextlib.contextmanager
+    def _sampler_mode(self, spec):
+        """the device sampler (spec) for the prefill and decode steps inside, or the argmax graphs (None); always set before start()
+        (the prefill picks the first token) and switched off last"""
+        if spec is not None:
+            self._engine.set_sampler(spec)
+        try:
+            yield
+        finally:
+            if spec is not None:
+                self._engine.set_sampler(None)
+
+    @contextlib.contextmanager
+    def _decode_modes(self, start, tok, lookup=None, drain=None):
+        """start() the call and put its first pick in tok.  drain given: the token ring is armed before the prefill, and on the way out
+        drain() waits for the armed work still running before it is disarmed.  lookup = (prompt_ids, k, n, max_new) given: prompt
+        lookup is set after the prefill (vcla_set_lookup refuses while an earlier call left more than one sequence resident) and unset
+        after the ring is disarmed."""
+        eng = self._engine
+        if drain is not None:
+            eng.stream_arm(True)
+        try:
+            _, first_tok = start(False)
+            tok.copy_(first_tok)
+            if lookup is not None:
+                eng.set_lookup(*lookup)
+            yield
+        finally:
+            if drain is not None:
+                drain()
+                eng.stream_arm(False)
+            if lookup is not None:
+                eng.set_lookup(None)
+
+    def _decode_polled(self, tok, max_new, all_done):
+        """graphs of 8 decode steps, one host poll of the per-row done flags (all_done()) between them, until every row is done or
+        max_new tokens exist -> tokens decoded.  Rows are independent and a done row's tokens no longer change, so the steps run past
+        the last one cannot change a retained token."""
+        n_done = 1
+        while n_done < max_new and not bool(all_done().bool().all()):
+            k = min(8, max_new - n_done)
+            self._engine.decode_many(tok, k)
+            n_done += k
+        return n_done
+
+    def _generate_graphs(self, spec, lookup, start, finish, B, max_new, eos, tok):
+        """generate() on the decode graphs with no host work per step.  Nothing can stop early: every step in one replay.  EOS: graphs of
+        8 steps with a poll of the finished flags between them (a finished row only emits pad).  Prompt lookup: graphs of LOOKUP_CHUNK
+        verification steps with a poll of the emitted count and the finished flag between them; each step emits the tokens one-token
+        decoding would emit there, so the result, the EOS cut and the cache handle are those of the call without it."""
+        eng = self._engine
+        with self._sampler_mode(spec):
+            with self._decode_modes(start, tok, lookup):
+                if lookup is not None:
+                    while True:
+                        n_done, fin = eng.lookup_stats()[:2]
+                        if n_done >= max_new or fin:
+                            break
+                        eng.decode_many(tok, self.LOOKUP_CHUNK)
+                elif eos:
+                    n_done = self._decode_polled(tok, max_new, lambda: eng.read_finished(B))
+                else:
+                    eng.decode_many(tok, max_new - 1)
+                    n_done = max_new
+            result = eng.read_history(B, n_done).t().to(torch.int64)
+        # every history row was fed to a decode step except the last
+        return finish(self._cut_at_eos(result, eos), result[:, : n_done - 1])
 
     # ---- streaming on the device: decode graphs publish every step into a pinned host ring (include/vcla.h, token streaming) ----
     STREAM_CHUNK = 8      # decode steps per graph replay while streaming
 
-    @staticmethod
-    def _stream_criteria_only(crit) -> bool:
-        from .modeling_utils import Stream
-        return len(crit) > 0 and all(isinstance(c, Stream) for c in crit)
-
-    def _generate_streamed(self, spec, start, finish, B, max_new, eos, tok, streamer, crit):
-        """generate() with a streamer and / or Stream criteria, on the device.  The prefill and graphs of up to STREAM_CHUNK decode steps
-        run as without streaming (spec: the device sampler, None: the argmax graphs) while armed, so each step's tokens are published
-        to the host as soon as they are chosen.  The next graph is enqueued once the second-to-last step of the running one is
-        published, so the device never waits for the host.  Every published step goes, in order, to streamer.put and then to the
-        criteria (HF _sample's order).  Launching stops when every row has emitted an EOS id, at max_new_tokens, or when a criterion
-        returns True; the steps still running then (at most STREAM_CHUNK + 1) are drained and dropped."""
-        eng = self._engine
+    def _generate_streamed(self, spec, lookup, start, finish, B, max_new, eos, tok, streamer, crit):
+        """generate() with a streamer and / or Stream criteria, on the device: the graphs of _generate_graphs run armed, so the tokens
+        reach the host through the ring as they are chosen.  HF's protocol: put an empty (B, 0) tensor first, then each batch of new
+        tokens (int64, on the CPU) to streamer.put and then to the criteria, and end() last.  Launching stops at EOS, at max_new_tokens
+        or when a criterion returns True; the steps still running then are drained and dropped."""
         if streamer is not None:
             streamer.put(torch.empty(B, 0, dtype=torch.int64))    # HF generate: put(input_ids) first -- none with inputs_embeds
-        rows = torch.empty(B, max_new, dtype=torch.int64)         # host copy of the published steps
-        eos_t = torch.tensor(eos, dtype=torch.int64) if eos else None
-        n_launched, n_kept = 0, 0
-        if spec is not None:
-            eng.set_sampler(spec)
-        try:
-            eng.stream_arm(True)
-            try:
-                _, first_tok = start(False)
-                tok.copy_(first_tok)
-                n_launched = 1
+        rows = torch.empty(B, max_new, dtype=torch.int64)         # host copy of the published tokens
 
-                def launch():
-                    nonlocal n_launched
-                    k = min(self.STREAM_CHUNK, max_new - n_launched)
-                    eng.decode_many(tok, k)
-                    n_launched += k
+        def publish(new, n_kept):
+            """new tokens, already in rows[:, :n_kept] -> the streamer, then the criteria; True when a criterion stops the call"""
+            if streamer is not None:
+                streamer.put(new.clone())
+            return self._criteria_stop(crit, rows[:, :n_kept], None)
 
-                if max_new > 1:
-                    launch()
-                finished = torch.zeros(B, dtype=torch.bool)
-                s, done = 0, False
-                while not done:
-                    seen = min(eng.stream_wait(s + 1), n_launched)
-                    new = eng.stream_read(s, seen, B).to(torch.int64)
-                    for row in new:
-                        rows[:, s] = row
-                        if eos:
-                            finished |= torch.isin(row, eos_t)
-                        last = s + 1 == max_new or (bool(eos) and bool(finished.all()))
-                        if not last and s >= n_launched - 2 and n_launched < max_new:
-                            launch()                                          # before the callbacks: keep the device busy
-                        n_kept = s + 1
-                        if streamer is not None:
-                            streamer.put(row.clone())
-                        stop = False
-                        for cfn in crit:
-                            r = cfn(rows[:, :n_kept], None)
-                            if isinstance(r, torch.Tensor):
-                                r = bool(r.all())
-                            stop = stop or bool(r)
-                        s += 1
-                        if last or stop:
-                            done = True
-                            break
-            finally:
-                if n_launched:
-                    eng.stream_wait(n_launched)                               # drain what is still running before disarming
-                eng.stream_arm(False)
-        finally:
-            if spec is not None:
-                eng.set_sampler(None)
+        with self._sampler_mode(spec):
+            if lookup is None:
+                n_kept = self._stream_steps(start, tok, rows, max_new, eos, publish)
+            else:
+                n_kept = self._stream_lookup(start, tok, rows, max_new, eos, publish, lookup)
         if streamer is not None:
             streamer.end()
-        result = rows[:, :n_kept].to(eng.device)                     # the device sampler already pads a finished row
-        # the cache handle records the tokens fed up to the cut; steps run past it lie beyond its length
-        return finish(result, rows[:, : n_kept - 1])
+        # the device sampler already pads a finished row; the cache handle records the tokens fed up to the cut, and steps run past
+        # it lie beyond its length
+        return finish(rows[:, :n_kept].to(self._engine.device), rows[:, : n_kept - 1])
+
+    def _stream_steps(self, start, tok, rows, max_new, eos, publish):
+        """graphs of up to STREAM_CHUNK decode steps; the next one is enqueued once the second-to-last step of the running one is
+        published, so the device never waits for the host.  One publish per step (HF _sample), so at most STREAM_CHUNK + 1 steps run
+        past a stop.  -> tokens kept"""
+        eng = self._engine
+        B = rows.shape[0]
+        eos_t = torch.tensor(eos, dtype=torch.int64) if eos else None
+        finished = torch.zeros(B, dtype=torch.bool)
+        n_launched = n_kept = 0
+
+        def launch():
+            nonlocal n_launched
+            k = min(self.STREAM_CHUNK, max_new - n_launched)
+            eng.decode_many(tok, k)
+            n_launched += k
+
+        with self._decode_modes(start, tok, drain=lambda: n_launched and eng.stream_wait(n_launched)):
+            n_launched = 1
+            if max_new > 1:
+                launch()
+            while True:
+                seen = min(eng.stream_wait(n_kept + 1), n_launched)
+                for row in eng.stream_read(n_kept, seen, B).to(torch.int64):
+                    rows[:, n_kept] = row
+                    if eos:
+                        finished |= torch.isin(row, eos_t)
+                    last = n_kept + 1 == max_new or (bool(eos) and bool(finished.all()))
+                    if not last and n_kept >= n_launched - 2 and n_launched < max_new:
+                        launch()                                          # before the callbacks: keep the device busy
+                    n_kept += 1
+                    if publish(row, n_kept) or last:
+                        return n_kept
 
     # ---- sampling / EOS on the device: one fused kernel per step inside the decode graph ---------------------
     def _device_sampler_spec(self, gc, eos, pad, min_new, extra_processors, crit, processors):
@@ -708,30 +769,6 @@ class VisualCLAModel:
         return eng.sampler_spec(do_sample=sampling, repetition_penalty=rp, no_repeat_ngram_size=ng, temperature=temperature, top_k=top_k or 0,
                                 top_p=top_p, min_new_tokens=min_new, eos_token_id=eos, pad_token_id=pad, seed=seed)
 
-    def _generate_on_device(self, spec, start, finish, B, max_new, eos, tok):
-        eng = self._engine
-        eng.set_sampler(spec)
-        try:
-            _, first_tok = start(False)
-            tok.copy_(first_tok)
-            n_done = 1
-            if not eos:
-                eng.decode_many(tok, max_new - 1)
-                n_done = max_new
-            else:
-                # EOS: graphs of 8 steps, one host poll of the per-sequence finished flags between them (sequences are independent
-                # and a finished one only emits pad, so running a few steps past the last EOS cannot change a retained token)
-                while n_done < max_new:
-                    if bool(eng.read_finished(B).bool().all()):
-                        break
-                    k = min(8, max_new - n_done)
-                    eng.decode_many(tok, k)
-                    n_done += k
-            result = eng.read_history(B, n_done).t().to(torch.int64)
-        finally:
-            eng.set_sampler(None)
-        return finish(self._cut_at_eos(result, eos), result[:, : n_done - 1])
-
     @staticmethod
     def _cut_at_eos(result, eos):
         """history rows -> the returned rows: cut where the last sequence finished (HF's per-step check); the device sampler already
@@ -763,88 +800,29 @@ class VisualCLAModel:
             return 0
         return k
 
-    def _generate_lookup(self, spec, start, finish, max_new, eos, tok, prompt_ids, k, n):
-        """generate() of one prompt by prompt lookup decoding on the device (spec: the device sampler, None: argmax): graphs of
-        LOOKUP_CHUNK verification steps, one host poll of the emitted count and the finished flag between them.  Each step emits the
-        tokens one-token decoding would emit there, so the result, the EOS cut and the cache handle are those of the call without it."""
-        eng = self._engine
-        if spec is not None:
-            eng.set_sampler(spec)
-        try:
-            _, first_tok = start(False)
-            tok.copy_(first_tok)
-            eng.set_lookup(prompt_ids, k, n, max_new)
-            try:
-                while True:
-                    n_done, fin = eng.lookup_stats()[:2]
-                    if n_done >= max_new or fin:
-                        break
-                    eng.decode_many(tok, self.LOOKUP_CHUNK)
-            finally:
-                eng.set_lookup(None)
-            result = eng.read_history(1, n_done).t().to(torch.int64)
-        finally:
-            if spec is not None:
-                eng.set_sampler(None)
-        # steps after the end emit nothing: every history row was fed except the last
-        return finish(self._cut_at_eos(result, eos), result[:, : n_done - 1])
-
-    def _generate_lookup_streamed(self, spec, start, finish, max_new, eos, tok, prompt_ids, k, n, streamer, crit):
-        """_generate_lookup with a streamer and / or Stream criteria: the verification steps run armed, so the tokens each step emits
-        reach the host through the ring.  Every wait that returns new tokens makes ONE streamer.put of them as a (1, n) int64 tensor
-        (HF _assisted_decoding's streamer.put(valid_tokens.cpu())), then runs the criteria once.  Graphs of LOOKUP_STREAM_CHUNK steps are
+    def _stream_lookup(self, start, tok, rows, max_new, eos, publish, lookup):
+        """prompt lookup verification steps streamed: every wait that returns new tokens makes ONE publish of them as a (1, n) tensor
+        (HF _assisted_decoding's streamer.put(valid_tokens.cpu()), then the criteria once).  Graphs of LOOKUP_STREAM_CHUNK steps are
         kept two deep: while the older one has not finished the newer one has not started, so a wait for one more token always has a
-        step that will emit it until every row is final.  Launching stops at an EOS, at max_new_tokens or when a criterion returns True;
-        the steps still running then (at most 2 x LOOKUP_STREAM_CHUNK) are drained and dropped."""
+        step that will emit it until the row is final, and at most 2 x LOOKUP_STREAM_CHUNK steps run past a stop.  -> tokens kept"""
         eng = self._engine
-        if streamer is not None:
-            streamer.put(torch.empty(1, 0, dtype=torch.int64))    # HF generate: put(input_ids) first -- none with inputs_embeds
-        rows = torch.empty(1, max_new, dtype=torch.int64)
         eos_t = torch.tensor(eos, dtype=torch.int64) if eos else None
+        pending = []                                          # an event after each graph in flight
         n_kept = 0
-        pending = []
-        if spec is not None:
-            eng.set_sampler(spec)
-        try:
-            eng.stream_arm(True)
-            try:
-                _, first_tok = start(False)
-                tok.copy_(first_tok)
-                eng.set_lookup(prompt_ids, k, n, max_new)
-                done = False
-                while not done:
-                    pending = [e for e in pending if not e.query()]
-                    while len(pending) < 2:
-                        eng.decode_many(tok, self.LOOKUP_STREAM_CHUNK)
-                        pending.append(eng.record_event())
-                    seen = min(eng.stream_wait(n_kept + 1), max_new)
-                    new = eng.stream_read(n_kept, seen, 1).to(torch.int64).t()      # (1, n)
-                    if eos:
-                        hit = torch.isin(new[0], eos_t)
-                        if bool(hit.any()):                       # the device stops at the EOS; nothing follows it
-                            done = True
-                    rows[:, n_kept:seen] = new
-                    n_kept = seen
-                    done = done or n_kept >= max_new
-                    if streamer is not None:
-                        streamer.put(new.clone())
-                    for cfn in crit:
-                        r = cfn(rows[:, :n_kept], None)
-                        if isinstance(r, torch.Tensor):
-                            r = bool(r.all())
-                        done = done or bool(r)
-            finally:
-                for e in pending:
-                    e.synchronize()                                           # drain what is still running before disarming
-                eng.stream_arm(False)
-                eng.set_lookup(None)
-        finally:
-            if spec is not None:
-                eng.set_sampler(None)
-        if streamer is not None:
-            streamer.end()
-        result = rows[:, :n_kept].to(eng.device)
-        return finish(result, rows[:, : n_kept - 1])
+        with self._decode_modes(start, tok, lookup, drain=lambda: [e.synchronize() for e in pending]):
+            while True:
+                pending = [e for e in pending if not e.query()]
+                while len(pending) < 2:
+                    eng.decode_many(tok, self.LOOKUP_STREAM_CHUNK)
+                    pending.append(eng.record_event())
+                seen = min(eng.stream_wait(n_kept + 1), max_new)
+                new = eng.stream_read(n_kept, seen, 1).to(torch.int64).t()      # (1, n)
+                rows[:, n_kept:seen] = new
+                n_kept = seen
+                # the device stops at an EOS; nothing follows it
+                last = n_kept >= max_new or (bool(eos) and bool(torch.isin(new[0], eos_t).any()))
+                if publish(new, n_kept) or last:
+                    return n_kept
 
     # ---- beam search: the beam kernels and copy-on-write KV pages inside the decode graphs -------------------------------------
     def _generate_beams(self, gc, input_ids, pixel_values, attention_mask, logits_processor, stopping_criteria, streamer):
@@ -904,13 +882,7 @@ class VisualCLAModel:
                 _, first, _ = eng.prefill(ids, mode, rows, all_logits=False, last_logits=False, left_pad=pads, pos_from_mask=True)
                 tok = eng.token_buffer(n * K)
                 tok.copy_(first)
-                n_done = 1
-                while n_done < max_new:
-                    if bool(eng.read_beam_done(n).bool().all()):
-                        break
-                    k = min(8, max_new - n_done)
-                    eng.decode_many(tok, k)
-                    n_done += k
+                self._decode_polled(tok, max_new, lambda: eng.read_beam_done(n))
                 t, ln, _, _ = eng.read_beams(n)
             finally:
                 eng.set_beam(None)
