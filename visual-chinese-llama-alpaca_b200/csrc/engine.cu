@@ -13,9 +13,9 @@
 #include <algorithm>
 #include <chrono>
 #include <thread>
-#include <list>
 #include <map>
 #include <string>
+#include <tuple>
 #include <vector>
 
 using namespace vcla;
@@ -60,18 +60,11 @@ struct GraphKey {
   int B; const void* tok_in; const void* logits; const void* tok_out; int n_steps = 1; int dp = 0; int samp = 0; int beam = 0;
   int stream = 0;   // captured armed: every step publishes into the token stream ring
   int lookup = 0;   // prompt lookup: rows per verification step (0: plain decode steps)
-  bool operator<(const GraphKey& o) const {
-    if (lookup != o.lookup) return lookup < o.lookup;
-    if (B != o.B) return B < o.B;
-    if (tok_in != o.tok_in) return tok_in < o.tok_in;
-    if (logits != o.logits) return logits < o.logits;
-    if (n_steps != o.n_steps) return n_steps < o.n_steps;
-    if (dp != o.dp) return dp < o.dp;
-    if (samp != o.samp) return samp < o.samp;
-    if (beam != o.beam) return beam < o.beam;
-    if (stream != o.stream) return stream < o.stream;
-    return tok_out < o.tok_out;
-  }
+  auto fields() const { return std::tie(B, tok_in, logits, tok_out, n_steps, dp, samp, beam, stream, lookup); }
+  bool operator<(const GraphKey& o) const { return fields() < o.fields(); }
+};
+struct DecodeGraph {
+  cudaGraphExec_t exec; int64_t launches; uint64_t last_use;   // launches: kernels one replay enqueues (vcla_kernel_launches)
 };
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -159,9 +152,8 @@ struct vcla_ctx {
   int l2_prefetch_kb = 0;    // decode GEMMs: weight k-blocks per CTA prefetched into L2 during the dependency wait (VCLA_L2_PREFETCH_KB).
                              // Off by default: the prefetch traffic can delay the latency-critical consumer kernel in front of the GEMM.
   // graphs
-  std::map<GraphKey, cudaGraphExec_t> graphs;
-  std::map<GraphKey, int64_t> graph_launches;
-  std::list<GraphKey> graph_lru;          // most recently used first; bounded (kMaxGraphs) so a caller with ever-new buffers cannot grow it
+  std::map<GraphKey, DecodeGraph> graphs;   // bounded (kMaxGraphs) so a caller with ever-new buffers cannot grow it
+  uint64_t graph_uses = 0;                  // clock of DecodeGraph::last_use
   int64_t launches = 0;
   void* staging = nullptr; size_t staging_bytes = 0;
   void* trace_buf = nullptr; unsigned long long trace_cap = 0;
@@ -434,8 +426,8 @@ int count(vcla_ctx* c, int n = 1) { c->launches += n; return 0; }
 int drop_graphs(vcla_ctx* c) {
   if (c->graphs.empty()) return 0;
   const cudaError_t e = cudaDeviceSynchronize();   // a launch of one of them may still be in flight
-  for (auto& kv : c->graphs) cudaGraphExecDestroy(kv.second);
-  c->graphs.clear(); c->graph_launches.clear(); c->graph_lru.clear();
+  for (auto& kv : c->graphs) cudaGraphExecDestroy(kv.second.exec);
+  c->graphs.clear();
   if (e != cudaSuccess) { set_error("drop_graphs: device error %s", cudaGetErrorString(e)); return -1; }
   return 0;
 }
@@ -900,6 +892,9 @@ int vcla_vision_encode(vcla_ctx* c, const void* pixels, int pixel_dtype, int B, 
 // int8 projections (weight_format 1) run the cluster split-K schedule at every batch: its int8 kernel has a 64-column batch tile.
 static bool decode_uses_csk(const vcla_ctx* c, int B) { return B <= 32 || c->cfg.weight_format == 1; }
 static int csk_max_batch(const vcla_ctx* c) { return c->cfg.weight_format == 1 ? 64 : 32; }
+// The bf16 lm_head of a decode step runs on the cluster kernel up to 32 rows, beyond on the workspace GEMM (one stream of its weights
+// over all rows).  The prefill's last-row head always takes the workspace GEMM (lm_head_last).
+static bool lm_head_uses_csk(int B) { return B <= 32; }
 
 // The five weight-streaming GEMMs of a decode step (numbering of vcla_bench_decode_gemm's `which`).
 enum DecodeGemm { DG_QKV = 0, DG_O = 1, DG_GATE_UP = 2, DG_DOWN = 3, DG_LM_HEAD = 4 };
@@ -981,10 +976,20 @@ static int dp_wait(vcla_ctx* c, cudaStream_t st) {
   return 0;
 }
 
-// logits reduce + argmax (+ token exchange when data parallel)
-static int logits_argmax(vcla_ctx* c, int B, float* logits, int32_t* tok, int fork, cudaStream_t st, int lm_splits = 0) {
+// The token pick of one step from the lm_splits partials the lm_head left in ws_lm: beam search, the sampler or the argmax (+ the
+// token exchange when data parallel).  fork == 0: the prefill's pick (beam search's first step, the exchange inline).  lookup: the
+// picks of all B rows of a prompt lookup verification step into lk_pick, without history, step, finished-flag or exchange writes.
+static int pick(vcla_ctx* c, int B, int lm_splits, float* logits, int32_t* tok, int fork, bool lookup, cudaStream_t st) {
   const vcla_config& g = c->cfg;
-  const int sp_lm = lm_splits > 0 ? lm_splits : c->sp_lm;     // 1: ws_lm already holds the reduced logits (cluster split-K lm_head)
+  if (lookup) {
+    const int V = g.t_vocab;
+    count(c, 2);
+    if (c->samp_on) {
+      if (dec_logits_reduce(c->ws_lm, lm_splits, B, V, B, V, c->samp_logits, V, c->cand_val, c->cand_idx, st)) return -1;
+      return dec_sample_lookup(c->samp_logits, V, V, B, c->tok_hist, c->step_idx, c->samp_params, c->lk_pick, st);
+    }
+    return dec_logits_argmax(c->ws_lm, lm_splits, B, V, B, V, nullptr, V, c->lk_pick, nullptr, nullptr, c->cand_val, c->cand_idx, nullptr, st);
+  }
   if (c->dp_on() && dp_wait(c, st)) return -1;            // the previous step's exchange must have read dp_send before it is rewritten
   if (c->beam_on) {
     // B rows: the prompts at the prefill (fork == 0; every item's beams are still its prompt), else B / K items of K beams
@@ -992,7 +997,7 @@ static int logits_argmax(vcla_ctx* c, int B, float* logits, int32_t* tok, int fo
     const bool first = fork == 0;
     const int R = first ? 1 : c->beam_K, items = B / R;
     count(c, 3);
-    if (dec_logits_reduce(c->ws_lm, sp_lm, B, g.t_vocab, B, g.t_vocab, lg, g.t_vocab, c->cand_val, c->cand_idx, st)) return -1;
+    if (dec_logits_reduce(c->ws_lm, lm_splits, B, g.t_vocab, B, g.t_vocab, lg, g.t_vocab, c->cand_val, c->cand_idx, st)) return -1;
     if (dec_beam_step(lg, g.t_vocab, g.t_vocab, B, c->tok_hist, c->step_idx, c->beam_params, first ? nullptr : c->beam_run, c->beam_cand_val,
                       c->beam_cand_tok, st)) return -1;
     return dec_beam_select(c->beam_params, items, R, g.t_vocab, c->step_idx, c->beam_cand_val, c->beam_cand_tok, c->tok_hist, c->beam_run,
@@ -1002,14 +1007,14 @@ static int logits_argmax(vcla_ctx* c, int B, float* logits, int32_t* tok, int fo
     // logits -> [repetition penalty, no-repeat-ngram, temperature, top-k, top-p, draw] in one kernel; raw logits stay available
     float* lg = logits ? logits : c->samp_logits;
     count(c, 2);
-    if (dec_logits_reduce(c->ws_lm, sp_lm, B, g.t_vocab, B, g.t_vocab, lg, g.t_vocab, c->cand_val, c->cand_idx, st)) return -1;
+    if (dec_logits_reduce(c->ws_lm, lm_splits, B, g.t_vocab, B, g.t_vocab, lg, g.t_vocab, c->cand_val, c->cand_idx, st)) return -1;
     if (dec_sample(lg, g.t_vocab, g.t_vocab, B, c->tok_hist, c->step_idx, c->samp_params, tok, c->tok_hist, c->dp_on() ? c->dp_send : nullptr, c->finished,
                    nullptr, st)) return -1;
     if (c->dp_on()) return dp_gather(c, st, fork);
     return 0;
   }
   count(c, 2);
-  if (dec_logits_argmax(c->ws_lm, sp_lm, B, g.t_vocab, B, g.t_vocab, logits, g.t_vocab, tok, c->tok_hist, c->step_idx, c->cand_val, c->cand_idx,
+  if (dec_logits_argmax(c->ws_lm, lm_splits, B, g.t_vocab, B, g.t_vocab, logits, g.t_vocab, tok, c->tok_hist, c->step_idx, c->cand_val, c->cand_idx,
                         c->dp_on() ? c->dp_send : nullptr, st)) return -1;
   if (c->dp_on()) return dp_gather(c, st, fork);
   return 0;
@@ -1020,7 +1025,7 @@ static int lm_head_last(vcla_ctx* c, int B, float* logits_dev, int32_t* tok_dev,
   const vcla_config& g = c->cfg;
   count(c); if (dec_resid_norm(nullptr, 0, B, c->d_resid, B, g.t_hidden, c->final_norm, g.t_eps, c->d_xn, st)) return -1;
   if (ws_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
-  return logits_argmax(c, B, logits_dev, tok_dev ? tok_dev : c->d_tok, 0, st);
+  return pick(c, B, c->sp_lm, logits_dev, tok_dev ? tok_dev : c->d_tok, 0, false, st);
 }
 
 // The LLaMA stack over the B x S rows already embedded in c->resid.  base_len == nullptr: a whole prompt (causal attention over its
@@ -1186,40 +1191,9 @@ static int beam_reorder(vcla_ctx* c, int rows_old, int rows_new, const int32_t* 
   return kv_page_copy(c->kv_arena, c->kv_layer_elems, g.t_layers, g.t_heads, c->page_tokens, c->beam_copy, rows_new, st);
 }
 
-static int advance_and_reserve(vcla_ctx* c, int B, const int32_t* tok, cudaStream_t st) {
-  if (advance_seq(c->seq_len, B, 1, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st,
-                  c->ring(), c->tok_hist)) return -1;
-  return c->beam_on ? beam_reorder(c, B, B, tok, st) : 0;
-}
-
 // -------------------------------------------------------------------------------------------------
 // decode
 // -------------------------------------------------------------------------------------------------
-// ---- workspace schedule (batches 33..64): 8 kernels per layer, split-K partials in L2 workspaces + separate consumer kernels ----
-static int decode_enqueue_workspace(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, cudaStream_t st) {
-  const vcla_config& g = c->cfg;
-  const int TH = g.t_hidden, F = g.t_ffn;
-  count(c); if (embed_tokens_i32(tok_in, B, TH, c->embed, g.t_vocab, c->d_resid, st)) return -1;
-  for (int i = 0; i < g.t_layers; ++i) {
-    const TextLayer& L = c->tl[i];
-    count(c); if (dec_resid_norm(i == 0 ? nullptr : c->ws_d, c->sp_d, B, c->d_resid, B, TH, L.ln1, g.t_eps, c->d_xn, st)) return -1;
-    if (ws_gemm(c, DG_QKV, i, B, st)) return -1;
-    count(c); if (attention_decode(decode_attn_call(c, L, B, c->sp_qkv), st)) return -1;
-    if (ws_gemm(c, DG_O, i, B, st)) return -1;
-    count(c); if (dec_resid_norm(c->ws_o, c->sp_o, B, c->d_resid, B, TH, L.ln2, g.t_eps, c->d_xn, st)) return -1;
-    if (ws_gemm(c, DG_GATE_UP, i, B, st)) return -1;
-    count(c); if (dec_silu_mul(c->ws_gu, c->sp_gu, B, B, F, c->d_h, st)) return -1;
-    if (ws_gemm(c, DG_DOWN, i, B, st)) return -1;
-  }
-  count(c); if (dec_resid_norm(c->ws_d, c->sp_d, B, c->d_resid, B, TH, c->final_norm, g.t_eps, c->d_xn, st)) return -1;
-  if (ws_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
-  if (logits_argmax(c, B, logits, tok_out, 1, st)) return -1;
-  count(c); if (advance_and_reserve(c, B, tok_out, st)) return -1;
-  return 0;
-}
-
-// ---- cluster split-K schedule (batches <= 32, every batch with int8 projections): 5 kernels per layer, no split-K workspace,
-// no consumer kernels ------------------------------------------------------------------------------------------------------------
 // CTAs per cluster for a [M, K] weight at batch B: the choice that keeps the largest share of the 2 x SMs CTA slots busy over whole
 // rounds of cluster-tiles (clusters are gang-scheduled: floor(slots / S) of them are resident).  q8: the int8 kernel's batch tiles.
 static int csk_pick(int M, int K, int B, bool q8 = false) {
@@ -1244,9 +1218,8 @@ static int csk_prepare(vcla_ctx* c, int B) {
   if (c->csk_batch == B) return 0;
   const vcla_config& g = c->cfg;
   const bool q8 = g.weight_format == 1;
-  // the bf16 lm_head runs on the cluster kernel only up to 32 rows (beyond: the workspace GEMM, see decode_enqueue_csk)
   int v[5] = {csk_pick(3 * g.t_hidden, g.t_hidden, B, q8), csk_pick(g.t_hidden, g.t_hidden, B, q8), csk_pick(2 * g.t_ffn, g.t_hidden, B, q8),
-              csk_pick(g.t_hidden, g.t_ffn, B, q8), B <= 32 ? csk_pick(g.t_vocab, g.t_hidden, B) : 1};
+              csk_pick(g.t_hidden, g.t_ffn, B, q8), lm_head_uses_csk(B) ? csk_pick(g.t_vocab, g.t_hidden, B) : 1};
   if (const char* e = getenv("VCLA_CSK_SPLITS")) {            // tuning override: "qkv,o,gu,d,lm"
     int o[5];
     if (sscanf(e, "%d,%d,%d,%d,%d", &o[0], &o[1], &o[2], &o[3], &o[4]) == 5) for (int i = 0; i < 5; ++i) if (o[i] >= 1 && o[i] <= 8) v[i] = o[i];
@@ -1256,32 +1229,58 @@ static int csk_prepare(vcla_ctx* c, int B) {
   return 0;
 }
 
-// Decode step, 5 kernels per layer:  QKV GEMM [rstd] -> attention(+RoPE, append) -> O GEMM [+residual, norm weight, sum sq]
-//   -> gate/up GEMM [rstd, SiLU*mul] -> down GEMM [+residual, next norm weight, sum sq].  The bracketed consumers run inside the
-// GEMM after the cluster's split-K reduction; RMSNorm's per-row scale rstd is deferred to the consuming GEMM.
-static int decode_enqueue_csk(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, cudaStream_t st) {
+// Workspace layer stack (bf16 at 33..64 rows), 8 kernels per layer: split-K partials in L2 workspaces reduced by separate consumer
+// kernels.  Ends with the final norm, so d_xn holds the normalised rows for the lm_head.
+static int ws_stack(vcla_ctx* c, const int32_t* tok_in, int B, cudaStream_t st) {
+  const vcla_config& g = c->cfg;
+  const int TH = g.t_hidden, F = g.t_ffn;
+  count(c); if (embed_tokens_i32(tok_in, B, TH, c->embed, g.t_vocab, c->d_resid, st)) return -1;
+  for (int i = 0; i < g.t_layers; ++i) {
+    const TextLayer& L = c->tl[i];
+    count(c); if (dec_resid_norm(i == 0 ? nullptr : c->ws_d, c->sp_d, B, c->d_resid, B, TH, L.ln1, g.t_eps, c->d_xn, st)) return -1;
+    if (ws_gemm(c, DG_QKV, i, B, st)) return -1;
+    count(c); if (attention_decode(decode_attn_call(c, L, B, c->sp_qkv), st)) return -1;
+    if (ws_gemm(c, DG_O, i, B, st)) return -1;
+    count(c); if (dec_resid_norm(c->ws_o, c->sp_o, B, c->d_resid, B, TH, L.ln2, g.t_eps, c->d_xn, st)) return -1;
+    if (ws_gemm(c, DG_GATE_UP, i, B, st)) return -1;
+    count(c); if (dec_silu_mul(c->ws_gu, c->sp_gu, B, B, F, c->d_h, st)) return -1;
+    if (ws_gemm(c, DG_DOWN, i, B, st)) return -1;
+  }
+  count(c); return dec_resid_norm(c->ws_d, c->sp_d, B, c->d_resid, B, TH, c->final_norm, g.t_eps, c->d_xn, st);
+}
+
+// Cluster split-K layer stack (batches <= 32, every batch with int8 projections), 5 kernels per layer:  QKV GEMM [rstd] ->
+// attention(+RoPE, append) -> O GEMM [+residual, norm weight, sum sq] -> gate/up GEMM [rstd, SiLU*mul] -> down GEMM [+residual, next
+// norm weight, sum sq].  The bracketed consumers run inside the GEMM after the cluster's split-K reduction; RMSNorm's per-row scale
+// rstd is deferred to the consuming GEMM.  lookup: a verification step over B rows of the one resident sequence, whose attention is
+// the multi-query mode with the one-row KV split count.
+static int csk_stack(vcla_ctx* c, const int32_t* tok_in, int B, bool lookup, cudaStream_t st) {
   const vcla_config& g = c->cfg;
   const int TH = g.t_hidden;
   count(c); if (dec_embed(tok_in, B, TH, c->embed, g.t_vocab, c->d_resid, c->tl[0].ln1, c->d_xn, c->d_ssq, (TH + 127) / 128, st)) return -1;
   for (int i = 0; i < g.t_layers; ++i) {
     if (csk_gemm(c, DG_QKV, i, B, st)) return -1;
-    count(c); if (attention_decode(decode_attn_call(c, c->tl[i], B, 1), st)) return -1;
+    if (lookup) {
+      DecodeAttnCall a = decode_attn_call(c, c->tl[i], 1, 1);
+      a.B = B; a.ws_rows = B;
+      count(c, 2); if (attention_decode_lookup(a, st)) return -1;
+    } else {
+      count(c); if (attention_decode(decode_attn_call(c, c->tl[i], B, 1), st)) return -1;
+    }
     if (csk_gemm(c, DG_O, i, B, st) || csk_gemm(c, DG_GATE_UP, i, B, st) || csk_gemm(c, DG_DOWN, i, B, st)) return -1;
   }
-  if (B > 32) {
-    // int8 projections at 33..64 rows: the bf16 lm_head streams once through the workspace GEMM over the normalised rows
-    count(c); if (dec_resid_norm(nullptr, 0, B, c->d_resid, B, TH, c->final_norm, g.t_eps, c->d_xn, st)) return -1;
-    if (ws_gemm(c, DG_LM_HEAD, 0, B, st) || logits_argmax(c, B, logits, tok_out, 1, st)) return -1;
-  } else {
-    if (csk_gemm(c, DG_LM_HEAD, 0, B, st)) return -1;
-    if (logits_argmax(c, B, logits, tok_out, 1, st, 1)) return -1;
-  }
-  count(c); if (advance_and_reserve(c, B, tok_out, st)) return -1;
   return 0;
 }
 
-static int decode_enqueue(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, cudaStream_t st) {
-  return decode_uses_csk(c, B) ? decode_enqueue_csk(c, tok_in, B, logits, tok_out, st) : decode_enqueue_workspace(c, tok_in, B, logits, tok_out, st);
+// The lm_head of a decode step over B rows.  -> the split-K partials it left in ws_lm (1: the cluster kernel reduced them), -1 on
+// error.  The workspace GEMM reads normalised rows: after the cluster stack (rows_normed false) d_resid is normalised first.
+static int lm_head(vcla_ctx* c, int B, bool rows_normed, cudaStream_t st) {
+  if (lm_head_uses_csk(B)) return csk_gemm(c, DG_LM_HEAD, 0, B, st) ? -1 : 1;
+  if (!rows_normed) {
+    const vcla_config& g = c->cfg;
+    count(c); if (dec_resid_norm(nullptr, 0, B, c->d_resid, B, g.t_hidden, c->final_norm, g.t_eps, c->d_xn, st)) return -1;
+  }
+  return ws_gemm(c, DG_LM_HEAD, 0, B, st) ? -1 : c->sp_lm;
 }
 
 static LookupCall lookup_call(vcla_ctx* c) {
@@ -1293,34 +1292,36 @@ static LookupCall lookup_call(vcla_ctx* c) {
   return k;
 }
 
-// Prompt lookup verification step of the one resident sequence: the cluster split-K schedule over R = lk_rows rows with the split
-// counts of a one-row step (csk_prepare(c, 1)), so every row's logits are those of a one-token step; attention in its multi-query
-// mode with the one-row KV split count; the picks of all rows; then accept / advance / draft in place of advance_seq.
-static int decode_enqueue_lookup(vcla_ctx* c, cudaStream_t st) {
-  const vcla_config& g = c->cfg;
-  const int TH = g.t_hidden, V = g.t_vocab, R = c->lk_rows;
-  count(c); if (dec_embed(c->lk_tok, R, TH, c->embed, V, c->d_resid, c->tl[0].ln1, c->d_xn, c->d_ssq, (TH + 127) / 128, st)) return -1;
-  for (int i = 0; i < g.t_layers; ++i) {
-    if (csk_gemm(c, DG_QKV, i, R, st)) return -1;
-    DecodeAttnCall a = decode_attn_call(c, c->tl[i], 1, 1);
-    a.B = R; a.ws_rows = R;
-    count(c, 2); if (attention_decode_lookup(a, st)) return -1;
-    if (csk_gemm(c, DG_O, i, R, st) || csk_gemm(c, DG_GATE_UP, i, R, st) || csk_gemm(c, DG_DOWN, i, R, st)) return -1;
-  }
-  if (csk_gemm(c, DG_LM_HEAD, 0, R, st)) return -1;
-  count(c, 2);
-  if (c->samp_on) {
-    if (dec_logits_reduce(c->ws_lm, 1, R, V, R, V, c->samp_logits, V, c->cand_val, c->cand_idx, st) ||
-        dec_sample_lookup(c->samp_logits, V, V, R, c->tok_hist, c->step_idx, c->samp_params, c->lk_pick, st)) return -1;
-  } else {
-    if (dec_logits_argmax(c->ws_lm, 1, R, V, R, V, nullptr, V, c->lk_pick, nullptr, nullptr, c->cand_val, c->cand_idx, nullptr, st)) return -1;
-  }
-  count(c); return lookup_accept(lookup_call(c), 0, st);
+// The B sequences take the step's tokens: their lengths grow by one and the page the next token goes to is reserved (beam search then
+// rearranges the rows after their parents).  lookup: accept the verified picks, advance, and draft the next step's rows instead.
+static int advance(vcla_ctx* c, int B, const int32_t* tok, bool lookup, cudaStream_t st) {
+  count(c);
+  if (lookup) return lookup_accept(lookup_call(c), 0, st);
+  if (advance_seq(c->seq_len, B, 1, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st,
+                  c->ring(), c->tok_hist)) return -1;
+  return c->beam_on ? beam_reorder(c, B, B, tok, st) : 0;
+}
+
+// One decode step: the layer stack of the batch's schedule, the lm_head, the pick and the advance.  With prompt lookup set, the step
+// verifies the lk_rows rows in lk_tok of the one resident sequence on the cluster stack at the split counts of a one-row step
+// (csk_prepare(c, 1)), so every row's logits are those of a one-token step.
+static int enqueue_decode_step(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, cudaStream_t st) {
+  const bool lookup = c->lk_on, csk = lookup || decode_uses_csk(c, B);
+  const int rows = lookup ? c->lk_rows : B;
+  if (csk ? csk_stack(c, lookup ? c->lk_tok : tok_in, rows, lookup, st) : ws_stack(c, tok_in, B, st)) return -1;
+  const int lm_splits = lm_head(c, rows, !csk, st);
+  if (lm_splits < 0 || pick(c, rows, lm_splits, logits, tok_out, 1, lookup, st)) return -1;
+  return advance(c, B, tok_out, lookup, st);
+}
+
+// The key of a captured decode graph: the call's buffers and step count, and every mode that changes the captured work.
+static GraphKey graph_key(const vcla_ctx* c, const int32_t* tok_in, int B, const float* logits, const int32_t* tok_out, int n_steps) {
+  return GraphKey{B, tok_in, logits, tok_out, n_steps, c->dp_on() ? 1 : 0, c->samp_on ? 1 : 0, c->beam_on ? c->beam_K : 0, c->stream_armed ? 1 : 0,
+                  c->lk_on ? c->lk_rows : 0};
 }
 
 static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, int n_steps, cudaStream_t st) {
-  GraphKey key{B, tok_in, logits, tok_out, n_steps, c->dp_on() ? 1 : 0, c->samp_on ? 1 : 0, c->beam_on ? c->beam_K : 0, c->stream_armed ? 1 : 0,
-               c->lk_on ? c->lk_rows : 0};
+  const GraphKey key = graph_key(c, tok_in, B, logits, tok_out, n_steps);
   auto it = c->graphs.find(key);
   if (it == c->graphs.end()) {
     const int64_t before = c->launches;
@@ -1328,8 +1329,7 @@ static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits
     if (!c->cap_stream) VCLA_CUDA_OK(cudaStreamCreateWithFlags(&c->cap_stream, cudaStreamNonBlocking));
     VCLA_CUDA_OK(cudaStreamBeginCapture(c->cap_stream, cudaStreamCaptureModeThreadLocal));
     int rc = 0;
-    for (int i = 0; i < n_steps && rc == 0; ++i)
-      rc = c->lk_on ? decode_enqueue_lookup(c, c->cap_stream) : decode_enqueue(c, tok_in, B, logits, tok_out, c->cap_stream);
+    for (int i = 0; i < n_steps && rc == 0; ++i) rc = enqueue_decode_step(c, tok_in, B, logits, tok_out, c->cap_stream);
     if (rc == 0 && c->dp_on()) rc = dp_wait(c, c->cap_stream);      // a captured graph must join its forked exchange branch
     cudaError_t e = cudaStreamEndCapture(c->cap_stream, &graph);
     if (rc != 0) { if (graph) cudaGraphDestroy(graph); (void)cudaGetLastError(); return -1; }
@@ -1338,37 +1338,35 @@ static int decode_graph(vcla_ctx* c, const int32_t* tok_in, int B, float* logits
     e = cudaGraphInstantiate(&exec, graph, 0);
     cudaGraphDestroy(graph);
     if (e != cudaSuccess) { set_error("decode: graph instantiate failed: %s", cudaGetErrorString(e)); return -1; }
-    c->graph_launches[key] = c->launches - before;
+    const int64_t launches = c->launches - before;
     c->launches = before;  // capture enqueued nothing
     // bounded cache: a caller that keeps passing fresh buffers evicts the least recently used graph instead of growing forever.
     // (Evicting while an older launch of that graph may still be in flight needs the device to be idle first.)
     constexpr size_t kMaxGraphs = 24;
     if (c->graphs.size() >= kMaxGraphs) {
-      const GraphKey victim = c->graph_lru.back();
-      c->graph_lru.pop_back();
+      const auto victim = std::min_element(c->graphs.begin(), c->graphs.end(),
+                                           [](const auto& x, const auto& y) { return x.second.last_use < y.second.last_use; });
       VCLA_CUDA_OK(cudaDeviceSynchronize());
-      cudaGraphExecDestroy(c->graphs[victim]);
+      cudaGraphExecDestroy(victim->second.exec);
       c->graphs.erase(victim);
-      c->graph_launches.erase(victim);
     }
-    c->graphs[key] = exec;
-    c->graph_lru.push_front(key);
-    it = c->graphs.find(key);
-  } else {
-    for (auto li = c->graph_lru.begin(); li != c->graph_lru.end(); ++li) {
-      if (!(*li < key) && !(key < *li)) { c->graph_lru.erase(li); break; }
-    }
-    c->graph_lru.push_front(key);
+    it = c->graphs.emplace(key, DecodeGraph{exec, launches, 0}).first;
   }
-  VCLA_CUDA_OK(cudaGraphLaunch(it->second, st));
-  c->launches += c->graph_launches[key];
+  it->second.last_use = ++c->graph_uses;
+  VCLA_CUDA_OK(cudaGraphLaunch(it->second.exec, st));
+  c->launches += it->second.launches;
   return 0;
 }
 
-// Every decode step appends one token per sequence: refuse the call instead of running past the context capacity (the kernels
-// index the page table, the RoPE table and the token history by the sequence length).
-static int decode_capacity(vcla_ctx* c, int n_steps, int B) {
+// What a decode call needs after its argument checks, and the split counts of its cluster split-K GEMMs (occupancy queries: never
+// inside a capture).  Every decode step appends one token per sequence: refuse the call instead of running past the context
+// capacity (the kernels index the page table, the RoPE table and the token history by the sequence length).
+static int decode_begin(vcla_ctx* c, int n_steps, int B) {
   if (c->len_bound <= 0) { set_error("decode: no prefilled sequences (call vcla_prefill first)"); return -1; }
+  if (c->lk_on) {
+    if (B != 1 || c->resident_b != 1) { set_error("decode: prompt lookup steps one resident sequence (got B=%d, %d resident)", B, c->resident_b); return -1; }
+    return csk_prepare(c, 1);
+  }
   if (c->beam_on && B != c->resident_b) {
     // the beams of an item share pages: a step advances exactly the rows the prefill forked
     set_error("decode: beam search steps all %d rows the prefill forked (got %d)", c->resident_b, B);
@@ -1378,7 +1376,15 @@ static int decode_capacity(vcla_ctx* c, int n_steps, int B) {
     set_error("decode: %lld cached tokens + %d steps exceed the context capacity max_seq=%d", (long long)c->len_bound, n_steps, c->cfg.max_seq);
     return -1;
   }
-  return 0;
+  return decode_uses_csk(c, B) ? csk_prepare(c, B) : 0;
+}
+
+// After a decode call enqueued its work (rc == 0): the bound on the cached tokens grows by the steps it issued, and the token
+// stream records the work that publishes into it.
+static int decode_end(vcla_ctx* c, int rc, int n_steps, cudaStream_t st) {
+  if (rc != 0) return rc;
+  c->len_bound += n_steps;
+  return stream_mark(c, st);
 }
 
 int vcla_decode_step(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, int32_t* tok_out, int use_graph, vcla_stream stream) {
@@ -1386,43 +1392,32 @@ int vcla_decode_step(vcla_ctx* c, const int32_t* tok_in, int B, float* logits, i
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_in || !tok_out) { set_error("decode: null token buffers"); return -1; }
   if (c->lk_on) { set_error("decode: prompt lookup verification steps run through vcla_decode_multi"); return -1; }
-  if (decode_capacity(c, 1, B)) return -1;
-  if (decode_uses_csk(c, B) && csk_prepare(c, B)) return -1;      // occupancy queries: never inside a capture
-  int rc = use_graph ? decode_graph(c, tok_in, B, logits, tok_out, 1, st) : decode_enqueue(c, tok_in, B, logits, tok_out, st);
+  if (decode_begin(c, 1, B)) return -1;
+  int rc = use_graph ? decode_graph(c, tok_in, B, logits, tok_out, 1, st) : enqueue_decode_step(c, tok_in, B, logits, tok_out, st);
   if (rc == 0 && !use_graph && c->dp_on()) rc = dp_wait(c, st);
-  if (rc == 0) c->len_bound += 1;
-  return rc == 0 ? stream_mark(c, st) : rc;
+  return decode_end(c, rc, 1, st);
 }
 
 int vcla_decode_multi(vcla_ctx* c, int32_t* tok_inout, int B, int n_steps, vcla_stream stream) {
   // n_steps greedy decode steps captured back to back in ONE CUDA graph (the token buffer is consumed and rewritten in place,
   // every chosen token is appended to the device-side history): amortises the gap between consecutive graph launches.
+  cudaStream_t st = (cudaStream_t)stream;
   if (B < 1 || B > c->cfg.max_batch || B > 64) { set_error("decode: batch %d unsupported", B); return -1; }
   if (!tok_inout || n_steps < 1 || n_steps > 64) { set_error("decode_multi: bad arguments"); return -1; }
-  if (c->lk_on) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (c->len_bound <= 0) { set_error("decode: no prefilled sequences (call vcla_prefill first)"); return -1; }
-    if (B != 1 || c->resident_b != 1) { set_error("decode: prompt lookup steps one resident sequence (got B=%d, %d resident)", B, c->resident_b); return -1; }
-    if (csk_prepare(c, 1)) return -1;
-    if (!c->lk_primed) {
-      // right after the prefill: history rows = the prefill's pick, seq_len = the prompt
-      if (c->len_bound + c->lk_max_new + c->lk_rows - 1 > c->cfg.max_seq) {
-        set_error("decode: %lld cached tokens + max_new %d + %d drafts exceed the context capacity max_seq=%d", (long long)c->len_bound,
-                  c->lk_max_new, c->lk_rows - 1, c->cfg.max_seq);
-        return -1;
-      }
-      count(c); if (lookup_accept(lookup_call(c), 1, st)) return -1;
-      c->lk_primed = true;
-      c->len_bound += c->lk_max_new - 1;     // upper bound: at most max_new - 1 decoded tokens are cached
+  if (decode_begin(c, n_steps, B)) return -1;
+  if (c->lk_on && !c->lk_primed) {
+    // right after the prefill: history rows = the prefill's pick, seq_len = the prompt
+    if (c->len_bound + c->lk_max_new + c->lk_rows - 1 > c->cfg.max_seq) {
+      set_error("decode: %lld cached tokens + max_new %d + %d drafts exceed the context capacity max_seq=%d", (long long)c->len_bound,
+                c->lk_max_new, c->lk_rows - 1, c->cfg.max_seq);
+      return -1;
     }
-    const int rc = decode_graph(c, tok_inout, 1, nullptr, tok_inout, n_steps, st);
-    return rc == 0 ? stream_mark(c, st) : rc;
+    count(c); if (lookup_accept(lookup_call(c), 1, st)) return -1;
+    c->lk_primed = true;
+    c->len_bound += c->lk_max_new - 1;     // upper bound: at most max_new - 1 decoded tokens are cached
   }
-  if (decode_capacity(c, n_steps, B)) return -1;
-  if (decode_uses_csk(c, B) && csk_prepare(c, B)) return -1;
-  const int rc = decode_graph(c, tok_inout, B, nullptr, tok_inout, n_steps, (cudaStream_t)stream);
-  if (rc == 0) c->len_bound += n_steps;
-  return rc == 0 ? stream_mark(c, (cudaStream_t)stream) : rc;
+  const int rc = decode_graph(c, tok_inout, B, nullptr, tok_inout, n_steps, st);
+  return decode_end(c, rc, c->lk_on ? 0 : n_steps, st);   // lookup: the priming above bounded every step's tokens
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1730,7 +1725,7 @@ int vcla_bench_decode_gemm(vcla_ctx* c, int which, int B, int reps, float* avg_u
   cudaEvent_t e0, e1;
   VCLA_CUDA_OK(cudaEventCreate(&e0));
   VCLA_CUDA_OK(cudaEventCreate(&e1));
-  const bool csk = decode_uses_csk(c, B) && !(which == DG_LM_HEAD && B > 32);
+  const bool csk = which == DG_LM_HEAD ? lm_head_uses_csk(B) : decode_uses_csk(c, B);
   if (csk && csk_prepare(c, B)) return -1;
   auto run_all = [&]() -> int {
     const int layers = which == DG_LM_HEAD ? 1 : g.t_layers;
