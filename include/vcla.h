@@ -377,7 +377,8 @@ int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v
 /* The paged prefill attention of vcla_prefill_extend on caller buffers (head dim 128): q (B*T rows, q_stride) bf16; kv_pages a layer
  * pool [pages][K|V][H][page_tokens][128] bf16; page_table int32 (B, pages_per_seq); base_len_dev int32 (B) cached tokens before the
  * chunk (the chunk's own K/V must already be in the pool at slots base_len .. base_len + T - 1); out (B*T rows, o_stride) bf16.
- * Key j is visible to chunk row t iff j <= base_len[b] + t.  Synchronises. */
+ * Key j is visible to chunk row t iff j <= base_len[b] + t.  Refused on the host, before any launch: base_len[b] < 0,
+ * base_len[b] + T > pages_per_seq * page_tokens, a negative page among the entries the chunk reads.  Synchronises. */
 int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, const int32_t* page_table, int pages_per_seq,
                             int page_tokens, const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T, float scale,
                             vcla_stream stream);

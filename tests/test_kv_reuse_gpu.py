@@ -94,6 +94,16 @@ def _paged_run(q, pool, table, lens, pt):
     return out.view(B, T, H, 128).float().cpu()
 
 
+def test_paged_attention_operator_refuses_a_negative_page():
+    """A negative table entry among those the chunk reads is refused on the host, before any launch."""
+    from visualcla import _native as N
+    lens, T, pt = [20, 3], 5, 8
+    q, pool, table, _ks, _vs = _paged_case(pt, lens, T, 2, seed=3)
+    table[1, 0] = -1                                   # sequence 1 reads page 0 only (3 + 5 tokens)
+    with pytest.raises(N.NativeError, match="no page 0"):
+        _paged_run(q, pool, table, lens, pt)
+
+
 @pytest.mark.parametrize("pt", [8, 16, 32, 64])
 @pytest.mark.parametrize("prefix", [0, 1, 63, 64, 65, 1500])
 def test_paged_attention_operator(pt, prefix):

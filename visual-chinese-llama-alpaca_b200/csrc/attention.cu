@@ -269,7 +269,7 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
 
   const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int T = c.H * HD, PT = c.page_tokens;
+  const int T = c.kv.heads * HD, PT = c.kv.page_tokens;
   const uint32_t stage_bytes = (uint32_t)PT * HD * 2 * 2;      // K page + V page
   TraceScope trace(MODE == kDecAppend ? 19 : 4);
   const int sb = MODE == kDecPlain ? b : 0;   // the sequence whose pages and length this CTA reads
@@ -296,13 +296,13 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
 
   auto issue_page = [&](int i) {                      // thread 0: request page i of this CTA into stage i % STAGES
     const int stage = i % STAGES;
-    const int page = __ldg(c.page_table + (size_t)sb * c.pages_per_seq + p0 + i);
+    const int page = __ldg(c.kv.seq_pages(sb) + p0 + i);
     const int ntok = min(PT, c_end - (t_begin + i * PT));
     const uint32_t bytes = (uint32_t)ntok * HD * 2;
     const uint32_t bar = smem_u32(&s_bar[stage]);
     const uint32_t dst = smem_u32(dsm) + stage * stage_bytes;
-    const bf16* ksrc = c.kv_pages + ((((size_t)page * 2 + 0) * c.H + h) * PT) * HD;
-    const bf16* vsrc = c.kv_pages + ((((size_t)page * 2 + 1) * c.H + h) * PT) * HD;
+    const bf16* ksrc = c.kv.at(page, 0, h, 0);
+    const bf16* vsrc = c.kv.at(page, 1, h, 0);
     mbar_arrive_expect_tx(bar, 2 * bytes);
     bulk_load_1d(dst, ksrc, bytes, bar);
     bulk_load_1d(dst + (uint32_t)PT * HD * 2, vsrc, bytes, bar);
@@ -341,10 +341,10 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
         s_k[d] = __bfloat162float(kb);
         s_v[d] = __bfloat162float(vb);
         if (MODE != kDecAttend) {
-          const int page = c.page_table[(size_t)sb * c.pages_per_seq + L / PT];
+          const int page = c.kv.seq_pages(sb)[L / PT];
           const int slot = L % PT;
-          bf16* kdst = c.kv_pages + ((((size_t)page * 2 + 0) * c.H + h) * PT + slot) * HD;
-          bf16* vdst = c.kv_pages + ((((size_t)page * 2 + 1) * c.H + h) * PT + slot) * HD;
+          bf16* kdst = c.kv.at(page, 0, h, slot);
+          bf16* vdst = c.kv.at(page, 1, h, slot);
           kdst[d] = kb;
           vdst[d] = vb;
         }
@@ -463,20 +463,20 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
     return;
   }
   // ---- cross-CTA combine: publish partial, last arriver reduces in fixed split order
-  float* sp = c.scratch + (((size_t)b * c.H + h) * c.kv_splits + split) * (HD + 2);
+  float* sp = c.scratch + (((size_t)b * c.kv.heads + h) * c.kv_splits + split) * (HD + 2);
   if (tid < HD) sp[tid] = O;
   if (tid == 0) { sp[HD] = M; sp[HD + 1] = Lsum; }
   __threadfence();
   __syncthreads();
   if (tid == 0) {
-    const int old = atomicAdd(c.counters + b * c.H + h, 1);
+    const int old = atomicAdd(c.counters + b * c.kv.heads + h, 1);
     s_last = (old == c.kv_splits - 1);
   }
   __syncthreads();
   if (!s_last) { trace.done(); return; }
   __threadfence();
   if (tid < HD) {
-    const float* base = c.scratch + ((size_t)b * c.H + h) * c.kv_splits * (HD + 2);
+    const float* base = c.scratch + ((size_t)b * c.kv.heads + h) * c.kv_splits * (HD + 2);
     float Mg = -INFINITY;
     for (int s = 0; s < c.kv_splits; ++s) Mg = fmaxf(Mg, __ldcg(base + (size_t)s * (HD + 2) + HD));
     float Lg = 0.f, Og = 0.f;
@@ -488,7 +488,7 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
     }
     c.out[(size_t)b * T + h * HD + tid] = __float2bfloat16(Og / Lg);
   }
-  if (tid == 0) c.counters[b * c.H + h] = 0;  // ready for the next step / graph replay
+  if (tid == 0) c.counters[b * c.kv.heads + h] = 0;  // ready for the next step / graph replay
   trace.done();
 }
 
@@ -517,7 +517,7 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
   __shared__ float s_m[kDecWarps], s_l[kDecWarps];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int T = c.H * HD, PT = c.page_tokens;
+  const int T = c.kv.heads * HD, PT = c.kv.page_tokens;
   const uint32_t stage_bytes = (uint32_t)PT * HD * 2 * 2;
   TraceScope trace(4);
   if (tid == 0) {
@@ -535,19 +535,19 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
     if (lane == 0) {
       uint32_t n = 0;                                   // pages issued so far (ring position)
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int b = item / c.H, h = item % c.H;
+        const int b = item / c.kv.heads, h = item % c.kv.heads;
         const int L = c.seq_len[b];
         const int npages = (L + PT - 1) / PT;
         for (int i = 0; i < npages; ++i, ++n) {
           const int stage = n % kDecStages;
           mbar_wait(smem_u32(&s_empty[stage]), ((n / kDecStages) & 1u) ^ 1u);
-          const int page = __ldg(c.page_table + (size_t)b * c.pages_per_seq + i);
+          const int page = __ldg(c.kv.seq_pages(b) + i);
           const int ntok = min(PT, L - i * PT);
           const uint32_t bytes = (uint32_t)ntok * HD * 2;
           const uint32_t bar = smem_u32(&s_full[stage]);
           const uint32_t dst = smem_u32(dsm) + stage * stage_bytes;
-          const bf16* ksrc = c.kv_pages + ((((size_t)page * 2 + 0) * c.H + h) * PT) * HD;
-          const bf16* vsrc = c.kv_pages + ((((size_t)page * 2 + 1) * c.H + h) * PT) * HD;
+          const bf16* ksrc = c.kv.at(page, 0, h, 0);
+          const bf16* vsrc = c.kv.at(page, 1, h, 0);
           mbar_arrive_expect_tx(bar, 2 * bytes);
           bulk_load_1d(dst, ksrc, bytes, bar);
           bulk_load_1d(dst + (uint32_t)PT * HD * 2, vsrc, bytes, bar);
@@ -562,7 +562,7 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
     for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++qi) {
       const int slot = qi & 1;
       mbar_wait(smem_u32(&s_qempty[slot]), ((qi >> 1) & 1u) ^ 1u);
-      const int b = item / c.H, h = item % c.H;
+      const int b = item / c.kv.heads, h = item % c.kv.heads;
       const int L = c.seq_len[b];
       float q4[4] = {0.f, 0.f, 0.f, 0.f}, k4[4] = {0.f, 0.f, 0.f, 0.f}, v4[4] = {0.f, 0.f, 0.f, 0.f};
       for (int s0 = 0; s0 < c.splits; s0 += 2) {          // two splits (6 x 16 B loads) in flight
@@ -602,10 +602,10 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
       *reinterpret_cast<float4*>(&s_q[slot][4 * lane]) = make_float4(qo[0], qo[1], qo[2], qo[3]);
       *reinterpret_cast<float4*>(&s_k[slot][4 * lane]) = make_float4(ko[0], ko[1], ko[2], ko[3]);
       *reinterpret_cast<float4*>(&s_v[slot][4 * lane]) = make_float4(vo[0], vo[1], vo[2], vo[3]);
-      const int page = __ldg(c.page_table + (size_t)b * c.pages_per_seq + L / PT);
+      const int page = __ldg(c.kv.seq_pages(b) + L / PT);
       const int cslot = L % PT;
-      *reinterpret_cast<uint2*>(c.kv_pages + ((((size_t)page * 2 + 0) * c.H + h) * PT + cslot) * HD + 4 * lane) = make_uint2(kpk[0], kpk[1]);
-      *reinterpret_cast<uint2*>(c.kv_pages + ((((size_t)page * 2 + 1) * c.H + h) * PT + cslot) * HD + 4 * lane) = make_uint2(vpk[0], vpk[1]);
+      *reinterpret_cast<uint2*>(c.kv.at(page, 0, h, cslot) + 4 * lane) = make_uint2(kpk[0], kpk[1]);
+      *reinterpret_cast<uint2*>(c.kv.at(page, 1, h, cslot) + 4 * lane) = make_uint2(vpk[0], vpk[1]);
       __syncwarp();
       if (lane == 0) mbar_arrive(smem_u32(&s_qfull[slot]));
     }
@@ -617,7 +617,7 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
   const uint32_t gmask = 0xffu << (grp * 8);
   uint32_t n = 0, qi = 0;
   for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++qi) {
-    const int b = item / c.H, h = item % c.H;
+    const int b = item / c.kv.heads, h = item % c.kv.heads;
     const int L = c.seq_len[b];
     const int npages = (L + PT - 1) / PT;
     const int slot = qi & 1;
@@ -742,7 +742,7 @@ int attention_init() {
 // a 2- or 3-stage ring.
 enum DecodeKernel { kDecPersistent, kDecOneShot2, kDecOneShot3 };
 static DecodeKernel decode_kernel_pick(const DecodeAttnCall& c, int* persistent_ctas) {
-  const int n_items = c.B * c.H;
+  const int n_items = c.B * c.kv.heads;
   int slots = 2 * num_sms();
   // persistent_mode: 0 = never, 1 (default) = when items outnumber the resident CTAs, 2 = whenever kv_splits == 1 (tests);
   // persistent_grid caps the persistent grid (tests: several items per CTA on small problems).  Both are read from the
@@ -758,12 +758,12 @@ static DecodeKernel decode_kernel_pick(const DecodeAttnCall& c, int* persistent_
 
 int attention_decode(const DecodeAttnCall& c, cudaStream_t st) {
   if (c.HD != 128) { set_error("attention_decode: head dim %d unsupported (128)", c.HD); return -1; }
-  if (c.page_tokens < 8 || c.page_tokens > kDecMaxPT || c.page_tokens % 8 != 0) { set_error("attention_decode: page_tokens %d unsupported (8..%d, multiple of 8)", c.page_tokens, kDecMaxPT); return -1; }
+  if (c.kv.page_tokens < 8 || c.kv.page_tokens > kDecMaxPT || c.kv.page_tokens % 8 != 0) { set_error("attention_decode: page_tokens %d unsupported (8..%d, multiple of 8)", c.kv.page_tokens, kDecMaxPT); return -1; }
   if (c.rope_cos == nullptr || c.rope_sin == nullptr) { set_error("attention_decode: rope table not initialised"); return -1; }
   if (attention_init()) return -1;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(c.kv_splits, c.H, c.B); cfg.blockDim = dim3(kDecWarps * 32);
-  cfg.dynamicSmemBytes = (size_t)kDecStages * c.page_tokens * 128 * 2 * 2; cfg.stream = st;
+  cfg.gridDim = dim3(c.kv_splits, c.kv.heads, c.B); cfg.blockDim = dim3(kDecWarps * 32);
+  cfg.dynamicSmemBytes = (size_t)kDecStages * c.kv.page_tokens * 128 * 2 * 2; cfg.stream = st;
   cudaLaunchAttribute attr[1];
   int na = 0;
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
@@ -773,10 +773,10 @@ int attention_decode(const DecodeAttnCall& c, cudaStream_t st) {
     case kDecPersistent:
       cfg.gridDim = dim3(persistent_ctas);
       cfg.blockDim = dim3((kDecWarps + 2) * 32);
-      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_persistent_kernel, c, c.rope_cos, c.rope_sin, c.B * c.H));
+      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_persistent_kernel, c, c.rope_cos, c.rope_sin, c.B * c.kv.heads));
       break;
     case kDecOneShot2:
-      cfg.dynamicSmemBytes = (size_t)kDecStagesSmallBatch * c.page_tokens * 128 * 2 * 2;
+      cfg.dynamicSmemBytes = (size_t)kDecStagesSmallBatch * c.kv.page_tokens * 128 * 2 * 2;
       VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch>, c, c.rope_cos, c.rope_sin));
       break;
     case kDecOneShot3:
@@ -788,7 +788,7 @@ int attention_decode(const DecodeAttnCall& c, cudaStream_t st) {
 
 int attention_decode_lookup(const DecodeAttnCall& c, cudaStream_t st) {
   if (c.HD != 128) { set_error("attention_decode_lookup: head dim %d unsupported (128)", c.HD); return -1; }
-  if (c.page_tokens < 8 || c.page_tokens > kDecMaxPT || c.page_tokens % 8 != 0) { set_error("attention_decode_lookup: page_tokens %d unsupported (8..%d, multiple of 8)", c.page_tokens, kDecMaxPT); return -1; }
+  if (c.kv.page_tokens < 8 || c.kv.page_tokens > kDecMaxPT || c.kv.page_tokens % 8 != 0) { set_error("attention_decode_lookup: page_tokens %d unsupported (8..%d, multiple of 8)", c.kv.page_tokens, kDecMaxPT); return -1; }
   if (c.rope_cos == nullptr || c.rope_sin == nullptr) { set_error("attention_decode_lookup: rope table not initialised"); return -1; }
   if (c.kv_splits < 1 || c.kv_splits > 8 || c.B < 1 || c.B > 16) { set_error("attention_decode_lookup: %d rows x %d KV splits unsupported", c.B, c.kv_splits); return -1; }
   if (attention_init()) return -1;
@@ -797,15 +797,15 @@ int attention_decode_lookup(const DecodeAttnCall& c, cudaStream_t st) {
   int na = 0;
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = attr; cfg.numAttrs = na; cfg.stream = st; cfg.blockDim = dim3(kDecWarps * 32);
-  cfg.gridDim = dim3(1, c.H, c.B); cfg.dynamicSmemBytes = 0;
+  cfg.gridDim = dim3(1, c.kv.heads, c.B); cfg.dynamicSmemBytes = 0;
   VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch, kDecAppend>, c, c.rope_cos, c.rope_sin));
   // the ring depth changes no arithmetic; the one-token rule picks it from the grid size
-  cfg.gridDim = dim3(c.kv_splits, c.H, c.B);
-  if (c.kv_splits * c.B * c.H <= 2 * num_sms()) {
-    cfg.dynamicSmemBytes = (size_t)kDecStagesSmallBatch * c.page_tokens * 128 * 2 * 2;
+  cfg.gridDim = dim3(c.kv_splits, c.kv.heads, c.B);
+  if (c.kv_splits * c.B * c.kv.heads <= 2 * num_sms()) {
+    cfg.dynamicSmemBytes = (size_t)kDecStagesSmallBatch * c.kv.page_tokens * 128 * 2 * 2;
     VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch, kDecAttend>, c, c.rope_cos, c.rope_sin));
   } else {
-    cfg.dynamicSmemBytes = (size_t)kDecStages * c.page_tokens * 128 * 2 * 2;
+    cfg.dynamicSmemBytes = (size_t)kDecStages * c.kv.page_tokens * 128 * 2 * 2;
     VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStages, kDecAttend>, c, c.rope_cos, c.rope_sin));
   }
   return 0;
@@ -817,13 +817,13 @@ int attention_decode_ctas_per_sm(const DecodeAttnCall& c) {
   cudaError_t e = cudaSuccess;
   switch (decode_kernel_pick(c, &persistent_ctas)) {
     case kDecPersistent:
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_persistent_kernel, (kDecWarps + 2) * 32, (size_t)kDecStages * c.page_tokens * 128 * 2 * 2);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_persistent_kernel, (kDecWarps + 2) * 32, (size_t)kDecStages * c.kv.page_tokens * 128 * 2 * 2);
       break;
     case kDecOneShot2:
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStagesSmallBatch>, kDecWarps * 32, (size_t)kDecStagesSmallBatch * c.page_tokens * 128 * 2 * 2);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStagesSmallBatch>, kDecWarps * 32, (size_t)kDecStagesSmallBatch * c.kv.page_tokens * 128 * 2 * 2);
       break;
     case kDecOneShot3:
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStages>, kDecWarps * 32, (size_t)kDecStages * c.page_tokens * 128 * 2 * 2);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStages>, kDecWarps * 32, (size_t)kDecStages * c.kv.page_tokens * 128 * 2 * 2);
       break;
   }
   if (e != cudaSuccess) { set_error("attention_decode_ctas_per_sm: %s", cudaGetErrorString(e)); (void)cudaGetLastError(); return -1; }

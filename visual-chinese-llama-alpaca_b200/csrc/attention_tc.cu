@@ -42,11 +42,11 @@ struct AttnTcParams {
   const int32_t* kv_start;         // [B] or null
   bf16* out; int o_stride;
   // PAGED only
-  const int32_t* page_table; int pages_per_seq, page_tokens;
   const int32_t* base_len;         // [B] cached tokens before the chunk
   int kv_splits;                   // CTAs per (query tile, head, sequence); blockIdx.z = b * kv_splits + split
   float* part;                     // kv_splits > 1: [tile][split][64 rows][HD + 4] = unnormalised O, running max, row sum, pad
   int32_t* counters;               // [tile] arrivals, back to 0 after the combine
+  KvPool kv;                       // the layer's pages
 };
 
 template <int HD>
@@ -139,11 +139,11 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         if constexpr (PAGED) {
           // one box of page_tokens rows per page and 64-column half; boxes past the sequence's last page re-read that page
           // (only pages the sequence owns are touched; those rows are masked)
-          const int pt = p.page_tokens, last_page = (n0 - 1) / pt;
-          const int32_t* prow = p.page_table + (size_t)b * p.pages_per_seq;
+          const int pt = p.kv.page_tokens, last_page = (n0 - 1) / pt;
+          const int32_t* prow = p.kv.seq_pages(b);
           for (int r = 0; r < kAtBKV; r += pt) {
             const int page = prow[min((j * kAtBKV + r) / pt, last_page)];
-            const int krow = ((page * 2) * p.H + h) * pt, vrow = krow + p.H * pt;
+            const int krow = p.kv.row<int>(page, 0, h), vrow = p.kv.row<int>(page, 1, h);
             for (int kb = 0; kb < C::KB; ++kb) {
               tma_load_2d(sk + kb * kAtBKV * 128 + r * 128, &tmK0, kb * 64, krow, kv_full(stage), kEvictNormal);
               tma_load_2d(sv + kb * kAtBKV * 128 + r * 128, &tmK0, kb * 64, vrow, kv_full(stage), kEvictNormal);
@@ -408,25 +408,25 @@ static int paged_kv_splits(int ctas, int max_kv) {
 
 int attention_paged(const AttnPagedCall& c, cudaStream_t st) {
   if (attn_tc_init()) return -1;
-  if (c.page_tokens < 8 || c.page_tokens > 64 || c.page_tokens % 8 != 0) { set_error("attention_paged: page_tokens %d must be a multiple of 8 <= 64", c.page_tokens); return -1; }
-  if (c.B < 1 || c.H < 1 || c.T < 1 || c.pool_pages < 1) { set_error("attention_paged: empty launch"); return -1; }
+  if (c.kv.page_tokens < 8 || c.kv.page_tokens > 64 || c.kv.page_tokens % 8 != 0) { set_error("attention_paged: page_tokens %d must be a multiple of 8 <= 64", c.kv.page_tokens); return -1; }
+  if (c.B < 1 || c.kv.heads < 1 || c.T < 1 || c.kv.total_pages < 1) { set_error("attention_paged: empty launch"); return -1; }
   if ((c.o_stride % 8) != 0) { set_error("attention_paged: output pitch must keep 16 B alignment"); return -1; }
   CUtensorMap tq, tkv;
-  if (attn_tmap(&tq, c.q, (uint64_t)c.B * c.T, (uint64_t)c.H * 128, c.q_stride)) return -1;
-  if (attn_tmap(&tkv, c.kv_pages, (uint64_t)c.pool_pages * 2 * c.H * c.page_tokens, 128, 128, c.page_tokens)) return -1;
-  const int qt = (c.T + kAtBQ - 1) / kAtBQ, ctas = qt * c.H * c.B;
+  if (attn_tmap(&tq, c.q, (uint64_t)c.B * c.T, (uint64_t)c.kv.heads * 128, c.q_stride)) return -1;
+  if (attn_tmap(&tkv, c.kv.pages, c.kv.row<uint64_t>(c.kv.total_pages, 0, 0), 128, 128, c.kv.page_tokens)) return -1;
+  const int qt = (c.T + kAtBQ - 1) / kAtBQ, ctas = qt * c.kv.heads * c.B;
   const int splits = paged_kv_splits(ctas, c.max_kv);
   if (splits > 1 && (c.part == nullptr || c.counters == nullptr || (int64_t)ctas * splits > attention_paged_partials())) {
     set_error("attention_paged: split-KV scratch missing or too small"); return -1;
   }
   AttnTcParams p;
   memset(&p, 0, sizeof(p));
-  p.Sq = c.T; p.H = c.H; p.sl2 = c.scale * 1.4426950408889634f; p.causal = 1; p.out = c.out; p.o_stride = c.o_stride;
-  p.page_table = c.page_table; p.pages_per_seq = c.pages_per_seq; p.page_tokens = c.page_tokens; p.base_len = c.base_len;
+  p.Sq = c.T; p.H = c.kv.heads; p.sl2 = c.scale * 1.4426950408889634f; p.causal = 1; p.out = c.out; p.o_stride = c.o_stride;
+  p.kv = c.kv; p.base_len = c.base_len;
   p.kv_splits = splits; p.part = c.part; p.counters = c.counters;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(qt, c.H, c.B * splits); cfg.blockDim = dim3(kAtThreads); cfg.stream = st;
+  cfg.gridDim = dim3(qt, c.kv.heads, c.B * splits); cfg.blockDim = dim3(kAtThreads); cfg.stream = st;
   cfg.dynamicSmemBytes = AttnTcCfg<128>::SMEM_BYTES;
   cudaLaunchAttribute attr[1];
   int na = 0;

@@ -508,56 +508,51 @@ int dp_unpack(const int32_t* recv, int n, int32_t* hist, int32_t* dp_step, cudaS
 // ------------------------------------------------------------------------------------------------
 // device-side KV page allocator
 // ------------------------------------------------------------------------------------------------
-__global__ void kv_reset_kernel(int32_t* __restrict__ kv_free, const int32_t* __restrict__ kv_order, int32_t* __restrict__ kv_state,
-                                int32_t* __restrict__ kv_npages, int total_pages, int max_batch) {
-  // stack top is the END of kv_free: page kv_order[0] must be popped first
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total_pages; i += gridDim.x * blockDim.x) kv_free[total_pages - 1 - i] = kv_order[i];
+__global__ void kv_reset_kernel(const KvCache kv, const int32_t* __restrict__ kv_order, int max_batch) {
+  // stack top is the END of the free stack: page kv_order[0] must be popped first
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < kv.total_pages; i += gridDim.x * blockDim.x) kv.free_stack[kv.total_pages - 1 - i] = kv_order[i];
   if (blockIdx.x == 0) {
-    for (int b = threadIdx.x; b < max_batch; b += blockDim.x) kv_npages[b] = 0;
-    if (threadIdx.x == 0) { kv_state[0] = total_pages; kv_state[1] = 0; }
+    for (int b = threadIdx.x; b < max_batch; b += blockDim.x) kv.npages[b] = 0;
+    if (threadIdx.x == 0) { kv.state[0] = kv.total_pages; kv.state[1] = 0; }
   }
 }
-int kv_reset(int32_t* kv_free, const int32_t* kv_order, int32_t* kv_state, int32_t* kv_npages, int total_pages, int max_batch, cudaStream_t st) {
-  int blocks = (total_pages + 255) / 256;
+int kv_reset(const KvCache& kv, const int32_t* kv_order, int max_batch, cudaStream_t st) {
+  int blocks = (kv.total_pages + 255) / 256;
   if (blocks > 64) blocks = 64;
   if (blocks < 1) blocks = 1;
-  kv_reset_kernel<<<blocks, 256, 0, st>>>(kv_free, kv_order, kv_state, kv_npages, total_pages, max_batch);
+  kv_reset_kernel<<<blocks, 256, 0, st>>>(kv, kv_order, max_batch);
   VCLA_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
 // One thread: for page rank p = 0,1,..: every sequence that needs a p-th page and does not own one yet pops the stack.
 // need[b] = pages for `tokens[b]` tokens, clamped to the table row.
-__device__ void kv_reserve_serial(int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq,
-                                  int page_tokens, int B, const int* s_tokens) {
-  int top = kv_state[0];
+__device__ void kv_reserve_serial(const KvCache& kv, int B, const int* s_tokens) {
+  int top = kv.state[0];
   bool more = true;
-  for (int p = 0; more && p < pages_per_seq; ++p) {
+  for (int p = 0; more && p < kv.pages_per_seq; ++p) {
     more = false;
     for (int b = 0; b < B; ++b) {
-      int need = (s_tokens[b] + page_tokens - 1) / page_tokens;
-      if (need > pages_per_seq) need = pages_per_seq;
+      const int need = kv.pages_for(s_tokens[b]);
       if (need > p + 1) more = true;
-      if (need > p && kv_npages[b] == p) {
-        if (top <= 0) { kv_state[1] = 1; continue; }          // pool exhausted (unreachable behind the host-side capacity check)
-        page_table[(size_t)b * pages_per_seq + p] = kv_free[--top];
-        kv_npages[b] = p + 1;
+      if (need > p && kv.npages[b] == p) {
+        if (top <= 0) { kv.state[1] = 1; continue; }          // pool exhausted (unreachable behind the host-side capacity check)
+        kv.seq_pages(b)[p] = kv.free_stack[--top];
+        kv.npages[b] = p + 1;
       }
     }
   }
-  kv_state[0] = top;
+  kv.state[0] = top;
 }
-__global__ void kv_reserve_kernel(int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq,
-                                  int page_tokens, int B, int S, const int32_t* __restrict__ left_pad, const int32_t* __restrict__ base_len) {
+__global__ void kv_reserve_kernel(const KvCache kv, int B, int S, const int32_t* __restrict__ left_pad, const int32_t* __restrict__ base_len) {
   __shared__ int s_tokens[64];
   if (threadIdx.x < B) s_tokens[threadIdx.x] = (base_len ? base_len[threadIdx.x] : 0) + S - (left_pad ? left_pad[threadIdx.x] : 0);
   __syncthreads();
-  if (threadIdx.x == 0) kv_reserve_serial(kv_free, kv_state, kv_npages, page_table, pages_per_seq, page_tokens, B, s_tokens);
+  if (threadIdx.x == 0) kv_reserve_serial(kv, B, s_tokens);
 }
-int kv_reserve(int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, int B, int S,
-               const int32_t* left_pad, cudaStream_t st, const int32_t* base_len) {
+int kv_reserve(const KvCache& kv, int B, int S, const int32_t* left_pad, cudaStream_t st, const int32_t* base_len) {
   if (B > 64) { set_error("kv_reserve: batch %d > 64", B); return -1; }
-  kv_reserve_kernel<<<1, 64, 0, st>>>(kv_free, kv_state, kv_npages, page_table, pages_per_seq, page_tokens, B, S, left_pad, base_len);
+  kv_reserve_kernel<<<1, 64, 0, st>>>(kv, B, S, left_pad, base_len);
   VCLA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -580,8 +575,7 @@ __device__ __forceinline__ void st_release_sys(int32_t* p, int32_t v) {
   asm volatile("st.release.sys.global.b32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
 }
 
-__global__ void advance_seq_kernel(int32_t* seq_len, int B, int by, const int32_t* __restrict__ left_pad, int32_t* step_idx, int32_t* kv_free,
-                                   int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens,
+__global__ void advance_seq_kernel(int32_t* seq_len, int B, int by, const int32_t* __restrict__ left_pad, int32_t* step_idx, const KvCache kv,
                                    StreamRing* ring, const int32_t* __restrict__ history) {
   __shared__ int s_tokens[64];
   __shared__ int s_step;
@@ -615,21 +609,15 @@ __global__ void advance_seq_kernel(int32_t* seq_len, int B, int by, const int32_
   if (threadIdx.x == 0) {
     // fast path (every step but one in page_tokens): nobody crosses a page boundary
     bool any = false;
-    for (int i = 0; i < B; ++i) {
-      int need = (s_tokens[i] + page_tokens - 1) / page_tokens;
-      if (need > pages_per_seq) need = pages_per_seq;
-      any |= need > kv_npages[i];
-    }
-    if (any) kv_reserve_serial(kv_free, kv_state, kv_npages, page_table, pages_per_seq, page_tokens, B, s_tokens);
+    for (int i = 0; i < B; ++i) any |= kv.pages_for(s_tokens[i]) > kv.npages[i];
+    if (any) kv_reserve_serial(kv, B, s_tokens);
   }
 }
-int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, int32_t* kv_free, int32_t* kv_state,
-                int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, cudaStream_t st, StreamRing* ring,
-                const int32_t* history) {
+int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, const KvCache& kv, cudaStream_t st,
+                StreamRing* ring, const int32_t* history) {
   if (B > 64) { set_error("advance_seq: batch %d > 64", B); return -1; }
   if (ring != nullptr && (history == nullptr || step_idx == nullptr)) { set_error("advance_seq: publishing needs the token history"); return -1; }
-  VCLA_LAUNCH(advance_seq_kernel, dim3(1), dim3(64), 0, st, seq_len, B, by, left_pad, step_idx, kv_free, kv_state, kv_npages, page_table,
-              pages_per_seq, page_tokens, ring, (const int32_t*)history);
+  VCLA_LAUNCH(advance_seq_kernel, dim3(1), dim3(64), 0, st, seq_len, B, by, left_pad, step_idx, kv, ring, (const int32_t*)history);
   return 0;
 }
 
@@ -671,10 +659,8 @@ __global__ void __launch_bounds__(256) lookup_accept_kernel(const LookupCall c, 
       done = produced >= max_new || fin;
     }
     // pages for the R rows the next step appends (idle steps after the end append there too, beyond seq_len)
-    int need = c.seq_len[0] + c.R;
-    int np = (need + c.page_tokens - 1) / c.page_tokens;
-    if (np > c.pages_per_seq) np = c.pages_per_seq;
-    if (np > c.kv_npages[0]) { int tokens[1] = {need}; kv_reserve_serial(c.kv_free, c.kv_state, c.kv_npages, c.page_table, c.pages_per_seq, c.page_tokens, 1, tokens); }
+    const int need = c.seq_len[0] + c.R;
+    if (c.kv.pages_for(need) > c.kv.npages[0]) { int tokens[1] = {need}; kv_reserve_serial(c.kv, 1, tokens); }
     s_done = done; s_prod = produced; s_best = 0x7fffffff;
   }
   __syncthreads();
@@ -727,19 +713,19 @@ int lookup_accept(const LookupCall& c, int prime, cudaStream_t st) {
 constexpr int kReorderThreads = 1024;
 __global__ void __launch_bounds__(kReorderThreads, 1)
 kv_beam_reorder_kernel(int rows_old, int rows_new, const int32_t* __restrict__ parent_row, const int32_t* __restrict__ new_tok, int32_t* seq_len,
-                       int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pps, int pt, int total_pages,
-                       int32_t* table_tmp, int32_t* history, const int32_t* __restrict__ step_idx, int32_t* copy_list,
-                       unsigned long long* cow_bytes, long long bytes_per_token) {
+                       const KvCache kv, int32_t* table_tmp, int32_t* history, const int32_t* __restrict__ step_idx, int32_t* copy_list,
+                       unsigned long long* cow_bytes) {
   extern __shared__ uint32_t s_mark[];
   __shared__ int s_np[64], s_len[64], s_par[64];
   TraceScope trace(17);
   trace.dep();
-  const int tid = threadIdx.x, words = (total_pages + 31) / 32;
-  if (tid < rows_old) { s_np[tid] = kv_npages[tid]; s_len[tid] = seq_len[tid]; }
+  const int pps = kv.pages_per_seq, pt = kv.page_tokens;
+  const int tid = threadIdx.x, words = (kv.total_pages + 31) / 32;
+  if (tid < rows_old) { s_np[tid] = kv.npages[tid]; s_len[tid] = seq_len[tid]; }
   if (tid < rows_new) s_par[tid] = parent_row[tid];
   for (int i = tid; i < words; i += kReorderThreads) s_mark[i] = 0u;
   __syncthreads();
-  for (int e = tid; e < rows_old * pps; e += kReorderThreads) if (e % pps < s_np[e / pps]) table_tmp[e] = page_table[e];
+  for (int e = tid; e < rows_old * pps; e += kReorderThreads) if (e % pps < s_np[e / pps]) table_tmp[e] = kv.table[e];
   __syncthreads();
   // mark every page a new row keeps
   for (int e = tid; e < rows_new * pps; e += kReorderThreads) {
@@ -749,37 +735,37 @@ kv_beam_reorder_kernel(int rows_old, int rows_new, const int32_t* __restrict__ p
   __syncthreads();
   if (tid == 0) {
     // release the unkept suffix of every old row (marking a released page stops a sibling that shares it from releasing it again)
-    int top = kv_state[0];
+    int top = kv.state[0];
     for (int k = 0; k < rows_old; ++k) {
       for (int i = s_np[k] - 1; i >= 0; --i) {
         const int pg = table_tmp[(size_t)k * pps + i];
         const uint32_t bit = 1u << (pg & 31);
         if (s_mark[pg >> 5] & bit) break;
         s_mark[pg >> 5] |= bit;
-        kv_free[top++] = pg;
+        kv.free_stack[top++] = pg;
       }
     }
-    kv_state[0] = top;
+    kv.state[0] = top;
   }
   __syncthreads();
   for (int e = tid; e < rows_new * pps; e += kReorderThreads) {
     const int j = e / pps, i = e % pps, p = s_par[j];
-    if (i < s_np[p]) page_table[e] = table_tmp[(size_t)p * pps + i];
+    if (i < s_np[p]) kv.table[e] = table_tmp[(size_t)p * pps + i];
   }
-  if (tid < rows_new) { kv_npages[tid] = s_np[s_par[tid]]; seq_len[tid] = s_len[s_par[tid]]; }
+  if (tid < rows_new) { kv.npages[tid] = s_np[s_par[tid]]; seq_len[tid] = s_len[s_par[tid]]; }
   __syncthreads();
   if (tid == 0) {
     // copy-on-write of the page the next token is written to: the first row continuing a parent keeps it, the others get a copy
-    int top = kv_state[0], n = 0;
+    int top = kv.state[0], n = 0;
     long long rows_copied = 0;
     uint64_t seen = 0;
     for (int j = 0; j < rows_new; ++j) {
       const int p = s_par[j], L = s_len[p], pw = L / pt;
       if (!((seen >> p) & 1ull)) { seen |= 1ull << p; continue; }
       if (pw >= s_np[p]) continue;                       // no page for a next token (the sequence is at its capacity)
-      if (top <= 0) { kv_state[1] = 1; continue; }       // pool exhausted (unreachable: distinct pages <= rows * pages_per_seq)
-      const int fresh = kv_free[--top];
-      page_table[(size_t)j * pps + pw] = fresh;
+      if (top <= 0) { kv.state[1] = 1; continue; }       // pool exhausted (unreachable: distinct pages <= rows * pages_per_seq)
+      const int fresh = kv.free_stack[--top];
+      kv.table[(size_t)j * pps + pw] = fresh;
       copy_list[1 + 3 * n] = table_tmp[(size_t)p * pps + pw];
       copy_list[2 + 3 * n] = fresh;
       copy_list[3 + 3 * n] = L % pt;
@@ -787,8 +773,8 @@ kv_beam_reorder_kernel(int rows_old, int rows_new, const int32_t* __restrict__ p
       ++n;
     }
     copy_list[0] = n;
-    kv_state[0] = top;
-    if (cow_bytes) *cow_bytes += (unsigned long long)(rows_copied * bytes_per_token);
+    kv.state[0] = top;
+    if (cow_bytes) *cow_bytes += (unsigned long long)(rows_copied * kv.layers * kv.planes() * 128 * (long long)sizeof(bf16));
   }
   // token history: columns gathered by parent, then this step's tokens as row t (one thread per history row: in place)
   const int t = *step_idx - 1;
@@ -800,43 +786,41 @@ kv_beam_reorder_kernel(int rows_old, int rows_new, const int32_t* __restrict__ p
   if (tid < rows_new) history[(size_t)t * rows_new + tid] = new_tok[tid];
   trace.done();
 }
-int kv_beam_reorder(int rows_old, int rows_new, const int32_t* parent_row, const int32_t* new_tok, int32_t* seq_len, int32_t* kv_free,
-                    int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, int total_pages,
+int kv_beam_reorder(int rows_old, int rows_new, const int32_t* parent_row, const int32_t* new_tok, int32_t* seq_len, const KvCache& kv,
                     int32_t* table_tmp, int32_t* history, const int32_t* step_idx, int32_t* copy_list, unsigned long long* cow_bytes,
-                    long long bytes_per_token, cudaStream_t st) {
+                    cudaStream_t st) {
   if (rows_old < 1 || rows_new < rows_old || rows_new > 64) { set_error("kv_beam_reorder: rows %d -> %d", rows_old, rows_new); return -1; }
-  const size_t smem = (size_t)((total_pages + 31) / 32) * 4;
-  if (smem > 200u * 1024u) { set_error("kv_beam_reorder: %d pages exceed the page bitmap", total_pages); return -1; }
+  const size_t smem = (size_t)((kv.total_pages + 31) / 32) * 4;
+  if (smem > 200u * 1024u) { set_error("kv_beam_reorder: %d pages exceed the page bitmap", kv.total_pages); return -1; }
   static bool opted_in = false;        // the first call is vcla_prefill's fork, outside any graph capture
   if (smem > 48u * 1024u && !opted_in) {
     VCLA_CUDA_OK(cudaFuncSetAttribute(kv_beam_reorder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     opted_in = true;
   }
-  kv_beam_reorder_kernel<<<1, kReorderThreads, smem, st>>>(rows_old, rows_new, parent_row, new_tok, seq_len, kv_free, kv_state, kv_npages, page_table,
-                                                            pages_per_seq, page_tokens, total_pages, table_tmp, history, step_idx, copy_list, cow_bytes,
-                                                            bytes_per_token);
+  kv_beam_reorder_kernel<<<1, kReorderThreads, smem, st>>>(rows_old, rows_new, parent_row, new_tok, seq_len, kv, table_tmp, history, step_idx,
+                                                            copy_list, cow_bytes);
   VCLA_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
-__global__ void kv_page_copy_kernel(bf16* kv_arena, size_t layer_elems, int heads, int pt, const int32_t* __restrict__ copy_list) {
+__global__ void kv_page_copy_kernel(const KvCache kv, const int32_t* __restrict__ copy_list) {
   TraceScope trace(18);
   trace.dep();
-  const int e = blockIdx.x, layer = blockIdx.y;
+  const int e = blockIdx.x;
   if (e >= copy_list[0]) return;
   const int src = copy_list[1 + 3 * e], dst = copy_list[2 + 3 * e], n = copy_list[3 + 3 * e];
-  const size_t page_elems = (size_t)2 * heads * pt * 128;
-  const uint4* s = reinterpret_cast<const uint4*>(kv_arena + layer * layer_elems + (size_t)src * page_elems);
-  uint4* d = reinterpret_cast<uint4*>(kv_arena + layer * layer_elems + (size_t)dst * page_elems);
-  const int per_plane = n * 16, plane_stride = pt * 16;           // 16 uint4 = one 128-wide bf16 row
-  for (int i = threadIdx.x; i < 2 * heads * per_plane; i += blockDim.x) {
+  const KvPool layer = kv.layer(blockIdx.y);
+  const uint4* s = reinterpret_cast<const uint4*>(layer.at(src, 0, 0, 0));
+  uint4* d = reinterpret_cast<uint4*>(layer.at(dst, 0, 0, 0));
+  const int per_plane = n * 16, plane_stride = kv.page_tokens * 16;   // 16 uint4 = one 128-wide bf16 row
+  for (int i = threadIdx.x; i < kv.planes() * per_plane; i += blockDim.x) {
     const int plane = i / per_plane, off = i % per_plane;
     d[(size_t)plane * plane_stride + off] = s[(size_t)plane * plane_stride + off];
   }
   trace.done();
 }
-int kv_page_copy(bf16* kv_arena, size_t layer_elems, int layers, int heads, int page_tokens, const int32_t* copy_list, int max_entries, cudaStream_t st) {
-  kv_page_copy_kernel<<<dim3(max_entries, layers), 256, 0, st>>>(kv_arena, layer_elems, heads, page_tokens, copy_list);
+int kv_page_copy(const KvCache& kv, const int32_t* copy_list, int max_entries, cudaStream_t st) {
+  kv_page_copy_kernel<<<dim3(max_entries, kv.layers), 256, 0, st>>>(kv, copy_list);
   VCLA_CUDA_OK(cudaGetLastError());
   return 0;
 }

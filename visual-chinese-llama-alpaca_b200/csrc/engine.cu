@@ -53,7 +53,6 @@ struct TextLayer {
   bf16 *wqkv, *wo, *wgu, *wd;                 // weight_format 0
   int8_t *qqkv, *qo, *qgu, *qd;               // weight_format 1: int8 rows (k in the decode kernel's fragment order, quant.cu) ...
   float *sqkv, *so, *sgu, *sd;                //                  ... and their fp32 scales
-  bf16* kv;  // this layer's pages
 };
 
 struct GraphKey {
@@ -83,7 +82,7 @@ struct vcla_ctx {
   // arenas
   uint8_t* w_arena = nullptr; size_t w_bytes = 0, w_off = 0;
   uint8_t* a_arena = nullptr; size_t a_bytes = 0, a_off = 0;
-  bf16* kv_arena = nullptr; size_t kv_bytes = 0;
+  size_t kv_bytes = 0;
   std::vector<Slot> slots;
   std::map<std::string, int> slot_index;
   // vision weights
@@ -96,13 +95,11 @@ struct vcla_ctx {
   // text
   bf16 *embed = nullptr, *lm_head = nullptr; float* final_norm = nullptr;
   std::vector<TextLayer> tl;
-  // kv cache
-  int pages_per_seq = 0, page_tokens = 64, total_pages = 0;
-  size_t kv_layer_elems = 0;
-  int32_t *page_table = nullptr, *seq_len = nullptr, *img_row_default = nullptr;
-  // device-side page allocator (elementwise.cu: kv_reset / kv_reserve / advance_seq): a stack of free physical pages, pages handed
-  // to sequences round-robin as they grow (so a sequence's pages are NOT contiguous), all stream-ordered and graph-capturable
-  int32_t *kv_free = nullptr, *kv_order = nullptr, *kv_state = nullptr, *kv_npages = nullptr;   // kv_state: [0] free count, [1] error flag
+  // kv cache: pages owned by the pool view (kv.pages is the arena of every layer) and handed to sequences round-robin as they grow by
+  // the device-side allocator (elementwise.cu: kv_reset / kv_reserve / advance_seq), so a sequence's pages are NOT contiguous; all
+  // stream-ordered and graph-capturable.  kv_order: the order in which a reset stacks the free pages.
+  KvCache kv;
+  int32_t *seq_len = nullptr, *img_row_default = nullptr, *kv_order = nullptr;
   // RoPE tables and argmax scratch are per context (another context may use another theta / device / stream)
   float *rope_cos = nullptr, *rope_sin = nullptr, *cand_val = nullptr; int32_t* cand_idx = nullptr;
   int attn_persistent_mode = 1, attn_persistent_grid = 0;
@@ -359,13 +356,13 @@ void layout_activations(vcla_ctx* c) {
   c->tok_hist = a_alloc<int32_t>(c, (size_t)(g.max_seq + 2) * Bp);
   c->step_idx = a_alloc<int32_t>(c, 16);
   c->d_ssq = a_alloc<float>(c, Bp * ((T + 127) / 128));
-  c->page_table = a_alloc<int32_t>(c, (size_t)g.max_batch * c->pages_per_seq);
+  c->kv.table = a_alloc<int32_t>(c, (size_t)g.max_batch * c->kv.pages_per_seq);
   c->seq_len = a_alloc<int32_t>(c, g.max_batch);
   c->img_row_default = a_alloc<int32_t>(c, g.max_batch);
-  c->kv_free = a_alloc<int32_t>(c, (size_t)c->total_pages);
-  c->kv_order = a_alloc<int32_t>(c, (size_t)c->total_pages);
-  c->kv_state = a_alloc<int32_t>(c, 4);
-  c->kv_npages = a_alloc<int32_t>(c, g.max_batch);
+  c->kv.free_stack = a_alloc<int32_t>(c, (size_t)c->kv.total_pages);
+  c->kv_order = a_alloc<int32_t>(c, (size_t)c->kv.total_pages);
+  c->kv.state = a_alloc<int32_t>(c, 4);
+  c->kv.npages = a_alloc<int32_t>(c, g.max_batch);
   c->rope_cos = a_alloc<float>(c, (size_t)(g.max_seq + 1) * 64);
   c->rope_sin = a_alloc<float>(c, (size_t)(g.max_seq + 1) * 64);
   c->cand_val = a_alloc<float>(c, Bp * kArgmaxChunks);
@@ -385,7 +382,7 @@ void layout_activations(vcla_ctx* c) {
   c->hyp_tmp = a_alloc<int32_t>(c, Bp * (size_t)g.max_seq);
   c->beam_state = a_alloc<int32_t>(c, Bp * 2);
   c->beam_copy = a_alloc<int32_t>(c, 1 + 3 * Bp);
-  c->beam_table_tmp = a_alloc<int32_t>(c, (size_t)g.max_batch * c->pages_per_seq);
+  c->beam_table_tmp = a_alloc<int32_t>(c, (size_t)g.max_batch * c->kv.pages_per_seq);
   c->beam_cow_bytes = a_alloc<unsigned long long>(c, 1);
   c->lk_prompt = a_alloc<int64_t>(c, (size_t)g.max_seq);
   c->lk_tok = a_alloc<int32_t>(c, 16);
@@ -528,9 +525,10 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   c->kpatch = 3 * g.v_patch * g.v_patch;
   c->kpad = (c->kpatch + 63) / 64 * 64;
   c->hd_t = 128;
-  c->page_tokens = g.page_tokens;
-  c->pages_per_seq = (g.max_seq + c->page_tokens - 1) / c->page_tokens;
-  c->total_pages = c->pages_per_seq * g.max_batch;
+  c->kv.heads = g.t_heads; c->kv.page_tokens = g.page_tokens; c->kv.layers = g.t_layers;
+  c->kv.pages_per_seq = (g.max_seq + g.page_tokens - 1) / g.page_tokens;
+  c->kv.total_pages = c->kv.pages_per_seq * g.max_batch;
+  c->kv.layer_elems = c->kv.row(c->kv.total_pages, 0, 0) * 128;
   c->sp_qkv = pick_splits(3 * g.t_hidden, g.t_hidden);
   c->sp_o = pick_splits(g.t_hidden, g.t_hidden);
   c->sp_gu = pick_splits(2 * g.t_ffn, g.t_hidden);
@@ -544,11 +542,10 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   // sizing passes
   layout_weights(c); c->w_bytes = c->w_off;
   layout_activations(c); c->a_bytes = c->a_off;
-  c->kv_layer_elems = (size_t)c->total_pages * 2 * g.t_heads * c->page_tokens * 128;
-  c->kv_bytes = c->kv_layer_elems * g.t_layers * sizeof(bf16);
+  c->kv_bytes = c->kv.layer_elems * g.t_layers * sizeof(bf16);
   cudaError_t e;
   if ((e = cudaMalloc(&c->w_arena, c->w_bytes)) != cudaSuccess || (e = cudaMalloc(&c->a_arena, c->a_bytes)) != cudaSuccess ||
-      (e = cudaMalloc(&c->kv_arena, c->kv_bytes)) != cudaSuccess) {
+      (e = cudaMalloc(&c->kv.pages, c->kv_bytes)) != cudaSuccess) {
     set_error("vcla_create: cudaMalloc failed (%s): weights %.2f GB, activations %.2f GB, kv %.2f GB", cudaGetErrorString(e),
               c->w_bytes / 1e9, c->a_bytes / 1e9, c->kv_bytes / 1e9);
     vcla_destroy(c);
@@ -558,9 +555,8 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   cudaMemset(c->a_arena, 0, c->a_bytes);
   layout_weights(c);
   layout_activations(c);
-  for (int i = 0; i < g.t_layers; ++i) c->tl[i].kv = c->kv_arena + (size_t)i * c->kv_layer_elems;
   // page allocation order: physical pages 0,1,2,... are handed out in this order after every reset (vcla_kv_debug_shuffle permutes it)
-  std::vector<int32_t> order((size_t)c->total_pages);
+  std::vector<int32_t> order((size_t)c->kv.total_pages);
   for (size_t i = 0; i < order.size(); ++i) order[i] = (int32_t)i;
   cudaMemcpy(c->kv_order, order.data(), order.size() * 4, cudaMemcpyHostToDevice);
   std::vector<int32_t> two(g.max_batch, 2);
@@ -578,7 +574,7 @@ void vcla_destroy(vcla_ctx* c) {
   drop_graphs(c);
   if (c->w_arena) cudaFree(c->w_arena);
   if (c->a_arena) cudaFree(c->a_arena);
-  if (c->kv_arena) cudaFree(c->kv_arena);
+  if (c->kv.pages) cudaFree(c->kv.pages);
   if (c->staging) cudaFree(c->staging);
   if (c->comm) { cudaDeviceSynchronize(); g_nccl.CommDestroy(c->comm); c->comm = nullptr; }
   if (c->dp_send) cudaFree(c->dp_send);
@@ -763,7 +759,7 @@ int vcla_reset(vcla_ctx* c, vcla_stream stream) {
   VCLA_CUDA_OK(cudaMemsetAsync(c->attn_counters, 0, (size_t)64 * c->cfg.t_heads * 4, (cudaStream_t)stream));
   VCLA_CUDA_OK(cudaMemsetAsync(c->step_idx, 0, 4, (cudaStream_t)stream));
   // every page back on the free stack, no sequence owns any
-  if (kv_reset(c->kv_free, c->kv_order, c->kv_state, c->kv_npages, c->total_pages, c->cfg.max_batch, (cudaStream_t)stream)) return -1;
+  if (kv_reset(c->kv, c->kv_order, c->cfg.max_batch, (cudaStream_t)stream)) return -1;
   if (c->dp_step) VCLA_CUDA_OK(cudaMemsetAsync(c->dp_step, 0, 4, (cudaStream_t)stream));
   VCLA_CUDA_OK(cudaMemsetAsync(c->finished, 0, 64 * 4, (cudaStream_t)stream));
   c->len_bound = 0;
@@ -787,7 +783,7 @@ int vcla_kv_truncate(vcla_ctx* c, const int32_t* len_host, int B, vcla_stream st
 
 int vcla_kv_debug_shuffle(vcla_ctx* c, uint32_t seed) {
   // test hook: permute the order in which physical pages are handed out (Fisher-Yates over an LCG); takes effect at the next reset
-  std::vector<int32_t> order((size_t)c->total_pages);
+  std::vector<int32_t> order((size_t)c->kv.total_pages);
   for (size_t i = 0; i < order.size(); ++i) order[i] = (int32_t)i;
   uint64_t x = 0x9E3779B97F4A7C15ull ^ seed;
   for (size_t i = order.size(); i > 1; --i) {
@@ -802,16 +798,16 @@ int vcla_kv_debug_shuffle(vcla_ctx* c, uint32_t seed) {
 int vcla_kv_read_pages(vcla_ctx* c, int32_t* table_host, int32_t* npages_host, int32_t* state_host) {
   // synchronous copy of the page table [max_batch][pages_per_seq], the per-sequence page counts and {free pages, error flag}
   VCLA_CUDA_OK(cudaDeviceSynchronize());
-  if (table_host) VCLA_CUDA_OK(cudaMemcpy(table_host, c->page_table, (size_t)c->cfg.max_batch * c->pages_per_seq * 4, cudaMemcpyDeviceToHost));
-  if (npages_host) VCLA_CUDA_OK(cudaMemcpy(npages_host, c->kv_npages, (size_t)c->cfg.max_batch * 4, cudaMemcpyDeviceToHost));
-  if (state_host) VCLA_CUDA_OK(cudaMemcpy(state_host, c->kv_state, 8, cudaMemcpyDeviceToHost));
+  if (table_host) VCLA_CUDA_OK(cudaMemcpy(table_host, c->kv.table, (size_t)c->cfg.max_batch * c->kv.pages_per_seq * 4, cudaMemcpyDeviceToHost));
+  if (npages_host) VCLA_CUDA_OK(cudaMemcpy(npages_host, c->kv.npages, (size_t)c->cfg.max_batch * 4, cudaMemcpyDeviceToHost));
+  if (state_host) VCLA_CUDA_OK(cudaMemcpy(state_host, c->kv.state, 8, cudaMemcpyDeviceToHost));
   return 0;
 }
 int vcla_kv_geometry(const vcla_ctx* c, int* pages_per_seq, int* total_pages, int* page_tokens) {
   if (!c) return -1;
-  if (pages_per_seq) *pages_per_seq = c->pages_per_seq;
-  if (total_pages) *total_pages = c->total_pages;
-  if (page_tokens) *page_tokens = c->page_tokens;
+  if (pages_per_seq) *pages_per_seq = c->kv.pages_per_seq;
+  if (total_pages) *total_pages = c->kv.total_pages;
+  if (page_tokens) *page_tokens = c->kv.page_tokens;
   return 0;
 }
 
@@ -942,14 +938,14 @@ static int csk_gemm(vcla_ctx* c, int which, int i, int B, cudaStream_t st) {
 }
 
 // Decode attention of layer L over the paged KV cache, reading the fused QKV projection from ws_qkv (qkv_splits partials).
-static DecodeAttnCall decode_attn_call(const vcla_ctx* c, const TextLayer& L, int B, int qkv_splits) {
+static DecodeAttnCall decode_attn_call(const vcla_ctx* c, int layer, int B, int qkv_splits) {
   const vcla_config& g = c->cfg;
-  DecodeAttnCall a; a.qkv_partial = c->ws_qkv; a.splits = qkv_splits; a.ws_rows = B; a.kv_pages = L.kv; a.page_table = c->page_table;
-  a.pages_per_seq = c->pages_per_seq; a.page_tokens = c->page_tokens; a.seq_len = c->seq_len; a.out = c->d_attn; a.scratch = c->attn_scratch;
-  a.counters = c->attn_counters; a.B = B; a.H = g.t_heads; a.HD = 128; a.scale = 1.0f / sqrtf(128.f); a.rope_theta = g.rope_theta;
+  DecodeAttnCall a; a.qkv_partial = c->ws_qkv; a.splits = qkv_splits; a.ws_rows = B; a.kv = c->kv.layer(layer);
+  a.seq_len = c->seq_len; a.out = c->d_attn; a.scratch = c->attn_scratch;
+  a.counters = c->attn_counters; a.B = B; a.HD = 128; a.scale = 1.0f / sqrtf(128.f); a.rope_theta = g.rope_theta;
   a.rope_cos = c->rope_cos; a.rope_sin = c->rope_sin; a.persistent_mode = c->attn_persistent_mode; a.persistent_grid = c->attn_persistent_grid;
   // enough CTAs to cover the SMs for small batches; long contexts split so a CTA streams <= ~12 pages
-  const int want = (num_sms() + B * a.H - 1) / (B * a.H);
+  const int want = (num_sms() + B * g.t_heads - 1) / (B * g.t_heads);
   a.kv_splits = std::min(8, std::max(want, c->kv_splits));
   return a;
 }
@@ -1057,8 +1053,8 @@ static int prefill_layers(vcla_ctx* c, int B, int S, const int32_t* left_pad, in
       GemmCall gc; if (weight(L.wqkv, L.qqkv, 3 * TH, TH, gc, L.sqkv)) return -1;
       gc.A = c->xn; gc.M = rows; gc.N = 3 * TH; gc.K = TH; gc.lda = TH; gc.ldb = TH; gc.mode = GEMM_STORE_BF16; gc.out = c->qkv; gc.ldo = 3 * TH;
       gc.rowscale = rsc;
-      gc.rope.cos = c->rope_cos; gc.rope.sin = c->rope_sin; gc.rope.kv_pages = L.kv; gc.rope.page_table = c->page_table; gc.rope.pages_per_seq = c->pages_per_seq;
-      gc.rope.page_tokens = c->page_tokens; gc.rope.S = S; gc.rope.T = TH; gc.rope.H = H; gc.rope.left_pad = left_pad; gc.rope.pos_from_mask = pos_from_mask;
+      gc.rope.cos = c->rope_cos; gc.rope.sin = c->rope_sin; gc.rope.kv = c->kv.layer(i);
+      gc.rope.S = S; gc.rope.T = TH; gc.rope.left_pad = left_pad; gc.rope.pos_from_mask = pos_from_mask;
       gc.rope.base_len = base_len;
       count(c); if (gemm_tc(gc, st)) return -1;
     }
@@ -1067,9 +1063,8 @@ static int prefill_layers(vcla_ctx* c, int B, int S, const int32_t* left_pad, in
       a.out = c->attn; a.o_stride = TH; a.B = B; a.H = H; a.Sq = S; a.HD = 128; a.scale = scale; a.causal = 1; a.kv_start = left_pad;
       count(c); if (attention_prefill(a, st)) return -1;
     } else {
-      AttnPagedCall a; a.q = c->qkv; a.q_stride = 3 * TH; a.kv_pages = L.kv; a.pool_pages = c->total_pages; a.page_table = c->page_table;
-      a.pages_per_seq = c->pages_per_seq; a.page_tokens = c->page_tokens; a.base_len = base_len; a.max_kv = (int)c->len_bound + S;
-      a.out = c->attn; a.o_stride = TH; a.B = B; a.H = H; a.T = S; a.scale = scale; a.part = c->pa_part; a.counters = c->pa_counters;
+      AttnPagedCall a; a.q = c->qkv; a.q_stride = 3 * TH; a.kv = c->kv.layer(i); a.base_len = base_len; a.max_kv = (int)c->len_bound + S;
+      a.out = c->attn; a.o_stride = TH; a.B = B; a.T = S; a.scale = scale; a.part = c->pa_part; a.counters = c->pa_counters;
       count(c); if (attention_paged(a, st)) return -1;
     }
     {
@@ -1136,7 +1131,7 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
   }
   if (vcla_reset(c, stream)) return -1;
   // pages for the prompt's tokens (real tokens only: left padding is never cached)
-  count(c); if (kv_reserve(c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, B, S, left_pad, st)) return -1;
+  count(c); if (kv_reserve(c->kv, B, S, left_pad, st)) return -1;
   count(c); if (embed_tokens(ids, B, T, S, TH, c->embed, g.t_vocab, image_mode == VCLA_IMAGE_AT_HEAD ? 1 : 0, nq, c->resid, st)) return -1;
   if (image_mode != VCLA_TEXT_ONLY) {
     const int32_t* rs = (image_mode == VCLA_IMAGE_AT_HEAD || img_row == nullptr) ? c->img_row_default : img_row;
@@ -1144,8 +1139,7 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
   }
   if (prefill_layers(c, B, S, left_pad, pos_from_mask, nullptr, st) || prefill_logits(c, B, S, logits_all, last_logits, next_tok, st)) return -1;
   // sequence lengths become S - pad; the page the first decoded token will be appended to is reserved here
-  count(c); if (advance_seq(c->seq_len, B, S, left_pad, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st,
-                            c->ring(), c->tok_hist)) return -1;
+  count(c); if (advance_seq(c->seq_len, B, S, left_pad, c->step_idx, c->kv, st, c->ring(), c->tok_hist)) return -1;
   if (c->beam_on && beam_reorder(c, B, B * c->beam_K, next_tok ? next_tok : c->d_tok, st)) return -1;
   c->len_bound = S;
   c->resident_b = c->beam_on ? B * c->beam_K : B;
@@ -1169,11 +1163,10 @@ int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* lo
   // like vcla_prefill: the token history, the step counter and the finished flags start over with this call's pick
   VCLA_CUDA_OK(cudaMemsetAsync(c->step_idx, 0, 4, st));
   VCLA_CUDA_OK(cudaMemsetAsync(c->finished, 0, 64 * 4, st));
-  count(c); if (kv_reserve(c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, B, T, nullptr, st, c->seq_len)) return -1;
+  count(c); if (kv_reserve(c->kv, B, T, nullptr, st, c->seq_len)) return -1;
   count(c); if (embed_tokens(ids, B, T, T, g.t_hidden, c->embed, g.t_vocab, 0, g.r_queries, c->resid, st)) return -1;
   if (prefill_layers(c, B, T, nullptr, 1, c->seq_len, st) || prefill_logits(c, B, T, logits_all, last_logits, next_tok, st)) return -1;
-  count(c); if (advance_seq(c->seq_len, B, T, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st,
-                            c->ring(), c->tok_hist)) return -1;
+  count(c); if (advance_seq(c->seq_len, B, T, nullptr, c->step_idx, c->kv, st, c->ring(), c->tok_hist)) return -1;
   c->len_bound += T;
   c->lk_primed = false;
   return stream_mark(c, st);
@@ -1182,13 +1175,11 @@ int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* lo
 // Beam search: rows_new rows continue the rows_old rows (beam_parent, written by the select kernel) with the tokens `tok`; then the
 // copy-on-write rows of the pages written next are copied for every layer.
 static int beam_reorder(vcla_ctx* c, int rows_old, int rows_new, const int32_t* tok, cudaStream_t st) {
-  const vcla_config& g = c->cfg;
-  const long long bytes_per_token = (long long)g.t_layers * 2 * g.t_heads * 128 * (long long)sizeof(bf16);
   count(c, 2);
-  if (kv_beam_reorder(rows_old, rows_new, c->beam_parent, tok, c->seq_len, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq,
-                      c->page_tokens, c->total_pages, c->beam_table_tmp, c->tok_hist, c->step_idx, c->beam_copy, c->beam_cow_bytes, bytes_per_token, st))
+  if (kv_beam_reorder(rows_old, rows_new, c->beam_parent, tok, c->seq_len, c->kv, c->beam_table_tmp, c->tok_hist, c->step_idx, c->beam_copy,
+                      c->beam_cow_bytes, st))
     return -1;
-  return kv_page_copy(c->kv_arena, c->kv_layer_elems, g.t_layers, g.t_heads, c->page_tokens, c->beam_copy, rows_new, st);
+  return kv_page_copy(c->kv, c->beam_copy, rows_new, st);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1239,7 +1230,7 @@ static int ws_stack(vcla_ctx* c, const int32_t* tok_in, int B, cudaStream_t st) 
     const TextLayer& L = c->tl[i];
     count(c); if (dec_resid_norm(i == 0 ? nullptr : c->ws_d, c->sp_d, B, c->d_resid, B, TH, L.ln1, g.t_eps, c->d_xn, st)) return -1;
     if (ws_gemm(c, DG_QKV, i, B, st)) return -1;
-    count(c); if (attention_decode(decode_attn_call(c, L, B, c->sp_qkv), st)) return -1;
+    count(c); if (attention_decode(decode_attn_call(c, i, B, c->sp_qkv), st)) return -1;
     if (ws_gemm(c, DG_O, i, B, st)) return -1;
     count(c); if (dec_resid_norm(c->ws_o, c->sp_o, B, c->d_resid, B, TH, L.ln2, g.t_eps, c->d_xn, st)) return -1;
     if (ws_gemm(c, DG_GATE_UP, i, B, st)) return -1;
@@ -1261,11 +1252,11 @@ static int csk_stack(vcla_ctx* c, const int32_t* tok_in, int B, bool lookup, cud
   for (int i = 0; i < g.t_layers; ++i) {
     if (csk_gemm(c, DG_QKV, i, B, st)) return -1;
     if (lookup) {
-      DecodeAttnCall a = decode_attn_call(c, c->tl[i], 1, 1);
+      DecodeAttnCall a = decode_attn_call(c, i, 1, 1);
       a.B = B; a.ws_rows = B;
       count(c, 2); if (attention_decode_lookup(a, st)) return -1;
     } else {
-      count(c); if (attention_decode(decode_attn_call(c, c->tl[i], B, 1), st)) return -1;
+      count(c); if (attention_decode(decode_attn_call(c, i, B, 1), st)) return -1;
     }
     if (csk_gemm(c, DG_O, i, B, st) || csk_gemm(c, DG_GATE_UP, i, B, st) || csk_gemm(c, DG_DOWN, i, B, st)) return -1;
   }
@@ -1287,8 +1278,7 @@ static LookupCall lookup_call(vcla_ctx* c) {
   LookupCall k; k.R = c->lk_rows; k.prompt = c->lk_prompt;
   k.tok = c->lk_tok; k.pick = c->lk_pick; k.history = c->tok_hist; k.step_idx = c->step_idx; k.seq_len = c->seq_len; k.finished = c->finished;
   k.samp = c->samp_on ? c->samp_params : nullptr; k.state = c->lk_state;
-  k.kv_free = c->kv_free; k.kv_state = c->kv_state; k.kv_npages = c->kv_npages; k.page_table = c->page_table;
-  k.pages_per_seq = c->pages_per_seq; k.page_tokens = c->page_tokens; k.ring = c->ring();
+  k.kv = c->kv; k.ring = c->ring();
   return k;
 }
 
@@ -1297,8 +1287,7 @@ static LookupCall lookup_call(vcla_ctx* c) {
 static int advance(vcla_ctx* c, int B, const int32_t* tok, bool lookup, cudaStream_t st) {
   count(c);
   if (lookup) return lookup_accept(lookup_call(c), 0, st);
-  if (advance_seq(c->seq_len, B, 1, nullptr, c->step_idx, c->kv_free, c->kv_state, c->kv_npages, c->page_table, c->pages_per_seq, c->page_tokens, st,
-                  c->ring(), c->tok_hist)) return -1;
+  if (advance_seq(c->seq_len, B, 1, nullptr, c->step_idx, c->kv, st, c->ring(), c->tok_hist)) return -1;
   return c->beam_on ? beam_reorder(c, B, B, tok, st) : 0;
 }
 
@@ -1942,7 +1931,7 @@ int vcla_debug_get_csk_splits(vcla_ctx* c, int B, int* out5) {
 int vcla_debug_decode_ctas_per_sm(vcla_ctx* c, int B, int* out2) {
   if (!c || !out2 || B < 1 || B > csk_max_batch(c)) { set_error("vcla_debug_decode_ctas_per_sm: bad arguments"); return -1; }
   out2[0] = gemm_csk_ctas_per_sm(B, c->cfg.weight_format == 1);
-  out2[1] = attention_decode_ctas_per_sm(decode_attn_call(c, c->tl[0], B, 1));
+  out2[1] = attention_decode_ctas_per_sm(decode_attn_call(c, 0, B, 1));
   return out2[0] > 0 && out2[1] > 0 ? 0 : -1;
 }
 int vcla_op_gemm_csk_clusters(int B, int splits) { return gemm_csk_clusters(B, splits); }
@@ -1954,6 +1943,35 @@ int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v
   a.B = B; a.H = H; a.Sq = Sq; a.HD = HD; a.scale = scale; a.causal = causal;
   return attention_prefill(a, (cudaStream_t)stream);
 }
+// Operator entries on a caller's pool: read back the page table [B][kv.pages_per_seq] and the lengths len_dev [B] (synchronising st) and
+// refuse, before any launch, a length below 0, a sequence whose len + rows tokens do not fit its table row, and a negative page among
+// the entries the launch reads.  Raises kv.total_pages to the pool extent (largest page read + 1).  -> the longest length, -1 if refused.
+static int op_check_pages(const char* who, KvPool& kv, const int32_t* len_dev, int B, int rows, cudaStream_t st) {
+  std::vector<int32_t> table((size_t)B * kv.pages_per_seq), len((size_t)B);
+  VCLA_CUDA_OK(cudaStreamSynchronize(st));
+  VCLA_CUDA_OK(cudaMemcpy(table.data(), kv.table, table.size() * 4, cudaMemcpyDeviceToHost));
+  VCLA_CUDA_OK(cudaMemcpy(len.data(), len_dev, len.size() * 4, cudaMemcpyDeviceToHost));
+  int longest = 0;
+  for (int b = 0; b < B; ++b) {
+    if (len[b] < 0 || (int64_t)len[b] + rows > (int64_t)kv.pages_per_seq * kv.page_tokens) {
+      set_error("%s: sequence %d (%d + %d tokens) exceeds its table row (%d pages of %d)", who, b, len[b], rows, kv.pages_per_seq, kv.page_tokens);
+      return -1;
+    }
+    for (int i = 0; i < kv.pages_for(len[b] + rows); ++i) {
+      const int32_t page = table[(size_t)b * kv.pages_per_seq + i];
+      if (page < 0) { set_error("%s: sequence %d has no page %d", who, b, i); return -1; }
+      kv.total_pages = std::max(kv.total_pages, page + 1);
+    }
+    longest = std::max(longest, len[b]);
+  }
+  return longest;
+}
+static KvPool op_pool(const void* pages, const int32_t* table, int pages_per_seq, int page_tokens, int heads) {
+  KvPool kv; kv.pages = (bf16*)pages; kv.table = const_cast<int32_t*>(table);
+  kv.heads = heads; kv.page_tokens = page_tokens; kv.pages_per_seq = pages_per_seq;
+  return kv;
+}
+
 int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, const int32_t* page_table, int pages_per_seq, int page_tokens,
                             const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T, float scale, vcla_stream stream) {
   // operator entry for tests: the pool extent and the longest sequence are read back from the caller's table and lengths, the
@@ -1962,24 +1980,15 @@ int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, c
     set_error("vcla_op_attention_paged: bad arguments"); return -1;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  std::vector<int32_t> table((size_t)B * pages_per_seq), len((size_t)B);
-  VCLA_CUDA_OK(cudaStreamSynchronize(st));
-  VCLA_CUDA_OK(cudaMemcpy(table.data(), page_table, table.size() * 4, cudaMemcpyDeviceToHost));
-  VCLA_CUDA_OK(cudaMemcpy(len.data(), base_len_dev, len.size() * 4, cudaMemcpyDeviceToHost));
-  int max_kv = 0; int64_t pool_pages = 0;
-  for (int b = 0; b < B; ++b) {
-    const int64_t kv = (int64_t)len[b] + T;
-    if (len[b] < 0 || kv > (int64_t)pages_per_seq * page_tokens) { set_error("vcla_op_attention_paged: sequence %d (%d + %d tokens) exceeds its table row", b, len[b], T); return -1; }
-    max_kv = std::max(max_kv, (int)kv);
-    for (int i = 0; i < (int)((kv + page_tokens - 1) / page_tokens); ++i) pool_pages = std::max<int64_t>(pool_pages, (int64_t)table[(size_t)b * pages_per_seq + i] + 1);
-  }
+  KvPool kv = op_pool(kv_pages, page_table, pages_per_seq, page_tokens, H);
+  const int longest = op_check_pages("vcla_op_attention_paged", kv, base_len_dev, B, T, st);
+  if (longest < 0) return -1;
   const int n = attention_paged_partials();
   void* scratch = nullptr;
   VCLA_CUDA_OK(cudaMalloc(&scratch, (size_t)n * kAttnPartialFloats * 4 + (size_t)n * 4));
   int32_t* counters = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(scratch) + (size_t)n * kAttnPartialFloats);
-  AttnPagedCall a; a.q = (const bf16*)q; a.q_stride = q_stride; a.kv_pages = (const bf16*)kv_pages; a.pool_pages = pool_pages; a.page_table = page_table;
-  a.pages_per_seq = pages_per_seq; a.page_tokens = page_tokens; a.base_len = base_len_dev; a.max_kv = max_kv; a.out = (bf16*)out; a.o_stride = o_stride;
-  a.B = B; a.H = H; a.T = T; a.scale = scale; a.part = reinterpret_cast<float*>(scratch); a.counters = counters;
+  AttnPagedCall a; a.q = (const bf16*)q; a.q_stride = q_stride; a.kv = kv; a.base_len = base_len_dev; a.max_kv = longest + T;
+  a.out = (bf16*)out; a.o_stride = o_stride; a.B = B; a.T = T; a.scale = scale; a.part = reinterpret_cast<float*>(scratch); a.counters = counters;
   int rc = cudaMemsetAsync(counters, 0, (size_t)n * 4, st) == cudaSuccess ? attention_paged(a, st) : -1;
   if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_attention_paged: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
   cudaFree(scratch);
@@ -1998,25 +2007,14 @@ int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_page
   if (persistent != 0 && persistent != 1) { set_error("vcla_op_attention_decode: persistent must be 0 or 1"); return -1; }
   if (persistent && kv_splits != 1) { set_error("vcla_op_attention_decode: the persistent kernel requires kv_splits == 1 (got %d)", kv_splits); return -1; }
   cudaStream_t st = (cudaStream_t)stream;
-  std::vector<int32_t> table((size_t)B * pages_per_seq), len((size_t)B);
-  VCLA_CUDA_OK(cudaStreamSynchronize(st));
-  VCLA_CUDA_OK(cudaMemcpy(table.data(), page_table, table.size() * 4, cudaMemcpyDeviceToHost));
-  VCLA_CUDA_OK(cudaMemcpy(len.data(), seq_len_dev, len.size() * 4, cudaMemcpyDeviceToHost));
-  int max_len = 0;
-  for (int b = 0; b < B; ++b) {
-    if (len[b] < 0 || (int64_t)len[b] + 1 > (int64_t)pages_per_seq * page_tokens) {
-      set_error("vcla_op_attention_decode: sequence %d (%d + 1 tokens) exceeds its table row (%d pages of %d)", b, len[b], pages_per_seq, page_tokens); return -1;
-    }
-    for (int i = 0; i <= len[b] / page_tokens; ++i) {
-      if (table[(size_t)b * pages_per_seq + i] < 0) { set_error("vcla_op_attention_decode: sequence %d has no page %d", b, i); return -1; }
-    }
-    max_len = std::max(max_len, len[b]);
-  }
+  KvPool kv = op_pool(kv_pages, page_table, pages_per_seq, page_tokens, H);
+  const int max_len = op_check_pages("vcla_op_attention_decode", kv, seq_len_dev, B, 1, st);
+  if (max_len < 0) return -1;
   const size_t rope_floats = (size_t)(max_len + 1) * 64, scratch_floats = (size_t)B * H * kv_splits * (128 + 2);
   float* buf = nullptr;
   VCLA_CUDA_OK(cudaMalloc(&buf, (2 * rope_floats + scratch_floats + (size_t)B * H) * 4));
-  DecodeAttnCall a; a.qkv_partial = qkv_partial; a.splits = splits; a.ws_rows = B; a.kv_pages = (bf16*)kv_pages; a.page_table = page_table;
-  a.pages_per_seq = pages_per_seq; a.page_tokens = page_tokens; a.seq_len = seq_len_dev; a.out = (bf16*)out; a.B = B; a.H = H; a.HD = 128;
+  DecodeAttnCall a; a.qkv_partial = qkv_partial; a.splits = splits; a.ws_rows = B; a.kv = kv;
+  a.seq_len = seq_len_dev; a.out = (bf16*)out; a.B = B; a.HD = 128;
   a.kv_splits = kv_splits; a.scale = scale; a.rope_theta = rope_theta; a.rope_cos = buf; a.rope_sin = buf + rope_floats;
   a.scratch = buf + 2 * rope_floats; a.counters = reinterpret_cast<int32_t*>(a.scratch + scratch_floats);
   a.persistent_mode = persistent ? 2 : 0; a.persistent_grid = persistent_grid;
@@ -2042,22 +2040,14 @@ int vcla_op_attention_decode_lookup(const float* qkv_partial, int splits, void* 
   }
   if (kv_splits < 1 || kv_splits > 8) { set_error("vcla_op_attention_decode_lookup: kv_splits %d outside 1..8", kv_splits); return -1; }
   cudaStream_t st = (cudaStream_t)stream;
-  std::vector<int32_t> table((size_t)pages_per_seq);
-  int32_t len = 0;
-  VCLA_CUDA_OK(cudaStreamSynchronize(st));
-  VCLA_CUDA_OK(cudaMemcpy(table.data(), page_table, table.size() * 4, cudaMemcpyDeviceToHost));
-  VCLA_CUDA_OK(cudaMemcpy(&len, seq_len_dev, 4, cudaMemcpyDeviceToHost));
-  if (len < 0 || (int64_t)len + rows > (int64_t)pages_per_seq * page_tokens) {
-    set_error("vcla_op_attention_decode_lookup: %d + %d tokens exceed the table row (%d pages of %d)", len, rows, pages_per_seq, page_tokens); return -1;
-  }
-  for (int i = 0; i <= (len + rows - 1) / page_tokens; ++i) {
-    if (table[i] < 0) { set_error("vcla_op_attention_decode_lookup: no page %d", i); return -1; }
-  }
+  KvPool kv = op_pool(kv_pages, page_table, pages_per_seq, page_tokens, H);
+  const int len = op_check_pages("vcla_op_attention_decode_lookup", kv, seq_len_dev, 1, rows, st);
+  if (len < 0) return -1;
   const size_t rope_floats = (size_t)(len + rows) * 64, scratch_floats = (size_t)rows * H * kv_splits * (128 + 2);
   float* buf = nullptr;
   VCLA_CUDA_OK(cudaMalloc(&buf, (2 * rope_floats + scratch_floats + (size_t)rows * H) * 4));
-  DecodeAttnCall a; a.qkv_partial = qkv_partial; a.splits = splits; a.ws_rows = rows; a.kv_pages = (bf16*)kv_pages; a.page_table = page_table;
-  a.pages_per_seq = pages_per_seq; a.page_tokens = page_tokens; a.seq_len = seq_len_dev; a.out = (bf16*)out; a.B = rows; a.H = H; a.HD = 128;
+  DecodeAttnCall a; a.qkv_partial = qkv_partial; a.splits = splits; a.ws_rows = rows; a.kv = kv;
+  a.seq_len = seq_len_dev; a.out = (bf16*)out; a.B = rows; a.HD = 128;
   a.kv_splits = kv_splits; a.scale = scale; a.rope_theta = rope_theta; a.rope_cos = buf; a.rope_sin = buf + rope_floats;
   a.scratch = buf + 2 * rope_floats; a.counters = reinterpret_cast<int32_t*>(a.scratch + scratch_floats);
   int rc = rope_fill_tables(len + rows, 128, rope_theta, buf, buf + rope_floats);

@@ -304,7 +304,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                   const bool cached = cpos >= 0;                           // padding rows are neither rotated nor cached
                   const int pos = R.base_len != nullptr ? cpos : (R.pos_from_mask ? (cpos > 0 ? cpos : 0) : sq);
                   int page = 0, slot = 0;
-                  if (cached) { page = __ldg(R.page_table + (size_t)bq * R.pages_per_seq + cpos / R.page_tokens); slot = cpos % R.page_tokens; }
+                  if (cached) { page = __ldg(R.kv.seq_pages(bq) + cpos / R.kv.page_tokens); slot = cpos % R.kv.page_tokens; }
                   const float* ct = R.cos + (size_t)pos * 64;
                   const float* stb = R.sin + (size_t)pos * 64;
                   bf16* orow_ptr = reinterpret_cast<bf16*>(p.out) + (size_t)orow * p.ldo;
@@ -313,7 +313,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     const int hcol = col_tile + hh * 128;                  // first column of this head inside [q | k | v]
                     if (hcol < p.N) {
                       const int region = hcol / R.T, head = (hcol % R.T) / 128;
-                      bf16* cdst = (region >= 1 && cached) ? R.kv_pages + ((((size_t)page * 2 + (region - 1)) * R.H + head) * R.page_tokens + slot) * 128 : nullptr;
+                      bf16* cdst = (region >= 1 && cached) ? R.kv.at(page, region - 1, head, slot) : nullptr;
 #pragma unroll
                       for (int jj = 0; jj < 8; ++jj) {                     // dims d = 8 jj + fc (+1) pair with d + 64 (HF rotate_half)
                         const int d = 8 * jj + fc;

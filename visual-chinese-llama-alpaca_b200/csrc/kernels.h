@@ -37,6 +37,41 @@ enum GemmMode {
 };
 enum Act { ACT_NONE = 0, ACT_QUICK_GELU = 1, ACT_GELU_ERF = 2 };
 
+// ---- paged KV cache ------------------------------------------------------------------------------------------------------
+// One view of a layer's cache: its page pool and the page table.  The pool holds [total_pages][K|V][heads][page_tokens][128] bf16, so
+// every (page, K|V, head) plane is page_tokens contiguous 128-wide rows.  Sequence b's i-th page is table[b][i]: its token t sits in
+// slot t % page_tokens of page table[b][t / page_tokens].  This struct is the only place that knows the layout.  It is a field of the
+// decode and prefill attention parameter blocks: keep it at 32 bytes, larger blocks change how those kernels are compiled.
+struct KvPool {
+  bf16* pages = nullptr;
+  int32_t* table = nullptr;          // [sequences][pages_per_seq]
+  int heads = 0, page_tokens = 0, pages_per_seq = 0, total_pages = 0;
+
+  // 128-element row of (page, K|V, head, slot) from the start of the pool: I = int for TMA coordinates, size_t for addresses
+  template <typename I = size_t>
+  __host__ __device__ __forceinline__ I row(int page, int kv, int head, int slot = 0) const {
+    return (((I)page * 2 + kv) * heads + head) * page_tokens + slot;
+  }
+  __host__ __device__ __forceinline__ bf16* at(int page, int kv, int head, int slot) const { return pages + row(page, kv, head, slot) * 128; }
+  __host__ __device__ __forceinline__ int planes() const { return 2 * heads; }   // (K|V, head) planes of a page
+  __host__ __device__ __forceinline__ int32_t* seq_pages(int b) const { return table + (size_t)b * pages_per_seq; }
+  // pages that hold n tokens, clamped to a table row
+  __host__ __device__ __forceinline__ int pages_for(int n) const {
+    const int p = (n + page_tokens - 1) / page_tokens;
+    return p > pages_per_seq ? pages_per_seq : p;
+  }
+};
+// The cache of every layer (pages is layer 0; the layers share the table) with the state of the device page allocator
+// (elementwise.cu), which hands pages to sequences as they grow.
+struct KvCache : KvPool {
+  int32_t* free_stack = nullptr;     // [total_pages] free physical pages; the top is free_stack[state[0] - 1]
+  int32_t* state = nullptr;          // {free pages, exhausted flag}
+  int32_t* npages = nullptr;         // [sequences] pages owned: table[b][0 .. npages[b])
+  int layers = 1;
+  size_t layer_elems = 0;            // = row(total_pages, 0, 0) * 128, set with the geometry
+  __host__ __device__ __forceinline__ KvPool layer(int i) const { KvPool v = *this; v.pages += i * layer_elems; return v; }
+};
+
 // ---- prefill epilogue fusions (non-swap GEMMs) --------------------------------------------------------------------------
 // Deferred RMSNorm: the A operand holds xw = bf16(resid * norm_w) (NOT normalised); the row scale rstd[row] =
 // rsqrt(sum_slots ssq[row][slot] / dim + eps) commutes with the GEMM and is applied to the accumulator in the epilogue.
@@ -56,8 +91,8 @@ struct GemmEmitNorm {
 // [pos][64]) on the fp32 accumulator, store q|k|v rows (the prefill attention reads them) AND append k, v to the paged KV cache.
 struct GemmRope {
   const float* cos = nullptr; const float* sin = nullptr;
-  bf16* kv_pages = nullptr; const int32_t* page_table = nullptr; int pages_per_seq = 0, page_tokens = 0;
-  int S = 0, T = 0, H = 0;                     // rows per sequence, hidden size (= H * 128), heads
+  KvPool kv;                                   // the layer's view; kv.heads heads
+  int S = 0, T = 0;                            // rows per sequence, hidden size (= kv.heads * 128)
   const int32_t* left_pad = nullptr; int pos_from_mask = 0;
   const int32_t* base_len = nullptr;           // [B] or null: row t of sequence b is token base_len[b] + t (position and cache slot)
 };
@@ -145,18 +180,16 @@ void attention_set_tc(int mode);                                 // 0: mma.sync 
 int trace_set_attention_tc(void* buf, unsigned long long cap);
 
 // Causal prefill of a chunk of T new rows per sequence over its cached prefix (head dim 128, wgmma kernel of attention_tc.cu):
-// queries q[(b*T + t)*q_stride + h*128 + d]; keys / values = the first base_len[b] + T tokens of sequence b in the layer's page
-// pool kv_pages [pool_pages][2][H][page_tokens][128], read through page_table [b][pages_per_seq] with TMA; key j is visible to row
-// t iff j <= base_len[b] + t.  max_kv (an upper bound of base_len + T) and the grid size choose the split-KV factor; a split launch
+// queries q[(b*T + t)*q_stride + h*128 + d]; keys / values = the first base_len[b] + T tokens of sequence b in the layer view kv
+// (kv.total_pages pages, kv.heads heads), read with TMA; key j is visible to row t iff j <= base_len[b] + t.  max_kv (an upper bound of base_len + T) and the grid size choose the split-KV factor; a split launch
 // needs part (attention_paged_partials() x 64 x 132 floats) and counters (attention_paged_partials() int32, zeroed once).
 struct AttnPagedCall {
   const bf16* q = nullptr; int q_stride = 0;
-  const bf16* kv_pages = nullptr; int64_t pool_pages = 0;
-  const int32_t* page_table = nullptr; int pages_per_seq = 0, page_tokens = 0;
+  KvPool kv;
   const int32_t* base_len = nullptr;
   int max_kv = 0;
   bf16* out = nullptr; int o_stride = 0;
-  int B = 0, H = 0, T = 0;
+  int B = 0, T = 0;
   float scale = 1.f;
   float* part = nullptr; int32_t* counters = nullptr;
 };
@@ -167,19 +200,17 @@ constexpr int kAttnPartialFloats = 64 * 132;
 struct DecodeAttnCall {
   const float* qkv_partial = nullptr;  // [splits][ws_rows][3*T] fp32 split-K partials of the fused QKV projection
   int splits = 1, ws_rows = 0;
-  bf16* kv_pages = nullptr;            // this layer: [pages][2][H][page_tokens][HD]
-  const int32_t* page_table = nullptr; // [max_batch][pages_per_seq]
-  int pages_per_seq = 0, page_tokens = 0;
   const int32_t* seq_len = nullptr;    // [B] tokens already in the cache (the new token is appended at this index)
   bf16* out = nullptr;                 // [ws_rows][T] attention output (bf16, GEMM operand of o_proj)
   float* scratch = nullptr;            // [B][H][kv_splits][HD+2]
   int32_t* counters = nullptr;         // [B][H]
-  int B = 0, H = 0, HD = 0, kv_splits = 1;
+  int B = 0, HD = 0, kv_splits = 1;
   float scale = 1.f, rope_theta = 10000.f;
   const float* rope_cos = nullptr;     // [max_pos][HD/2] fp32 tables owned by the context
   const float* rope_sin = nullptr;
   int persistent_mode = 1;             // VCLA_ATTN_PERSISTENT (read once per context)
   int persistent_grid = 0;             // VCLA_ATTN_PERSISTENT_GRID
+  KvPool kv;                           // this layer's view (kv.heads heads of HD = 128)
 };
 int attention_decode(const DecodeAttnCall& c, cudaStream_t st);
 // Prompt lookup verification over c.B <= 16 query rows of sequence 0 (row r at position seq_len[0] + r, qkv / out row r): two launches,
@@ -276,16 +307,13 @@ int trace_set_beam(void* buf, unsigned long long cap);
 // ssq[b][0] = sum resid^2, ssq[b][1..slots) = 0 (head of the deferred-norm chain)
 int dec_embed(const int32_t* ids, int B, int D, const bf16* table, int vocab, float* resid, const float* norm_w,
               bf16* xw, float* ssq, int slots, cudaStream_t st);
-// ---- device-side KV page allocator (stream-ordered, graph-capturable; one thread walks the <= 64 sequences, so the
+// ---- device-side KV page allocator over a KvCache (stream-ordered, graph-capturable; one thread walks the <= 64 sequences, so the
 //      assignment is deterministic) ------------------------------------------------------------------------------
-// kv_state[0] = free pages, kv_state[1] = error flag (pool exhausted); kv_free = stack of free physical pages;
-// kv_npages[b] = pages owned by sequence b; page_table[b][i] = i-th page of sequence b.
-int kv_reset(int32_t* kv_free, const int32_t* kv_order, int32_t* kv_state, int32_t* kv_npages, int total_pages, int max_batch,
-             cudaStream_t st);
+// every page back on the free stack (kv_order[0] popped first), no sequence of max_batch owns any
+int kv_reset(const KvCache& kv, const int32_t* kv_order, int max_batch, cudaStream_t st);
 // make sure sequence b owns pages for (S - left_pad[b]) tokens, b < B; pages are handed out round-robin over the sequences
 // (base_len non-null: make sure sequence b owns pages for base_len[b] + S tokens -- a chunk appended to cached tokens)
-int kv_reserve(int32_t* kv_free, int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens,
-               int B, int S, const int32_t* left_pad, cudaStream_t st, const int32_t* base_len = nullptr);
+int kv_reserve(const KvCache& kv, int B, int S, const int32_t* left_pad, cudaStream_t st, const int32_t* base_len = nullptr);
 // seq_len[b] = min(seq_len[b], len[b]) for b < B <= 64 (the pages stay owned)
 int kv_truncate(int32_t* seq_len, const int32_t* len_host, int B, cudaStream_t st);
 // Token stream ring (vcla_stream_*): pinned, mapped host memory the device writes and the host polls.  tokens[L][b] = token of
@@ -301,8 +329,7 @@ inline size_t stream_ring_bytes(int rows) { return offsetof(StreamRing, tokens) 
 // seq_len[b] += by - left_pad[b] ; *step_idx += 1 ; then reserve the page the NEXT token of every sequence will be appended to.
 // ring (nullable, device view of the mapped ring): first publish step L = *step_idx -- history row L ([L][B]) into ring row L, a
 // system-scope fence per writer, then ring->published = L + 1 with st.release.sys.  ring == nullptr executes none of it.
-int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, int32_t* kv_free, int32_t* kv_state,
-                int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, cudaStream_t st,
+int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, const KvCache& kv, cudaStream_t st,
                 StreamRing* ring = nullptr, const int32_t* history = nullptr);
 // ---- prompt lookup decoding (one sequence): a verification step runs R = k + 1 rows -- the last emitted token and k drafts -- through
 // the decode step; lookup_accept then replaces advance_seq.  Restates HF:generation/utils.py:3603-3620 (_assisted_decoding, greedy
@@ -322,7 +349,7 @@ struct LookupCall {
   int32_t* history = nullptr; int32_t* step_idx = nullptr; int32_t* seq_len = nullptr; int32_t* finished = nullptr;
   const SamplerParams* samp = nullptr;          // nullable: the EOS ids
   LookupState* state = nullptr;
-  int32_t *kv_free = nullptr, *kv_state = nullptr, *kv_npages = nullptr, *page_table = nullptr; int pages_per_seq = 0, page_tokens = 0;
+  KvCache kv;                                   // pages for the next step's rows
   StreamRing* ring = nullptr;                   // nullable: publish the emitted tokens (as advance_seq does)
 };
 // prime != 0: no acceptance (right after the prefill): reserve pages for R rows and draft the first step.  Otherwise, unless the row is
@@ -337,14 +364,12 @@ int lookup_accept(const LookupCall& c, int prime, cudaStream_t st);
 // copy-list entry {src page, dst page, rows [0, seq_len % page_tokens)} (copy_list[0] = count, then 3 ints per entry).  The token
 // history [t][rows_old] (t = *step_idx - 1) is gathered into [t][rows_new] and new_tok is appended as its row t.  One CTA; the stack
 // operations are serial, so the result is deterministic.  Scratch: table_tmp [rows_old][pages_per_seq], mark (total_pages / 32 words
-// of dynamic shared memory).  cow_bytes (nullable) accumulates copied rows * bytes_per_token.
-int kv_beam_reorder(int rows_old, int rows_new, const int32_t* parent_row, const int32_t* new_tok, int32_t* seq_len, int32_t* kv_free,
-                    int32_t* kv_state, int32_t* kv_npages, int32_t* page_table, int pages_per_seq, int page_tokens, int total_pages,
+// of dynamic shared memory).  cow_bytes (nullable) accumulates the bytes of the copied rows over every layer.
+int kv_beam_reorder(int rows_old, int rows_new, const int32_t* parent_row, const int32_t* new_tok, int32_t* seq_len, const KvCache& kv,
                     int32_t* table_tmp, int32_t* history, const int32_t* step_idx, int32_t* copy_list, unsigned long long* cow_bytes,
-                    long long bytes_per_token, cudaStream_t st);
+                    cudaStream_t st);
 // copies the copy list's rows of every layer (K and V, every head) from src to dst page; fixed grid (max_entries x layers)
-int kv_page_copy(bf16* kv_arena, size_t layer_elems, int layers, int heads, int page_tokens, const int32_t* copy_list, int max_entries,
-                 cudaStream_t st);
+int kv_page_copy(const KvCache& kv, const int32_t* copy_list, int max_entries, cudaStream_t st);
 // fp32 RoPE tables [max_pos][head_dim/2], computed on the host the way HF does and uploaded to cos_dev / sin_dev
 int rope_fill_tables(int max_pos, int head_dim, float theta, float* cos_dev, float* sin_dev);
 
