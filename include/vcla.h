@@ -279,6 +279,18 @@ typedef struct {
   int min_new_tokens;
 } vcla_beam;
 int vcla_set_beam(vcla_ctx* ctx, const vcla_beam* beam_or_null);
+/* ---- fan-out: n sampled replies per prompt from one prefill (HF generate(do_sample=True, num_return_sequences=n)) ------------------
+ * With n > 1 set, vcla_prefill prefills each of its B prompts once and forks prompt b to rows b * n .. b * n + n - 1 (the order of HF's
+ * repeat_interleave) through the beam search page-table reorder: the rows share every full page of the prompt, and every row but the
+ * first of a prompt gets its own copy of the partly filled page it writes next (vcla_beam_cow_bytes counts those rows).  The first pick
+ * is the sampler's over B * n rows, row r scoring the last logits of prompt r / n with its own draw counter (0, r) -- so siblings draw
+ * independently and a row's draw and processed scores are exactly those of an unforked row r with the same logits; without a sampler
+ * each row takes its prompt's argmax.  next_tok_dev (if not NULL) receives the B * n picks and last_logits_dev stays (B, V); the token
+ * history, the finished flags, the sequence lengths and the page table then describe B * n resident rows, which vcla_decode_step /
+ * vcla_decode_multi step like a batch, and an armed token stream receives the B * n picks as the prefill's step.  n = 1: off (the
+ * default).  Refused by vcla_prefill: B * n > min(max_batch, 64), beam mode, the data-parallel exchange.  vcla_prefill_extend is refused
+ * in fan-out mode and while forked rows are resident (until the next vcla_prefill or vcla_reset). */
+int vcla_set_fanout(vcla_ctx* ctx, int n);
 int vcla_read_beams(vcla_ctx* ctx, int32_t* tokens_host, int32_t* lengths_host, float* scores_host, int32_t* done_host);
 int vcla_beam_cow_bytes(vcla_ctx* ctx, int64_t* bytes, int reset);
 int vcla_op_beam_step(const float* logits_dev, int B, int V, const int32_t* history_dev, int t, const vcla_beam* beam, float* run_scores_dev,
@@ -422,7 +434,7 @@ int vcla_bench_decode_gemm(vcla_ctx* ctx, int which, int B, int reps, float* avg
 /* Timeline trace for profiles/: when enabled, CTA (0,0,0) of every kernel appends {tag, t_entry, t_dependency_resolved, t_exit}
  * (%globaltimer, ns).  Tags: 1 swap-AB GEMM, 2 GEMM, 3 prefill attention, 4 decode attention, 5 layernorm, 6 rmsnorm, 7 rope+cache,
  * 8 resid+rmsnorm, 9 silu*mul, 10/11 logits+argmax, 12 advance, 13 embed, 14 sampler, 15 beam step, 16 beam select, 17 beam page
- * reorder, 18 beam page copy.  vcla_trace_read synchronises and clears. */
+ * reorder, 18 beam page copy, 21 fan-out row map.  vcla_trace_read synchronises and clears. */
 int vcla_trace_enable(vcla_ctx* ctx, int max_events);
 int vcla_trace_read(vcla_ctx* ctx, uint64_t* dst_host, int max_events, int* n_events);
 /* enable/disable programmatic dependent launch for subsequently enqueued kernels (process-wide) */

@@ -576,7 +576,7 @@ __device__ __forceinline__ void st_release_sys(int32_t* p, int32_t v) {
 }
 
 __global__ void advance_seq_kernel(int32_t* seq_len, int B, int by, const int32_t* __restrict__ left_pad, int32_t* step_idx, const KvCache kv,
-                                   StreamRing* ring, const int32_t* __restrict__ history) {
+                                   StreamRing* ring, const int32_t* __restrict__ history, int publish_rows) {
   __shared__ int s_tokens[64];
   __shared__ int s_step;
   TraceScope trace(12);
@@ -599,8 +599,8 @@ __global__ void advance_seq_kernel(int32_t* seq_len, int B, int by, const int32_
     // publish: tokens into the host ring, each writer's stores made visible system-wide, then one release store of the count.
     // The ring has as many rows as the history (max_seq + 2), so any step whose history row exists has a ring row.
     const int step = s_step;
-    if (b < B) {
-      ring->tokens[(size_t)step * 64 + b] = history[(size_t)step * B + b];
+    if (b < publish_rows) {
+      ring->tokens[(size_t)step * 64 + b] = history[(size_t)step * publish_rows + b];
       __threadfence_system();
     }
     __syncthreads();
@@ -614,10 +614,33 @@ __global__ void advance_seq_kernel(int32_t* seq_len, int B, int by, const int32_
   }
 }
 int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, const KvCache& kv, cudaStream_t st,
-                StreamRing* ring, const int32_t* history) {
-  if (B > 64) { set_error("advance_seq: batch %d > 64", B); return -1; }
+                StreamRing* ring, const int32_t* history, int publish_rows) {
+  if (publish_rows <= 0) publish_rows = B;
+  if (B > 64 || publish_rows > 64) { set_error("advance_seq: batch %d (%d published) > 64", B, publish_rows); return -1; }
   if (ring != nullptr && (history == nullptr || step_idx == nullptr)) { set_error("advance_seq: publishing needs the token history"); return -1; }
-  VCLA_LAUNCH(advance_seq_kernel, dim3(1), dim3(64), 0, st, seq_len, B, by, left_pad, step_idx, kv, ring, (const int32_t*)history);
+  VCLA_LAUNCH(advance_seq_kernel, dim3(1), dim3(64), 0, st, seq_len, B, by, left_pad, step_idx, kv, ring, (const int32_t*)history, publish_rows);
+  return 0;
+}
+
+// ---- fan-out: N replies per prompt forked from one prefill (vcla_set_fanout) ------------------------------------------------------
+__global__ void fanout_rows_kernel(int n, int rows, int32_t* __restrict__ parent, int32_t* tok, int32_t* history) {
+  TraceScope trace(21);
+  trace.dep();
+  const int r = threadIdx.x;
+  int v = 0;
+  if (tok != nullptr && r < rows) v = tok[r / n];
+  __syncthreads();                     // every prompt pick is read before any row is rewritten in place
+  if (r < rows) {
+    parent[r] = r / n;
+    if (tok != nullptr) { tok[r] = v; history[r] = v; }
+  }
+  trace.done();
+}
+int fanout_rows(int n, int rows, int32_t* parent, int32_t* tok, int32_t* history, cudaStream_t st) {
+  if (n < 1 || rows < n || rows > 64 || rows % n != 0) { set_error("fanout_rows: %d rows are not a fan-out of %d", rows, n); return -1; }
+  if (tok != nullptr && history == nullptr) { set_error("fanout_rows: expanding the picks needs the token history"); return -1; }
+  fanout_rows_kernel<<<1, 64, 0, st>>>(n, rows, parent, tok, history);
+  VCLA_CUDA_OK(cudaGetLastError());
   return 0;
 }
 

@@ -117,6 +117,9 @@ struct vcla_ctx {
   int32_t *beam_cand_tok = nullptr, *beam_parent = nullptr, *hyp_len = nullptr, *hyp_fin = nullptr, *hyp_tok = nullptr, *hyp_tmp = nullptr;
   int32_t *beam_state = nullptr, *beam_copy = nullptr, *beam_table_tmp = nullptr;
   unsigned long long* beam_cow_bytes = nullptr;
+  // fan-out (vcla_set_fanout): vcla_prefill forks each prompt to `fanout` rows through the beam reorder (parent r / fanout); forked:
+  // the resident rows came from such a fork (cleared by vcla_reset)
+  int fanout = 1; bool forked = false;
   // token streaming (vcla_stream_*): ring in pinned, mapped host memory; stream_done is recorded after every armed enqueue
   StreamRing *ring_host = nullptr, *ring_dev = nullptr; bool stream_armed = false;
   cudaEvent_t stream_done = nullptr; bool stream_pending = false;
@@ -764,6 +767,7 @@ int vcla_reset(vcla_ctx* c, vcla_stream stream) {
   VCLA_CUDA_OK(cudaMemsetAsync(c->finished, 0, 64 * 4, (cudaStream_t)stream));
   c->len_bound = 0;
   c->resident_b = 0;
+  c->forked = false;
   return 0;
 }
 
@@ -973,8 +977,9 @@ static int dp_wait(vcla_ctx* c, cudaStream_t st) {
 }
 
 // The token pick of one step from the lm_splits partials the lm_head left in ws_lm: beam search, the sampler or the argmax (+ the
-// token exchange when data parallel).  fork == 0: the prefill's pick (beam search's first step, the exchange inline).  lookup: the
-// picks of all B rows of a prompt lookup verification step into lk_pick, without history, step, finished-flag or exchange writes.
+// token exchange when data parallel).  fork == 0: the prefill's pick (beam search's first step, the exchange inline; with fan-out the
+// sampler draws fanout picks from each of the B prompts' logits rows).  lookup: the picks of all B rows of a prompt lookup verification
+// step into lk_pick, without history, step, finished-flag or exchange writes.
 static int pick(vcla_ctx* c, int B, int lm_splits, float* logits, int32_t* tok, int fork, bool lookup, cudaStream_t st) {
   const vcla_config& g = c->cfg;
   if (lookup) {
@@ -1002,10 +1007,11 @@ static int pick(vcla_ctx* c, int B, int lm_splits, float* logits, int32_t* tok, 
   if (c->samp_on) {
     // logits -> [repetition penalty, no-repeat-ngram, temperature, top-k, top-p, draw] in one kernel; raw logits stay available
     float* lg = logits ? logits : c->samp_logits;
+    const int n = fork == 0 ? c->fanout : 1;
     count(c, 2);
     if (dec_logits_reduce(c->ws_lm, lm_splits, B, g.t_vocab, B, g.t_vocab, lg, g.t_vocab, c->cand_val, c->cand_idx, st)) return -1;
-    if (dec_sample(lg, g.t_vocab, g.t_vocab, B, c->tok_hist, c->step_idx, c->samp_params, tok, c->tok_hist, c->dp_on() ? c->dp_send : nullptr, c->finished,
-                   nullptr, st)) return -1;
+    if (dec_sample(lg, g.t_vocab, g.t_vocab, B * n, c->tok_hist, c->step_idx, c->samp_params, tok, c->tok_hist, c->dp_on() ? c->dp_send : nullptr,
+                   c->finished, nullptr, st, n)) return -1;
     if (c->dp_on()) return dp_gather(c, st, fork);
     return 0;
   }
@@ -1129,6 +1135,14 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
     if ((long)S + c->beam_max_new > g.max_seq) { set_error("prefill: prompt %d + %d new tokens exceed max_seq %d", S, c->beam_max_new, g.max_seq); return -1; }
     if (c->dp_on()) { set_error("prefill: beam search is not available while the data-parallel token exchange is active"); return -1; }
   }
+  const int n = c->fanout, rows = B * n;
+  if (n > 1) {
+    // each prompt is prefilled once and forked to n rows after the first pick
+    const int cap = std::min(g.max_batch, 64);
+    if (rows > cap) { set_error("prefill: %d prompts x %d replies exceed %d rows (min(max_batch, 64))", B, n, cap); return -1; }
+    if (c->beam_on) { set_error("prefill: fan-out (vcla_set_fanout) is not available with beam search"); return -1; }
+    if (c->dp_on()) { set_error("prefill: fan-out is not available while the data-parallel token exchange is active"); return -1; }
+  }
   if (vcla_reset(c, stream)) return -1;
   // pages for the prompt's tokens (real tokens only: left padding is never cached)
   count(c); if (kv_reserve(c->kv, B, S, left_pad, st)) return -1;
@@ -1138,11 +1152,19 @@ int vcla_prefill(vcla_ctx* c, const int64_t* ids, int B, int T, int image_mode, 
     count(c); if (scatter_image_rows(c->img_embeds, B, nq, TH, rs, S, c->resid, st)) return -1;
   }
   if (prefill_layers(c, B, S, left_pad, pos_from_mask, nullptr, st) || prefill_logits(c, B, S, logits_all, last_logits, next_tok, st)) return -1;
-  // sequence lengths become S - pad; the page the first decoded token will be appended to is reserved here
-  count(c); if (advance_seq(c->seq_len, B, S, left_pad, c->step_idx, c->kv, st, c->ring(), c->tok_hist)) return -1;
-  if (c->beam_on && beam_reorder(c, B, B * c->beam_K, next_tok ? next_tok : c->d_tok, st)) return -1;
+  int32_t* picks = next_tok ? next_tok : c->d_tok;
+  // fan-out: the parent map of the fork; the argmax picked once per prompt, so its picks (and history row 0) are widened to the rows
+  if (n > 1) { count(c); if (fanout_rows(n, rows, c->beam_parent, c->samp_on ? nullptr : picks, c->tok_hist, st)) return -1; }
+  // sequence lengths become S - pad; the page the first decoded token will be appended to is reserved here.  The step published to the
+  // token stream is history row 0 of all the rows.
+  count(c); if (advance_seq(c->seq_len, B, S, left_pad, c->step_idx, c->kv, st, c->ring(), c->tok_hist, rows)) return -1;
+  if (c->beam_on && beam_reorder(c, B, B * c->beam_K, picks, st)) return -1;
+  // fan-out: row r continues prompt r / n -- it shares the prompt's full pages, and every row but the first of a prompt gets its own copy
+  // of the partly filled page it writes next
+  if (n > 1 && beam_reorder(c, B, rows, picks, st)) return -1;
   c->len_bound = S;
-  c->resident_b = c->beam_on ? B * c->beam_K : B;
+  c->resident_b = c->beam_on ? B * c->beam_K : rows;
+  c->forked = n > 1;
   c->lk_primed = false;
   return stream_mark(c, st);
 }
@@ -1155,6 +1177,7 @@ int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* lo
   if (B != c->resident_b) { set_error("prefill_extend: batch %d differs from the %d resident sequences", B, c->resident_b); return -1; }
   if (c->dp_on()) { set_error("prefill_extend: not available while the data-parallel token exchange is active"); return -1; }
   if (c->beam_on) { set_error("prefill_extend: not available in beam-search mode"); return -1; }
+  if (c->fanout > 1 || c->forked) { set_error("prefill_extend: not available in fan-out mode or while forked rows are resident"); return -1; }
   if ((long)B * T > g.max_prefill_tokens) { set_error("prefill_extend: %d x %d tokens exceed max_prefill_tokens %d", B, T, g.max_prefill_tokens); return -1; }
   if (c->len_bound + T > g.max_seq) {
     set_error("prefill_extend: %lld cached tokens + %d exceed the context capacity max_seq=%d", (long long)c->len_bound, T, g.max_seq);
@@ -1557,6 +1580,13 @@ int vcla_set_beam(vcla_ctx* c, const vcla_beam* s) {
   if (p.max_new > c->cfg.max_seq) { set_error("beam: max_new_tokens %d exceeds max_seq %d", p.max_new, c->cfg.max_seq); return -1; }
   VCLA_CUDA_OK(cudaMemcpy(c->beam_params, &p, sizeof(p), cudaMemcpyHostToDevice));
   c->beam_on = true; c->beam_K = p.K; c->beam_max_new = p.max_new;
+  return 0;
+}
+
+int vcla_set_fanout(vcla_ctx* c, int n) {
+  if (!c) return -1;
+  if (n < 1 || n > 64) { set_error("vcla_set_fanout: %d replies per prompt not in 1..64", n); return -1; }
+  c->fanout = n;
   return 0;
 }
 

@@ -274,9 +274,10 @@ struct SamplerParams {     // lives in device memory: graphs captured once serve
 };
 int sampler_supported(int V);
 int sampler_init();
-// history: [L][B] int32 with L = *step_idx; writes tok[b], history_out[L][b], dp_send[b]; finished[b] (nullable): sticky EOS flag
+// history: [L][B] int32 with L = *step_idx; writes tok[b], history_out[L][b], dp_send[b]; finished[b] (nullable): sticky EOS flag.
+// fanout > 1: B is a multiple of it and sequence b scores logits row b / fanout (the prefill's pick of N replies per prompt)
 int dec_sample(const float* logits, int ld, int V, int B, const int32_t* history, const int32_t* step_idx, const SamplerParams* params_dev,
-               int32_t* tok, int32_t* history_out, int32_t* dp_send, int32_t* finished, float* scores_out, cudaStream_t st);
+               int32_t* tok, int32_t* history_out, int32_t* dp_send, int32_t* finished, float* scores_out, cudaStream_t st, int fanout = 1);
 // prompt lookup verification (B = 1): row r < R scores logits row r with the history column of length *step_idx + r and draws with
 // counter (*step_idx + r, 0); tok[r] = pick.  No history, finished or send-buffer writes.
 int dec_sample_lookup(const float* logits, int ld, int V, int R, const int32_t* history, const int32_t* step_idx, const SamplerParams* params_dev,
@@ -329,8 +330,14 @@ inline size_t stream_ring_bytes(int rows) { return offsetof(StreamRing, tokens) 
 // seq_len[b] += by - left_pad[b] ; *step_idx += 1 ; then reserve the page the NEXT token of every sequence will be appended to.
 // ring (nullable, device view of the mapped ring): first publish step L = *step_idx -- history row L ([L][B]) into ring row L, a
 // system-scope fence per writer, then ring->published = L + 1 with st.release.sys.  ring == nullptr executes none of it.
+// publish_rows (<= 64; 0: B): the width of history row L and of the published step -- a fan-out prefill publishes its B * N picks
+// while it advances the B prompts.
 int advance_seq(int32_t* seq_len, int B, int by, const int32_t* left_pad, int32_t* step_idx, const KvCache& kv, cudaStream_t st,
-                StreamRing* ring = nullptr, const int32_t* history = nullptr);
+                StreamRing* ring = nullptr, const int32_t* history = nullptr, int publish_rows = 0);
+// Fan-out (vcla_set_fanout): parent[r] = r / n for the rows = B * n rows forked from B prompts (the parent map of kv_beam_reorder).
+// tok != nullptr: tok[0..B) holds one pick per prompt (the argmax); it is expanded in place to tok[r] = tok[r / n], which also becomes
+// history row 0 ([0][rows]).  With the device sampler the picks are already per row (tok = nullptr).  One CTA.
+int fanout_rows(int n, int rows, int32_t* parent, int32_t* tok, int32_t* history, cudaStream_t st);
 // ---- prompt lookup decoding (one sequence): a verification step runs R = k + 1 rows -- the last emitted token and k drafts -- through
 // the decode step; lookup_accept then replaces advance_seq.  Restates HF:generation/utils.py:3603-3620 (_assisted_decoding, greedy
 // and sampled without an assistant: n_matches = leading drafts equal to the model's picks, valid_tokens = picks[: n_matches + 1],

@@ -38,11 +38,13 @@ __device__ __forceinline__ float philox_uniform(unsigned long long seed, uint32_
 // LOOKUP (prompt lookup verification, B = 1): CTA r scores query row r, whose history is column 0 with length *step_idx + r (the drafts
 // being verified sit provisionally at rows *step_idx ..), and draws with counter (*step_idx + r, 0): exactly the draw one-token decoding
 // makes at that length.  finished is neither read nor written (the accept kernel owns it); tok[r] receives the pick.
+// fanout (not LOOKUP): sequence b reads logits row b / fanout -- the prefill's pick of N replies per prompt, where the B = prompts x N
+// rows forked from one prompt share its last logits row and differ in their draw counters (L, b).  1 everywhere else.
 template <bool LOOKUP = false>
 __global__ void __launch_bounds__(kSampThreads, 1)
 dec_sample_kernel(const float* __restrict__ logits, int ld, int V, int B, const int32_t* __restrict__ history, const int32_t* __restrict__ step_idx,
                   const SamplerParams* __restrict__ pp, int32_t* __restrict__ tok, int32_t* __restrict__ history_out, int32_t* __restrict__ dp_send,
-                  int32_t* __restrict__ finished, float* __restrict__ scores_out) {
+                  int32_t* __restrict__ finished, float* __restrict__ scores_out, int fanout) {
   extern __shared__ __align__(16) uint8_t s_raw[];
   float* s_row = reinterpret_cast<float*>(s_raw);
   const int vpad = (V + 31) & ~31;
@@ -61,12 +63,12 @@ dec_sample_kernel(const float* __restrict__ logits, int ld, int V, int B, const 
   pdl_wait();
   trace.dep();
   const int b = LOOKUP ? 0 : blockIdx.x, tid = threadIdx.x;
-  const int row = blockIdx.x;
+  const int row = blockIdx.x, lrow = LOOKUP ? row : row / fanout;
   const SamplerParams p = *pp;
   const int L = *step_idx + (LOOKUP ? row : 0);     // tokens generated so far = rows of the history
   const float NEG_INF = -INFINITY;
 
-  for (int v = tid; v < V; v += kSampThreads) s_row[v] = logits[(size_t)row * ld + v];
+  for (int v = tid; v < V; v += kSampThreads) s_row[v] = logits[(size_t)lrow * ld + v];
   for (int i = tid; i < vpad / 32; i += kSampThreads) s_seen[i] = 0u;
   if (tid == 0) { s_n = 0; s_choice = 0; s_keep = 0; s_thr = 0xFFFFFFFFu; }
   __syncthreads();
@@ -172,8 +174,9 @@ size_t sampler_smem_bytes(int V) {
 int sampler_supported(int V) { return sampler_smem_bytes(V) <= 227u * 1024u - 1024u ? 1 : 0; }
 
 int dec_sample(const float* logits, int ld, int V, int B, const int32_t* history, const int32_t* step_idx, const SamplerParams* params_dev,
-               int32_t* tok, int32_t* history_out, int32_t* dp_send, int32_t* finished, float* scores_out, cudaStream_t st) {
+               int32_t* tok, int32_t* history_out, int32_t* dp_send, int32_t* finished, float* scores_out, cudaStream_t st, int fanout) {
   if (!sampler_supported(V)) { set_error("device sampler: vocabulary %d does not fit one CTA's shared memory", V); return -1; }
+  if (fanout < 1 || B % fanout != 0) { set_error("device sampler: %d rows are not a fan-out of %d per logits row", B, fanout); return -1; }
   const size_t smem = sampler_smem_bytes(V);      // the opt-in for this much dynamic shared memory is done by sampler_init()
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(B); cfg.blockDim = dim3(kSampThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
@@ -181,7 +184,7 @@ int dec_sample(const float* logits, int ld, int V, int B, const int32_t* history
   int na = 0;
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = attr; cfg.numAttrs = na;
-  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, dec_sample_kernel<false>, logits, ld, V, B, history, step_idx, params_dev, tok, history_out, dp_send, finished, scores_out));
+  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, dec_sample_kernel<false>, logits, ld, V, B, history, step_idx, params_dev, tok, history_out, dp_send, finished, scores_out, fanout));
   return 0;
 }
 
@@ -195,7 +198,7 @@ int dec_sample_lookup(const float* logits, int ld, int V, int R, const int32_t* 
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = attr; cfg.numAttrs = na;
   VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, dec_sample_kernel<true>, logits, ld, V, 1, history, step_idx, params_dev, tok, (int32_t*)nullptr,
-                                  (int32_t*)nullptr, (int32_t*)nullptr, (float*)nullptr));
+                                  (int32_t*)nullptr, (int32_t*)nullptr, (float*)nullptr, 1));
   return 0;
 }
 

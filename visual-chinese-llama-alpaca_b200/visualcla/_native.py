@@ -80,6 +80,7 @@ _SIGNATURES = [
     ("vcla_set_lookup", C.c_int, [_P, C.POINTER(VclaLookup), _P]),
     ("vcla_read_lookup_stats", C.c_int, [_P, _P, _P]),
     ("vcla_set_beam", C.c_int, [_P, C.POINTER(VclaBeam)]),
+    ("vcla_set_fanout", C.c_int, [_P, C.c_int]),
     ("vcla_read_beams", C.c_int, [_P, _P, _P, _P, _P]),
     ("vcla_beam_cow_bytes", C.c_int, [_P, C.POINTER(C.c_int64), C.c_int]),
     ("vcla_op_beam_step", C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, C.POINTER(VclaBeam), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -179,7 +179,7 @@ class Engine:
         S = T + self.nq if image_mode == N.IMAGE_AT_HEAD else T
         la = torch.empty(B, S, self.vocab, dtype=torch.float32, device=self.device) if all_logits else None
         ll = torch.empty(B, self.vocab, dtype=torch.float32, device=self.device) if last_logits else None
-        tok = torch.empty(B * (self._beam.num_beams if self._beam is not None else 1), dtype=torch.int32, device=self.device)
+        tok = torch.empty(B * (self._beam.num_beams if self._beam is not None else self._fanout), dtype=torch.int32, device=self.device)
         rows = None if img_rows is None else img_rows.to(self.device, dtype=torch.int32).contiguous()
         pad = None if left_pad is None else left_pad.to(self.device, dtype=torch.int32).contiguous()
         self.session += 1
@@ -358,6 +358,14 @@ class Engine:
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_set_beam(self._ctx, C.byref(spec) if spec is not None else None), "vcla_set_beam")
         self._beam = spec
+
+    # ---- fan-out: n sampled replies per prompt from one prefill (include/vcla.h, "fan-out") -------------------------------------
+    _fanout = 1
+
+    def set_fanout(self, n: int):
+        """n > 1: prefill forks every prompt to n rows sharing its KV pages (row b * n + j), the first pick drawn per row; 1: off."""
+        N.check(self.lib.vcla_set_fanout(self._ctx, int(n)), "vcla_set_fanout")
+        self._fanout = int(n)
 
     def read_beams(self, items: int):
         """-> (tokens (items, K, max_new) int32, lengths (items, K), scores (items, K) f32, done (items,)) host tensors: the finished-

@@ -420,8 +420,7 @@ class VisualCLAModel:
         nrs = getattr(gc, "num_return_sequences", 1) or 1
         if beams > 1 and nrs > beams:
             raise ValueError(f"`num_return_sequences` ({nrs}) has to be smaller or equal to `num_beams` ({beams}).")
-        if beams == 1 and nrs != 1:
-            raise NotImplementedError("num_return_sequences > 1 without beam search is not on the H100 path")
+        # without beams, num_return_sequences > 1 reaches generate() only with do_sample=True (GenerationConfig refuses greedy)
         return gc
 
     @staticmethod
@@ -434,6 +433,10 @@ class VisualCLAModel:
     @torch.no_grad()
     def generate(self, input_ids=None, pixel_values=None, attention_mask=None, generation_config=None,
                  logits_processor=None, stopping_criteria=None, prefix_allowed_tokens_fn=None, synced_gpus=False, **kwargs):
+        """HF generate() over the device path; returns the new tokens only.  do_sample=True with num_return_sequences=N > 1 returns
+        B * N rows, row b * N + j being reply j of prompt b (HF's repeat_interleave order): each prompt is encoded and prefilled once
+        and its KV pages are shared by its N rows, which then decode as a batch, each with its own draws.  prompt_lookup_num_tokens is
+        ignored then, as for any batch above one row (HF refuses assisted generation with num_return_sequences > 1)."""
         past_key_values = kwargs.pop("past_key_values", None)
         streamer = kwargs.pop("streamer", None)
         gc = self._resolve_generation_config(generation_config, kwargs)
@@ -443,12 +446,21 @@ class VisualCLAModel:
             return self._generate_beams(gc, input_ids, pixel_values, attention_mask, logits_processor, stopping_criteria, streamer)
         eng = self._engine
         B = input_ids.shape[0]
-        if B > eng.max_batch:
+        n_ret = int(getattr(gc, "num_return_sequences", 1) or 1)     # > 1 only when sampling: rows b * n_ret + j, forked per prompt
+        per_call = eng.max_batch
+        if n_ret > 1:
+            cap = min(eng.max_batch, 64)
+            if n_ret > cap:
+                raise NotImplementedError(f"num_return_sequences={n_ret} exceeds this model instance (at most min(max_batch, 64) = {cap} rows)")
+            per_call = cap // n_ret
+        if B > per_call:
             if streamer is not None:
+                if n_ret > 1:
+                    raise NotImplementedError(f"streaming {B} prompts x {n_ret} return sequences above {per_call * n_ret} rows is not supported")
                 raise NotImplementedError(f"streaming a batch of {B} > max_batch={eng.max_batch} prompts is not supported")
             outs = []
-            for s in range(0, B, eng.max_batch):
-                sl = slice(s, s + eng.max_batch)
+            for s in range(0, B, per_call):
+                sl = slice(s, s + per_call)
                 outs.append(self.generate(input_ids[sl], None if pixel_values is None else pixel_values[sl],
                                           None if attention_mask is None else attention_mask[sl],
                                           gc, logits_processor, stopping_criteria, None, synced_gpus))
@@ -472,14 +484,17 @@ class VisualCLAModel:
         need_logits = sampling or len(processors) > 0 or bool(getattr(gc, "output_logits", False) or getattr(gc, "output_scores", False))
         crit = list(stopping_criteria) if stopping_criteria is not None else []
 
-        reuse = self._plan_kv_reuse(past_key_values, input_ids, pixel_values, mode, rows, pads)
+        R = B * n_ret                                                  # decoded rows
+        reuse = self._plan_kv_reuse(past_key_values, input_ids, pixel_values, mode, rows, pads) if n_ret == 1 else None
         if mode != N.TEXT_ONLY and reuse is None:
             eng.vision_encode(pixel_values)
 
         def start(want_last_logits):
-            """prefill the prompt, or keep the reusable cached prefix and extend it by the rest -> (last logits, first pick)"""
+            """prefill the prompt, or keep the reusable cached prefix and extend it by the rest -> (last logits (B, V), first pick (R,))"""
             if reuse is None:
-                ll, first, _ = eng.prefill(input_ids, mode, rows, all_logits=False, last_logits=want_last_logits, left_pad=pads, pos_from_mask=True)
+                with self._fanout_mode(n_ret):
+                    ll, first, _ = eng.prefill(input_ids, mode, rows, all_logits=False, last_logits=want_last_logits, left_pad=pads,
+                                               pos_from_mask=True)
             else:
                 keep, rest = reuse
                 eng.truncate([keep])
@@ -491,36 +506,38 @@ class VisualCLAModel:
             if not getattr(gc, "return_dict_in_generate", False):
                 return result
             ids = px = None
-            if B == 1 and pads is None:       # only such a cache can be reused: keep its ids and pixels, nothing otherwise
+            if R == 1 and pads is None:       # only such a cache can be reused: keep its ids and pixels, nothing otherwise
                 ids = torch.cat([input_ids[0].detach().to("cpu", torch.int64), fed[0].detach().to("cpu", torch.int64)])
                 px = None if pixel_values is None else pixel_values.detach().to(eng.device).clone()
             cache = VclaKVCache(eng, getattr(eng, "session", 0), ids, mode, px)
             return SimpleNamespace(sequences=result, logits=logits, scores=None, past_key_values=cache)
 
         dev = eng.device
-        key = (B, need_logits)
+        key = (R, need_logits)
         if key not in self._tok_buf:
             # persistent step buffers (their addresses key the captured CUDA graph).  chat() runs under torch.inference_mode and
             # chat_in_stream's worker thread does not: allocate them as ordinary tensors so both may update them in place.
             with torch.inference_mode(False):
-                self._tok_buf[key] = (torch.zeros(B, dtype=torch.int32, device=dev),
-                                      torch.empty(B, eng.vocab, dtype=torch.float32, device=dev) if need_logits else None)
+                self._tok_buf[key] = (torch.zeros(R, dtype=torch.int32, device=dev),
+                                      torch.empty(R, eng.vocab, dtype=torch.float32, device=dev) if need_logits else None)
         tok, logits = self._tok_buf[key]
 
-        plan = self._device_plan(gc, B, S, max_new, eos, pad, min_new, need_logits, logits_processor, processors, crit, streamer)
+        plan = self._device_plan(gc, R, S, max_new, eos, pad, min_new, need_logits, logits_processor, processors, crit, streamer)
         if plan is not None:
             lookup = (input_ids[0], *plan.lookup, max_new) if plan.lookup else None
             if plan.streamed:
-                return self._generate_streamed(plan.spec, lookup, start, finish, B, max_new, eos, tok, streamer, crit)
-            return self._generate_graphs(plan.spec, lookup, start, finish, B, max_new, eos, tok)
+                return self._generate_streamed(plan.spec, lookup, start, finish, R, max_new, eos, tok, streamer, crit)
+            return self._generate_graphs(plan.spec, lookup, start, finish, R, max_new, eos, tok)
 
         # the per-step host loop: HF logits processors / sampling / criteria on the logits of every step
-        out = torch.full((B, max_new), pad, dtype=torch.int64, device=dev)
+        out = torch.full((R, max_new), pad, dtype=torch.int64, device=dev)
         all_logits: List[torch.Tensor] = []
         if streamer is not None:
-            streamer.put(torch.empty(B, 0, dtype=torch.int64))    # HF generate: put(input_ids) first -- none with inputs_embeds
+            streamer.put(torch.empty(R, 0, dtype=torch.int64))    # HF generate: put(input_ids) first -- none with inputs_embeds
         last, first_tok = start(need_logits)
-        finished = torch.zeros(B, dtype=torch.bool, device=dev)
+        if n_ret > 1 and last is not None:
+            last = last.repeat_interleave(n_ret, dim=0)          # the first step scores each prompt's last logits once per reply
+        finished = torch.zeros(R, dtype=torch.bool, device=dev)
         n_done = 0
         for step in range(max_new):
             if step == 0:
@@ -606,6 +623,17 @@ class VisualCLAModel:
         return stop
 
     # ---- the decode graphs: argmax, the device sampler, prompt lookup, each optionally streamed ------------------------------------
+    @contextlib.contextmanager
+    def _fanout_mode(self, n):
+        """n > 1: the prefill inside forks every prompt to n rows (num_return_sequences); switched off again right after it"""
+        if n > 1:
+            self._engine.set_fanout(n)
+        try:
+            yield
+        finally:
+            if n > 1:
+                self._engine.set_fanout(1)
+
     @contextlib.contextmanager
     def _sampler_mode(self, spec):
         """the device sampler (spec) for the prefill and decode steps inside, or the argmax graphs (None); always set before start()
