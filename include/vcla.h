@@ -383,9 +383,24 @@ int vcla_debug_decode_ctas_per_sm(vcla_ctx* ctx, int B, int* out2);
 /* prefill attention kernel: 0 = the mma.sync kernel everywhere, 1 (default) = wgmma flash attention (QK^T / PV on the warpgroup tensor
  * cores, S and O in registers, TMA operands) at head dim 128 (LLaMA prefill) and mma.sync at head dim 64 (ViT / Resampler), 2 = wgmma everywhere */
 void vcla_set_attention_tc(int mode);
+/* The prefill attention of vcla_vision_encode and vcla_prefill on caller buffers, through the same dispatch (vcla_set_attention_tc).
+ * All operands bf16, head h at columns [h*HD, (h+1)*HD) of a row; HD 64 or 128; strides in elements.
+ *   q        B*Sq rows: query i of sequence b is row b*Sq + i (q_stride)
+ *   k0, v0   segment 0, B*n0 rows: key j < n0 of sequence b is row b*n0 + j (kv0_stride)
+ *   k1, v1   segment 1, B*n1 rows (NULL when n1 = 0): key n0 + j of sequence b is row b*n1 + j (kv1_stride)
+ *   out      B*Sq rows (o_stride): out = softmax(scale * q k^T) v over the keys visible to the query; only the H*HD columns of
+ *            the B*Sq rows are written
+ * Key j of sequence b is visible to query i iff kv_start[b] <= j < n0 + n1 and, when causal, j <= i + n0 + n1 - Sq.  kv_start_dev is
+ * int32 (B) in device memory (left padding: the first kv_start[b] keys of sequence b are hidden), NULL for none.  A query that sees no
+ * key gets a row of zeros.  Hidden keys that share a 64-key tile with visible ones are still loaded, and a zero probability does not
+ * cancel a NaN in P*V: such K/V rows -- the left padding, the causal future, the rows after a sequence's last key up to its tile's end
+ * (the next sequence's first rows, or the allocation's) -- must be finite.  Causal attention takes one KV segment on the wgmma kernel;
+ * a call that kernel cannot describe (a pitch or an output stride that is not a multiple of 8, causal with two segments) runs on the
+ * mma.sync kernel.  Refused on the host, before any launch: a NULL q, k0, v0 or out (k1, v1 when n1 > 0), B, H or Sq below 1, and
+ * kv_start[b] outside [0, n0 + n1] (read back after synchronising the stream).  Synchronises. */
 int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v0, int kv0_stride, int n0, const void* k1,
                       const void* v1, int kv1_stride, int n1, void* out, int o_stride, int B, int H, int Sq, int HD, float scale,
-                      int causal, vcla_stream stream);
+                      int causal, vcla_stream stream, const int32_t* kv_start_dev);
 /* The paged prefill attention of vcla_prefill_extend on caller buffers (head dim 128): q (B*T rows, q_stride) bf16; kv_pages a layer
  * pool [pages][K|V][H][page_tokens][128] bf16; page_table int32 (B, pages_per_seq); base_len_dev int32 (B) cached tokens before the
  * chunk (the chunk's own K/V must already be in the pool at slots base_len .. base_len + T - 1); out (B*T rows, o_stride) bf16.

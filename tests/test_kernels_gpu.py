@@ -124,64 +124,6 @@ def test_gemm_swap_ab_splitk(lib, Nout, K, B, splits):
     assert err <= 2e-3 * max(1.0, ref.abs().max().item()), f"max err {err}"
 
 
-def _attn_ref(q, k, v, scale, causal):
-    # q (B,Sq,H,hd) k/v (B,Sk,H,hd)
-    qf, kf, vf = (t.float().transpose(1, 2) for t in (q, k, v))
-    s = qf @ kf.transpose(-1, -2) * scale
-    if causal:
-        Sq, Sk = s.shape[-2:]
-        m = torch.ones(Sq, Sk, dtype=torch.bool, device=s.device).tril(diagonal=Sk - Sq)
-        s = s.masked_fill(~m, float("-inf"))
-    return (torch.softmax(s, -1) @ vf).transpose(1, 2)
-
-
-# The ids are stable test names: "tcgen05" labels VCLA_ATTN_TC mode 2, the tensor-core kernel of csrc/attention_tc.cu (wgmma on sm_90a).
-@pytest.fixture(params=[0, 2], ids=["mma_sync", "tcgen05"])
-def attn_impl(request, lib):
-    """Both prefill attention kernels behind the same entry point: the mma.sync one (csrc/attention.cu) and the wgmma one
-    (csrc/attention_tc.cu: QK^T and PV on the warpgroup tensor cores, S / O in registers, TMA operands)."""
-    lib.vcla_set_attention_tc(request.param)
-    yield request.param
-    lib.vcla_set_attention_tc(int(__import__("os").environ.get("VCLA_ATTN_TC", "1")))
-
-
-@pytest.mark.parametrize("B,H,S,HD,causal", [(2, 16, 257, 64, 0), (3, 2, 17, 64, 0), (2, 32, 96, 128, 1), (1, 4, 200, 128, 1),
-                                              (2, 2, 64, 128, 1), (1, 2, 1, 128, 1), (2, 4, 128, 128, 1), (1, 2, 1088, 128, 1),
-                                              (2, 3, 300, 64, 1), (1, 2, 640, 64, 0)])
-def test_attention_self(lib, attn_impl, B, H, S, HD, causal):
-    D = H * HD
-    qkv = _rand((B * S, 3 * D), 1.0, 20)
-    out = torch.empty((B * S, D), dtype=torch.bfloat16, device="cuda")
-    scale = HD ** -0.5
-    _check(lib, lib.vcla_op_attention(_p(qkv), 3 * D, C.c_void_p(qkv.data_ptr() + D * 2), C.c_void_p(qkv.data_ptr() + 2 * D * 2), 3 * D, S,
-                                      None, None, 0, 0, _p(out), D, B, H, S, HD, scale, causal, _stream()))
-    torch.cuda.synchronize()
-    q, k, v = (qkv.view(B, S, 3, H, HD)[:, :, i] for i in range(3))
-    ref = _attn_ref(q, k, v, scale, causal).reshape(B * S, D)
-    assert (out.float() - ref).abs().max().item() <= 2e-2
-
-
-def test_attention_two_segments(lib, attn_impl):
-    """Resampler layout: 64 queries attend over [their own 64 rows ; 257 image rows] (ref resampler :315)."""
-    B, H, HD, Q, NI, L = 2, 16, 64, 64, 257, 3
-    D = H * HD
-    qkv = _rand((B * Q, 3 * D), 1.0, 21)
-    kvimg = _rand((B * NI, L * 2 * D), 1.0, 22)
-    layer = 1
-    out = torch.empty((B * Q, D), dtype=torch.bfloat16, device="cuda")
-    k1 = C.c_void_p(kvimg.data_ptr() + layer * 2 * D * 2)
-    v1 = C.c_void_p(kvimg.data_ptr() + (layer * 2 * D + D) * 2)
-    _check(lib, lib.vcla_op_attention(_p(qkv), 3 * D, C.c_void_p(qkv.data_ptr() + D * 2), C.c_void_p(qkv.data_ptr() + 2 * D * 2), 3 * D, Q,
-                                      k1, v1, L * 2 * D, NI, _p(out), D, B, H, Q, HD, HD ** -0.5, 0, _stream()))
-    torch.cuda.synchronize()
-    q = qkv.view(B, Q, 3, H, HD)[:, :, 0]
-    kq, vq = qkv.view(B, Q, 3, H, HD)[:, :, 1], qkv.view(B, Q, 3, H, HD)[:, :, 2]
-    ki = kvimg.view(B, NI, L, 2, H, HD)[:, :, layer, 0]
-    vi = kvimg.view(B, NI, L, 2, H, HD)[:, :, layer, 1]
-    ref = _attn_ref(q, torch.cat([kq, ki], 1), torch.cat([vq, vi], 1), HD ** -0.5, 0).reshape(B * Q, D)
-    assert (out.float() - ref).abs().max().item() <= 2e-2
-
-
 @pytest.mark.parametrize("rows,D", [(514, 1024), (7, 128), (96, 4096)])
 def test_layernorm_rmsnorm(lib, rows, D):
     x = torch.randn(rows, D, device="cuda") * 3 + 0.5

@@ -1967,11 +1967,29 @@ int vcla_debug_decode_ctas_per_sm(vcla_ctx* c, int B, int* out2) {
 int vcla_op_gemm_csk_clusters(int B, int splits) { return gemm_csk_clusters(B, splits); }
 void vcla_set_attention_tc(int on) { attention_set_tc(on); }
 int vcla_op_attention(const void* q, int q_stride, const void* k0, const void* v0, int kv0_stride, int n0, const void* k1, const void* v1,
-                      int kv1_stride, int n1, void* out, int o_stride, int B, int H, int Sq, int HD, float scale, int causal, vcla_stream stream) {
+                      int kv1_stride, int n1, void* out, int o_stride, int B, int H, int Sq, int HD, float scale, int causal, vcla_stream stream,
+                      const int32_t* kv_start_dev) {
+  // operator entry for tests: the left padding is read back and checked before the launch.  Synchronises.
+  if (!q || !k0 || !v0 || !out || (n1 > 0 && (!k1 || !v1)) || B < 1 || H < 1 || Sq < 1 || n0 < 0 || n1 < 0) {
+    set_error("vcla_op_attention: bad arguments"); return -1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (kv_start_dev) {
+    std::vector<int32_t> kv_start((size_t)B);
+    VCLA_CUDA_OK(cudaStreamSynchronize(st));
+    VCLA_CUDA_OK(cudaMemcpy(kv_start.data(), kv_start_dev, kv_start.size() * 4, cudaMemcpyDeviceToHost));
+    for (int b = 0; b < B; ++b) {
+      if (kv_start[b] < 0 || kv_start[b] > n0 + n1) {
+        set_error("vcla_op_attention: kv_start[%d] = %d outside [0, %d]", b, kv_start[b], n0 + n1); return -1;
+      }
+    }
+  }
   AttnCall a; a.q = (const bf16*)q; a.q_stride = q_stride; a.k0 = (const bf16*)k0; a.v0 = (const bf16*)v0; a.kv0_stride = kv0_stride; a.n0 = n0;
   a.k1 = (const bf16*)k1; a.v1 = (const bf16*)v1; a.kv1_stride = kv1_stride; a.n1 = n1; a.out = (bf16*)out; a.o_stride = o_stride;
-  a.B = B; a.H = H; a.Sq = Sq; a.HD = HD; a.scale = scale; a.causal = causal;
-  return attention_prefill(a, (cudaStream_t)stream);
+  a.B = B; a.H = H; a.Sq = Sq; a.HD = HD; a.scale = scale; a.causal = causal; a.kv_start = kv_start_dev;
+  int rc = attention_prefill(a, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_attention: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
+  return rc;
 }
 // Operator entries on a caller's pool: read back the page table [B][kv.pages_per_seq] and the lengths len_dev [B] (synchronising st) and
 // refuse, before any launch, a length below 0, a sequence whose len + rows tokens do not fit its table row, and a negative page among

@@ -106,7 +106,7 @@ _SIGNATURES = [
     ("vcla_debug_decode_ctas_per_sm", C.c_int, [_P, C.c_int, C.POINTER(C.c_int * 2)]),
     ("vcla_set_attention_tc", None, [C.c_int]),
     ("vcla_op_attention", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, C.c_int,
-                                    C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _P]),
+                                    C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _P, _P]),
     ("vcla_op_attention_paged", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_float, _P]),
     ("vcla_op_attention_decode", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float,
