@@ -57,6 +57,8 @@ typedef struct {
   int page_tokens;         /* tokens per KV-cache page (default 64 if 0) */
   /* storage of the LLaMA projections: 0 = bf16 (default), 1 = weight-only int8 (load_in_8bit, below) */
   int weight_format;
+  /* storage of the paged KV cache: 0 = bf16 (default), 1 = int8 rows + one fp32 scale per row (kv_cache_dtype="int8", below) */
+  int kv_format;
 } vcla_config;
 
 const char* vcla_last_error(void);
@@ -121,6 +123,17 @@ int vcla_reset(vcla_ctx* ctx, vcla_stream stream);
 int vcla_kv_geometry(const vcla_ctx* ctx, int* pages_per_seq, int* total_pages, int* page_tokens);
 int vcla_kv_read_pages(vcla_ctx* ctx, int32_t* table_host, int32_t* npages_host, int32_t* state_host);
 int vcla_kv_debug_shuffle(vcla_ctx* ctx, uint32_t seed);
+/* int8 KV cache (kv_format 1).  The reference keeps K/V in its DynamicCache as the model dtype (HF:cache_utils.py:88-120,
+ * DynamicCache.update: torch.cat of the new key_states / value_states); HF's QuantizedCache (HF:cache_utils.py, QuantizedCache) and
+ * vLLM's kv_cache_dtype store them in fewer bits instead.  Here every LLaMA K row (after RoPE) and V row is replaced, per head, by its
+ * int8 round trip the moment it is computed, with the load_in_8bit rule applied to the row's 128 fp32 values: a = max|x|,
+ * s = a / 127, q = clamp(rint(x * (127 / a)), -127, 127) (half to even; a = 0 gives s = q = 0).  Every attention reads q * s: the
+ * prefill QKV epilogue also writes bf16(q * s) into the K/V columns its own attention reads, the decode step quantises the new row
+ * before attending to it.  Per layer the pool holds the int8 rows [total_pages][K|V][heads][page_tokens][128] followed by their fp32
+ * scales [total_pages][K|V][heads][page_tokens]: 132 bytes per row instead of 256 (0.516x).  The page table, allocator, truncate /
+ * extend and copy-on-write are those of the bf16 cache; vcla_beam_cow_bytes counts 132 bytes per copied row.
+ *   vcla_kv_read_layer   synchronous copy of one layer's pool bytes (vcla_memory_bytes' kv / layers) to the host */
+int vcla_kv_read_layer(vcla_ctx* ctx, int layer, void* host);
 /* Keep each resident sequence's first min(current length, len_host[b]) cached tokens (b < B, B = the batch of the last
  * vcla_prefill) and forget the rest; the pages stay owned by the sequence (vcla_reset returns them).  With vcla_prefill_extend this
  * reuses the common prefix of a conversation: HF DynamicCache.crop (HF:cache_utils.py) before generate(past_key_values=...). */
@@ -434,6 +447,19 @@ int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_page
 int vcla_op_attention_decode_lookup(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq,
                                     int page_tokens, const int32_t* seq_len_dev, void* out, int rows, int H, int kv_splits, float scale,
                                     float rope_theta, vcla_stream stream);
+/* The paged prefill attention and the two decode entries on a pool in the int8 layout (kv_format 1, above): int8 rows of the
+ * total_pages pages, then their fp32 scales (the scale region starts total_pages * 2 * H * page_tokens * 128 bytes in).  Keys and
+ * values are read as q * s; the decode entries quantise the new row per head and write it as q and s.  Same refusals as the bf16
+ * entries, plus total_pages < 1 and a page the call reads at or beyond total_pages. */
+int vcla_op_attention_paged_q8(const void* q, int q_stride, const void* kv_pool, int total_pages, const int32_t* page_table,
+                               int pages_per_seq, int page_tokens, const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T,
+                               float scale, vcla_stream stream);
+int vcla_op_attention_decode_q8(const float* qkv_partial, int splits, void* kv_pool, int total_pages, const int32_t* page_table,
+                                int pages_per_seq, int page_tokens, const int32_t* seq_len_dev, void* out, int B, int H, int kv_splits,
+                                float scale, float rope_theta, int persistent, int persistent_grid, int launches, vcla_stream stream);
+int vcla_op_attention_decode_lookup_q8(const float* qkv_partial, int splits, void* kv_pool, int total_pages, const int32_t* page_table,
+                                       int pages_per_seq, int page_tokens, const int32_t* seq_len_dev, void* out, int rows, int H,
+                                       int kv_splits, float scale, float rope_theta, vcla_stream stream);
 /* The greedy pick of vcla_decode_step on caller buffers: logits_out f32 (B, V) or NULL = sum over splits (in split order) of partial f32
  * [splits][B][ldp] (ldp >= V; columns >= V are not read), tok_out int32 (B) = its argmax, the smallest index among equal maxima as
  * torch.argmax; a row that is -inf everywhere gives 0.  Synchronises. */

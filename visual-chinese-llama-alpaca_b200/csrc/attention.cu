@@ -253,12 +253,53 @@ constexpr int kDecMaxPT = 64;       // page_tokens supported by the smem ring
 // runs exactly the arithmetic of the one-token kernel at length seq_len[0] + r + 1.  Rows read keys that lower rows append, and CTAs
 // of one launch cannot rely on each other's stores, so a verification step launches this kernel twice: kDecAppend (grid (1, H, R), no
 // KV stream) writes the RoPE'd K and V of all R rows, then kDecAttend attends without writing the cache.
+//
+// FMT = KV_INT8 reads a pool of int8 rows + fp32 row scales (kernels.h): a stage holds the page's K rows, V rows, K scales and V
+// scales (PT x 264 B, 16.5 KB at 64 tokens); a score is s_k * sum q k and the accumulator takes (p s_v) v.  The new row is quantised
+// (absmax over its 128 dims), stored, and attended through the same arithmetic as a cached row.  Stage counts and occupancy are the
+// bf16 kernel's (the register budget, not shared memory, bounds the CTAs per SM), so the kv_splits choice stays format-independent.
 constexpr int kDecPlain = 0, kDecAttend = 1, kDecAppend = 2;
-template <int STAGES, int MODE = kDecPlain>
+constexpr int kDecQ8Extra = 16 * 4;   // KV_INT8: floats after the ring: per-warp k / v absmax [0, 8), the new row's s_k, s_v [8, 10)
+__host__ __device__ constexpr uint32_t dec_stage_bytes(int fmt, int pt) { return fmt == KV_INT8 ? (uint32_t)pt * (128 * 2 + 4 * 2) : (uint32_t)pt * 128 * 2 * 2; }
+static size_t dec_smem_bytes(int fmt, int stages, int pt) { return (size_t)stages * dec_stage_bytes(fmt, pt) + (fmt == KV_INT8 ? kDecQ8Extra : 0); }
+// KV_INT8: attend over ntok cached rows of one ring stage {K rows, V rows, K scales, V scales}; the token / lane split of the bf16 loop
+// (lane `sub` of a token group owns dims [8 sub, 8 sub + 8) and [64 + 8 sub, 64 + 8 sub + 8): two 8 B loads per row)
+__device__ __forceinline__ void dec_page_q8(const uint8_t* stage, int PT, int ntok, int warp, int grp, int sub, uint32_t gmask,
+                                            const float (&qreg)[16], float& m, float& l, float (&acc)[16]) {
+  constexpr int HD = 128;
+  const uint8_t* vbase = stage + (size_t)PT * HD;
+  const float* ksc = reinterpret_cast<const float*>(stage + (size_t)PT * HD * 2);
+  const float* vsc = ksc + PT;
+  for (int tk = warp * 4 + grp; tk < ntok; tk += kDecWarps * 4) {
+    const uint2 k0 = *reinterpret_cast<const uint2*>(stage + (size_t)tk * HD + sub * 8);
+    const uint2 k1 = *reinterpret_cast<const uint2*>(stage + (size_t)tk * HD + 64 + sub * 8);
+    const uint2 v0 = *reinterpret_cast<const uint2*>(vbase + (size_t)tk * HD + sub * 8);
+    const uint2 v1 = *reinterpret_cast<const uint2*>(vbase + (size_t)tk * HD + 64 + sub * 8);
+    const uint32_t kw[4] = {k0.x, k0.y, k1.x, k1.y};
+    const uint32_t vw[4] = {v0.x, v0.y, v1.x, v1.y};
+    float sc = 0.f;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) sc += qreg[j] * q8_lane(kw[j >> 2], j & 3);
+    sc += __shfl_xor_sync(gmask, sc, 1);
+    sc += __shfl_xor_sync(gmask, sc, 2);
+    sc += __shfl_xor_sync(gmask, sc, 4);
+    sc *= ksc[tk];
+    const float mn = fmaxf(m, sc);
+    const float cr = __expf(m - mn), p = __expf(sc - mn);
+    m = mn;
+    l = l * cr + p;
+    const float pv = p * vsc[tk];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) acc[j] = acc[j] * cr + pv * q8_lane(vw[j >> 2], j & 3);
+  }
+}
+
+template <int STAGES, int MODE = kDecPlain, int FMT = KV_BF16>
 __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_decode_kernel(const DecodeAttnCall c, const float* __restrict__ rope_cos,
                                                                                   const float* __restrict__ rope_sin) {
   constexpr int HD = 128;
-  extern __shared__ __align__(128) uint8_t dsm[];      // [STAGES][2][PT][HD] bf16
+  constexpr bool Q8 = FMT == KV_INT8;
+  extern __shared__ __align__(128) uint8_t dsm[];      // [STAGES][2][PT][HD] bf16 (KV_INT8: [STAGES]{K rows, V rows, K scales, V scales}, then kDecQ8Extra)
   __shared__ __align__(8) uint64_t s_bar[STAGES];
   __shared__ float s_q[HD];
   __shared__ float s_k[HD];
@@ -270,7 +311,7 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
   const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int T = c.kv.heads * HD, PT = c.kv.page_tokens;
-  const uint32_t stage_bytes = (uint32_t)PT * HD * 2 * 2;      // K page + V page
+  const uint32_t stage_bytes = Q8 ? dec_stage_bytes(KV_INT8, PT) : (uint32_t)PT * HD * 2 * 2;      // K page + V page
   TraceScope trace(MODE == kDecAppend ? 19 : 4);
   const int sb = MODE == kDecPlain ? b : 0;   // the sequence whose pages and length this CTA reads
 
@@ -301,11 +342,20 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
     const uint32_t bytes = (uint32_t)ntok * HD * 2;
     const uint32_t bar = smem_u32(&s_bar[stage]);
     const uint32_t dst = smem_u32(dsm) + stage * stage_bytes;
+    if constexpr (Q8) {
+      const uint32_t rbytes = (uint32_t)ntok * HD, sbytes = (uint32_t)((ntok + 3) & ~3) * 4;   // scales in whole 16 B (inside the plane)
+      mbar_arrive_expect_tx(bar, 2 * (rbytes + sbytes));
+      bulk_load_1d(dst, c.kv.q8_at(page, 0, h, 0), rbytes, bar);
+      bulk_load_1d(dst + (uint32_t)PT * HD, c.kv.q8_at(page, 1, h, 0), rbytes, bar);
+      bulk_load_1d(dst + (uint32_t)PT * HD * 2, c.kv.q8_scale(page, 0, h, 0), sbytes, bar);
+      bulk_load_1d(dst + (uint32_t)PT * (HD * 2 + 4), c.kv.q8_scale(page, 1, h, 0), sbytes, bar);
+    } else {
     const bf16* ksrc = c.kv.at(page, 0, h, 0);
     const bf16* vsrc = c.kv.at(page, 1, h, 0);
     mbar_arrive_expect_tx(bar, 2 * bytes);
     bulk_load_1d(dst, ksrc, bytes, bar);
     bulk_load_1d(dst + (uint32_t)PT * HD * 2, vsrc, bytes, bar);
+    }
   };
   if (tid == 0) {
     for (int i = 0; i < npages && i < STAGES; ++i) issue_page(i);   // the KV stream starts before the q reduction below
@@ -333,6 +383,33 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
       kr = kv * cs + kp * sn;
     }
     __syncthreads();
+    if constexpr (Q8) {
+      // the cache holds q and s: quantise both rows (block absmax over the 128 dims of warps 0..3), keep q in s_k / s_v and the
+      // scales in q8x[8..9], so the new row is attended with the arithmetic every later step applies to it
+      float* q8x = reinterpret_cast<float*>(dsm + (MODE == kDecAppend ? 0 : (size_t)STAGES * stage_bytes));   // the append streams no pages
+      if (owns_new) {
+        const float ka = warp_max(tid < HD ? fabsf(kr) : 0.f), va = warp_max(tid < HD ? fabsf(vv) : 0.f);
+        if (tid < HD && lane == 0) { q8x[warp] = ka; q8x[4 + warp] = va; }
+      }
+      __syncthreads();
+      if (tid < HD) {
+        s_q[d] = qr;
+        if (owns_new) {
+          const float ka = fmaxf(fmaxf(q8x[0], q8x[1]), fmaxf(q8x[2], q8x[3])), va = fmaxf(fmaxf(q8x[4], q8x[5]), fmaxf(q8x[6], q8x[7]));
+          const int kq = q8_quant(kr, q8_inv(ka)), vq = q8_quant(vv, q8_inv(va));
+          s_k[d] = (float)kq;
+          s_v[d] = (float)vq;
+          if (tid == 0) { q8x[8] = q8_step(ka); q8x[9] = q8_step(va); }
+          if (MODE != kDecAttend) {
+            const int page = c.kv.seq_pages(sb)[L / PT];
+            const int slot = L % PT;
+            c.kv.q8_at(page, 0, h, slot)[d] = (int8_t)kq;
+            c.kv.q8_at(page, 1, h, slot)[d] = (int8_t)vq;
+            if (tid == 0) { *c.kv.q8_scale(page, 0, h, slot) = q8_step(ka); *c.kv.q8_scale(page, 1, h, slot) = q8_step(va); }
+          }
+        }
+      }
+    } else {
     if (tid < HD) {
       s_q[d] = qr;
       if (owns_new) {
@@ -349,6 +426,7 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
           vdst[d] = vb;
         }
       }
+    }
     }
     __syncthreads();
   }
@@ -372,6 +450,9 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
     mbar_wait(smem_u32(&s_bar[stage]), parity);
     const int ntok = min(PT, c_end - (t_begin + i * PT));
     const uint8_t* kbase = dsm + (size_t)stage * stage_bytes;
+    if constexpr (Q8) {
+      dec_page_q8(kbase, PT, ntok, warp, grp, sub, gmask, qreg, m, l, acc);
+    } else {
     const uint8_t* vbase = kbase + (size_t)PT * HD * 2;
     for (int tk = warp * 4 + grp; tk < ntok; tk += kDecWarps * 4) {
       const uint4 k0 = *reinterpret_cast<const uint4*>(kbase + (size_t)tk * HD * 2 + sub * 16);
@@ -401,6 +482,7 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
         acc[2 * j + 1] = acc[2 * j + 1] * cr + p * vf.y;
       }
     }
+    }
     __syncthreads();                                   // every warp is done with this stage
     if (tid == 0 && i + STAGES < npages) issue_page(i + STAGES);
   }
@@ -413,14 +495,21 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
     sc += __shfl_xor_sync(0x000000ffu, sc, 1);
     sc += __shfl_xor_sync(0x000000ffu, sc, 2);
     sc += __shfl_xor_sync(0x000000ffu, sc, 4);
+    float pv_scale = 1.f;
+    if constexpr (Q8) {
+      const float* q8x = reinterpret_cast<const float*>(dsm + (size_t)STAGES * stage_bytes);
+      sc *= q8x[8];
+      pv_scale = q8x[9];
+    }
     const float mn = fmaxf(m, sc);
     const float cr = __expf(m - mn), p = __expf(sc - mn);
     m = mn;
     l = l * cr + p;
+    const float pv = Q8 ? p * pv_scale : p;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      acc[i] = acc[i] * cr + p * s_v[sub * 8 + i];
-      acc[8 + i] = acc[8 + i] * cr + p * s_v[64 + sub * 8 + i];
+      acc[i] = acc[i] * cr + pv * s_v[sub * 8 + i];
+      acc[8 + i] = acc[8 + i] * cr + pv * s_v[64 + sub * 8 + i];
     }
   }
   __syncwarp();
@@ -498,6 +587,7 @@ __global__ void __launch_bounds__(kDecWarps * 32, STAGES == 2 ? 3 : 2) attn_deco
 // reduction / epilogue of item i, so the fixed per-item latency chain (seq_len -> page table -> TMA -> q reduce -> combine)
 // is paid once per CTA instead of once per wave (B=32: 3.5 waves of one-shot CTAs).
 // ------------------------------------------------------------------------------------------------------------------------
+template <int FMT = KV_BF16>
 __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persistent_kernel(const DecodeAttnCall c, const float* __restrict__ rope_cos,
                                                                                        const float* __restrict__ rope_sin, int n_items) {
   // warps 0..7: consumers; warp 8: KV page producer (TMA bulk copies); warp 9: q/k/v producer (split-K reduce, deferred norm
@@ -505,7 +595,8 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
   // round trip is left on the consumers' per-item critical path.
   constexpr int HD = 128;
   constexpr int NC = kDecWarps * 32;                    // consumer threads
-  extern __shared__ __align__(128) uint8_t dsm[];      // [kDecStages][2][PT][HD] bf16
+  constexpr bool Q8 = FMT == KV_INT8;
+  extern __shared__ __align__(128) uint8_t dsm[];      // [kDecStages][2][PT][HD] bf16 (KV_INT8: as attn_decode_kernel, then s_k, s_v of both q slots)
   __shared__ __align__(8) uint64_t s_full[kDecStages];
   __shared__ __align__(8) uint64_t s_empty[kDecStages];
   __shared__ __align__(8) uint64_t s_qfull[2];
@@ -518,7 +609,7 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int T = c.kv.heads * HD, PT = c.kv.page_tokens;
-  const uint32_t stage_bytes = (uint32_t)PT * HD * 2 * 2;
+  const uint32_t stage_bytes = Q8 ? dec_stage_bytes(KV_INT8, PT) : (uint32_t)PT * HD * 2 * 2;
   TraceScope trace(4);
   if (tid == 0) {
     for (int s = 0; s < kDecStages; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), kDecWarps); }
@@ -546,11 +637,20 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
           const uint32_t bytes = (uint32_t)ntok * HD * 2;
           const uint32_t bar = smem_u32(&s_full[stage]);
           const uint32_t dst = smem_u32(dsm) + stage * stage_bytes;
+          if constexpr (Q8) {
+            const uint32_t rbytes = (uint32_t)ntok * HD, sbytes = (uint32_t)((ntok + 3) & ~3) * 4;
+            mbar_arrive_expect_tx(bar, 2 * (rbytes + sbytes));
+            bulk_load_1d(dst, c.kv.q8_at(page, 0, h, 0), rbytes, bar);
+            bulk_load_1d(dst + (uint32_t)PT * HD, c.kv.q8_at(page, 1, h, 0), rbytes, bar);
+            bulk_load_1d(dst + (uint32_t)PT * HD * 2, c.kv.q8_scale(page, 0, h, 0), sbytes, bar);
+            bulk_load_1d(dst + (uint32_t)PT * (HD * 2 + 4), c.kv.q8_scale(page, 1, h, 0), sbytes, bar);
+          } else {
           const bf16* ksrc = c.kv.at(page, 0, h, 0);
           const bf16* vsrc = c.kv.at(page, 1, h, 0);
           mbar_arrive_expect_tx(bar, 2 * bytes);
           bulk_load_1d(dst, ksrc, bytes, bar);
           bulk_load_1d(dst + (uint32_t)PT * HD * 2, vsrc, bytes, bar);
+          }
         }
       }
     }
@@ -588,6 +688,40 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
       const float cs[4] = {cs4.x, cs4.y, cs4.z, cs4.w}, sn[4] = {sn4.x, sn4.y, sn4.z, sn4.w};
       float qo[4], ko[4], vo[4];
       uint32_t kpk[2], vpk[2];
+      if constexpr (Q8) {
+        // quantise the new k / v rows (warp absmax: lane l holds dims [4l, 4l+4)); s_k / s_v take q, the scales go after the ring
+        float kr[4], ka = 0.f, va = 0.f;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float kp = __shfl_xor_sync(0xffffffffu, k4[j], 16), qp = __shfl_xor_sync(0xffffffffu, q4[j], 16);
+          const float sgn = (lane < 16) ? -1.f : 1.f;
+          qo[j] = (q4[j] * cs[j] + sgn * qp * sn[j]) * c.scale;
+          kr[j] = k4[j] * cs[j] + sgn * kp * sn[j];
+          ka = fmaxf(ka, fabsf(kr[j])); va = fmaxf(va, fabsf(v4[j]));
+        }
+        ka = warp_max(ka); va = warp_max(va);
+        const float kinv = q8_inv(ka), vinv = q8_inv(va);
+        uint32_t kq = 0, vq = 0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int a = q8_quant(kr[j], kinv), v = q8_quant(v4[j], vinv);
+          ko[j] = (float)a; vo[j] = (float)v;
+          kq |= (uint32_t)(a & 0xff) << (8 * j); vq |= (uint32_t)(v & 0xff) << (8 * j);
+        }
+        float* q8x = reinterpret_cast<float*>(dsm + (size_t)kDecStages * stage_bytes);
+        *reinterpret_cast<float4*>(&s_q[slot][4 * lane]) = make_float4(qo[0], qo[1], qo[2], qo[3]);
+        *reinterpret_cast<float4*>(&s_k[slot][4 * lane]) = make_float4(ko[0], ko[1], ko[2], ko[3]);
+        *reinterpret_cast<float4*>(&s_v[slot][4 * lane]) = make_float4(vo[0], vo[1], vo[2], vo[3]);
+        if (lane == 0) { q8x[2 * slot] = q8_step(ka); q8x[2 * slot + 1] = q8_step(va); }
+        const int page = __ldg(c.kv.seq_pages(b) + L / PT);
+        const int cslot = L % PT;
+        *reinterpret_cast<uint32_t*>(c.kv.q8_at(page, 0, h, cslot) + 4 * lane) = kq;
+        *reinterpret_cast<uint32_t*>(c.kv.q8_at(page, 1, h, cslot) + 4 * lane) = vq;
+        if (lane == 0) { *c.kv.q8_scale(page, 0, h, cslot) = q8_step(ka); *c.kv.q8_scale(page, 1, h, cslot) = q8_step(va); }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&s_qfull[slot]));
+        continue;
+      }
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const float qv = q4[j], kv = k4[j], vv = v4[j];
@@ -633,6 +767,9 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
       mbar_wait(smem_u32(&s_full[stage]), (n / kDecStages) & 1u);
       const int ntok = min(PT, L - i * PT);
       const uint8_t* kbase = dsm + (size_t)stage * stage_bytes;
+      if constexpr (Q8) {
+        dec_page_q8(kbase, PT, ntok, warp, grp, sub, gmask, qreg, m, l, acc);
+      } else {
       const uint8_t* vbase = kbase + (size_t)PT * HD * 2;
       for (int tk = warp * 4 + grp; tk < ntok; tk += kDecWarps * 4) {
         const uint4 k0 = *reinterpret_cast<const uint4*>(kbase + (size_t)tk * HD * 2 + sub * 16);
@@ -658,6 +795,7 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
           acc[2 * j + 1] = acc[2 * j + 1] * cr + p * vf.y;
         }
       }
+      }
       __syncwarp();
       if (lane == 0) mbar_arrive(smem_u32(&s_empty[stage]));     // this warp is done with the stage
     }
@@ -669,14 +807,21 @@ __global__ void __launch_bounds__((kDecWarps + 2) * 32, 2) attn_decode_persisten
       sc += __shfl_xor_sync(0x000000ffu, sc, 1);
       sc += __shfl_xor_sync(0x000000ffu, sc, 2);
       sc += __shfl_xor_sync(0x000000ffu, sc, 4);
+      float pv_scale = 1.f;
+      if constexpr (Q8) {
+        const float* q8x = reinterpret_cast<const float*>(dsm + (size_t)kDecStages * stage_bytes);
+        sc *= q8x[2 * slot];
+        pv_scale = q8x[2 * slot + 1];
+      }
       const float mn = fmaxf(m, sc);
       const float cr = __expf(m - mn), p = __expf(sc - mn);
       m = mn;
       l = l * cr + p;
+      const float pv = Q8 ? p * pv_scale : p;
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        acc[i] = acc[i] * cr + p * s_v[slot][sub * 8 + i];
-        acc[8 + i] = acc[8 + i] * cr + p * s_v[slot][64 + sub * 8 + i];
+        acc[i] = acc[i] * cr + pv * s_v[slot][sub * 8 + i];
+        acc[8 + i] = acc[8 + i] * cr + pv * s_v[slot][64 + sub * 8 + i];
       }
     }
     __syncwarp();
@@ -728,18 +873,24 @@ int attention_init() {
     auto set = [](const void* fn, int bytes) { return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess ? 0 : -1; };
     rc |= set((const void*)attn_decode_kernel<kDecStages>, kDecStages * kDecMaxPT * 128 * 2 * 2);
     rc |= set((const void*)attn_decode_kernel<kDecStagesSmallBatch>, kDecStagesSmallBatch * kDecMaxPT * 128 * 2 * 2);
-    rc |= set((const void*)attn_decode_persistent_kernel, kDecStages * kDecMaxPT * 128 * 2 * 2);
+    rc |= set((const void*)attn_decode_persistent_kernel<KV_BF16>, kDecStages * kDecMaxPT * 128 * 2 * 2);
     rc |= set((const void*)attn_decode_kernel<kDecStages, kDecAttend>, kDecStages * kDecMaxPT * 128 * 2 * 2);
     rc |= set((const void*)attn_decode_kernel<kDecStagesSmallBatch, kDecAttend>, kDecStagesSmallBatch * kDecMaxPT * 128 * 2 * 2);
     rc |= set((const void*)attn_prefill_kernel<128>, 5 * 64 * 128 * 2);
     rc |= set((const void*)attn_prefill_kernel<64>, 5 * 64 * 64 * 2);
+    const int q8_3 = (int)dec_smem_bytes(KV_INT8, kDecStages, kDecMaxPT), q8_2 = (int)dec_smem_bytes(KV_INT8, kDecStagesSmallBatch, kDecMaxPT);
+    rc |= set((const void*)attn_decode_kernel<kDecStages, kDecPlain, KV_INT8>, q8_3);
+    rc |= set((const void*)attn_decode_kernel<kDecStagesSmallBatch, kDecPlain, KV_INT8>, q8_2);
+    rc |= set((const void*)attn_decode_persistent_kernel<KV_INT8>, q8_3);
+    rc |= set((const void*)attn_decode_kernel<kDecStages, kDecAttend, KV_INT8>, q8_3);
+    rc |= set((const void*)attn_decode_kernel<kDecStagesSmallBatch, kDecAttend, KV_INT8>, q8_2);
     if (rc) set_error("attention_init: cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError()));
   });
   return rc;
 }
 
 // The decode kernel attention_decode launches for c: the persistent kernel (-> its grid in *persistent_ctas) or the one-shot kernel with
-// a 2- or 3-stage ring.
+// a 2- or 3-stage ring.  The choice does not depend on the cache format.
 enum DecodeKernel { kDecPersistent, kDecOneShot2, kDecOneShot3 };
 static DecodeKernel decode_kernel_pick(const DecodeAttnCall& c, int* persistent_ctas) {
   const int n_items = c.B * c.kv.heads;
@@ -756,14 +907,19 @@ static DecodeKernel decode_kernel_pick(const DecodeAttnCall& c, int* persistent_
   return c.kv_splits * n_items <= 2 * num_sms() ? kDecOneShot2 : kDecOneShot3;
 }
 
-int attention_decode(const DecodeAttnCall& c, cudaStream_t st) {
-  if (c.HD != 128) { set_error("attention_decode: head dim %d unsupported (128)", c.HD); return -1; }
-  if (c.kv.page_tokens < 8 || c.kv.page_tokens > kDecMaxPT || c.kv.page_tokens % 8 != 0) { set_error("attention_decode: page_tokens %d unsupported (8..%d, multiple of 8)", c.kv.page_tokens, kDecMaxPT); return -1; }
-  if (c.rope_cos == nullptr || c.rope_sin == nullptr) { set_error("attention_decode: rope table not initialised"); return -1; }
-  if (attention_init()) return -1;
+static int decode_check(const char* who, const DecodeAttnCall& c, KvFormat fmt) {
+  if (c.HD != 128) { set_error("%s: head dim %d unsupported (128)", who, c.HD); return -1; }
+  if (c.kv.page_tokens < 8 || c.kv.page_tokens > kDecMaxPT || c.kv.page_tokens % 8 != 0) { set_error("%s: page_tokens %d unsupported (8..%d, multiple of 8)", who, c.kv.page_tokens, kDecMaxPT); return -1; }
+  if (c.rope_cos == nullptr || c.rope_sin == nullptr) { set_error("%s: rope table not initialised", who); return -1; }
+  if (fmt != KV_BF16 && fmt != KV_INT8) { set_error("%s: KV cache format %d unsupported", who, (int)fmt); return -1; }
+  return attention_init();
+}
+
+template <int FMT>
+static int decode_launch(const DecodeAttnCall& c, cudaStream_t st) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(c.kv_splits, c.kv.heads, c.B); cfg.blockDim = dim3(kDecWarps * 32);
-  cfg.dynamicSmemBytes = (size_t)kDecStages * c.kv.page_tokens * 128 * 2 * 2; cfg.stream = st;
+  cfg.dynamicSmemBytes = dec_smem_bytes(FMT, kDecStages, c.kv.page_tokens); cfg.stream = st;
   cudaLaunchAttribute attr[1];
   int na = 0;
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
@@ -773,61 +929,74 @@ int attention_decode(const DecodeAttnCall& c, cudaStream_t st) {
     case kDecPersistent:
       cfg.gridDim = dim3(persistent_ctas);
       cfg.blockDim = dim3((kDecWarps + 2) * 32);
-      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_persistent_kernel, c, c.rope_cos, c.rope_sin, c.B * c.kv.heads));
+      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_persistent_kernel<FMT>, c, c.rope_cos, c.rope_sin, c.B * c.kv.heads));
       break;
     case kDecOneShot2:
-      cfg.dynamicSmemBytes = (size_t)kDecStagesSmallBatch * c.kv.page_tokens * 128 * 2 * 2;
-      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch>, c, c.rope_cos, c.rope_sin));
+      cfg.dynamicSmemBytes = dec_smem_bytes(FMT, kDecStagesSmallBatch, c.kv.page_tokens);
+      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch, kDecPlain, FMT>, c, c.rope_cos, c.rope_sin));
       break;
     case kDecOneShot3:
-      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStages>, c, c.rope_cos, c.rope_sin));
+      VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStages, kDecPlain, FMT>, c, c.rope_cos, c.rope_sin));
       break;
   }
   return 0;
 }
 
-int attention_decode_lookup(const DecodeAttnCall& c, cudaStream_t st) {
-  if (c.HD != 128) { set_error("attention_decode_lookup: head dim %d unsupported (128)", c.HD); return -1; }
-  if (c.kv.page_tokens < 8 || c.kv.page_tokens > kDecMaxPT || c.kv.page_tokens % 8 != 0) { set_error("attention_decode_lookup: page_tokens %d unsupported (8..%d, multiple of 8)", c.kv.page_tokens, kDecMaxPT); return -1; }
-  if (c.rope_cos == nullptr || c.rope_sin == nullptr) { set_error("attention_decode_lookup: rope table not initialised"); return -1; }
-  if (c.kv_splits < 1 || c.kv_splits > 8 || c.B < 1 || c.B > 16) { set_error("attention_decode_lookup: %d rows x %d KV splits unsupported", c.B, c.kv_splits); return -1; }
-  if (attention_init()) return -1;
+int attention_decode(const DecodeAttnCall& c, cudaStream_t st, KvFormat fmt) {
+  if (decode_check("attention_decode", c, fmt)) return -1;
+  return fmt == KV_INT8 ? decode_launch<KV_INT8>(c, st) : decode_launch<KV_BF16>(c, st);
+}
+
+template <int FMT>
+static int decode_lookup_launch(const DecodeAttnCall& c, cudaStream_t st) {
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   int na = 0;
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = attr; cfg.numAttrs = na; cfg.stream = st; cfg.blockDim = dim3(kDecWarps * 32);
-  cfg.gridDim = dim3(1, c.kv.heads, c.B); cfg.dynamicSmemBytes = 0;
-  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch, kDecAppend>, c, c.rope_cos, c.rope_sin));
+  // the append launch streams no pages: no ring; the int8 rows need only the absmax scratch
+  cfg.gridDim = dim3(1, c.kv.heads, c.B); cfg.dynamicSmemBytes = FMT == KV_INT8 ? kDecQ8Extra : 0;
+  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch, kDecAppend, FMT>, c, c.rope_cos, c.rope_sin));
   // the ring depth changes no arithmetic; the one-token rule picks it from the grid size
   cfg.gridDim = dim3(c.kv_splits, c.kv.heads, c.B);
   if (c.kv_splits * c.B * c.kv.heads <= 2 * num_sms()) {
-    cfg.dynamicSmemBytes = (size_t)kDecStagesSmallBatch * c.kv.page_tokens * 128 * 2 * 2;
-    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch, kDecAttend>, c, c.rope_cos, c.rope_sin));
+    cfg.dynamicSmemBytes = dec_smem_bytes(FMT, kDecStagesSmallBatch, c.kv.page_tokens);
+    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStagesSmallBatch, kDecAttend, FMT>, c, c.rope_cos, c.rope_sin));
   } else {
-    cfg.dynamicSmemBytes = (size_t)kDecStages * c.kv.page_tokens * 128 * 2 * 2;
-    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStages, kDecAttend>, c, c.rope_cos, c.rope_sin));
+    cfg.dynamicSmemBytes = dec_smem_bytes(FMT, kDecStages, c.kv.page_tokens);
+    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_decode_kernel<kDecStages, kDecAttend, FMT>, c, c.rope_cos, c.rope_sin));
   }
   return 0;
 }
 
-int attention_decode_ctas_per_sm(const DecodeAttnCall& c) {
-  if (attention_init()) return -1;
+int attention_decode_lookup(const DecodeAttnCall& c, cudaStream_t st, KvFormat fmt) {
+  if (c.kv_splits < 1 || c.kv_splits > 8 || c.B < 1 || c.B > 16) { set_error("attention_decode_lookup: %d rows x %d KV splits unsupported", c.B, c.kv_splits); return -1; }
+  if (decode_check("attention_decode_lookup", c, fmt)) return -1;
+  return fmt == KV_INT8 ? decode_lookup_launch<KV_INT8>(c, st) : decode_lookup_launch<KV_BF16>(c, st);
+}
+
+template <int FMT>
+static int decode_ctas_per_sm(const DecodeAttnCall& c) {
   int persistent_ctas = 0, n = 0;
   cudaError_t e = cudaSuccess;
   switch (decode_kernel_pick(c, &persistent_ctas)) {
     case kDecPersistent:
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_persistent_kernel, (kDecWarps + 2) * 32, (size_t)kDecStages * c.kv.page_tokens * 128 * 2 * 2);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_persistent_kernel<FMT>, (kDecWarps + 2) * 32, dec_smem_bytes(FMT, kDecStages, c.kv.page_tokens));
       break;
     case kDecOneShot2:
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStagesSmallBatch>, kDecWarps * 32, (size_t)kDecStagesSmallBatch * c.kv.page_tokens * 128 * 2 * 2);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStagesSmallBatch, kDecPlain, FMT>, kDecWarps * 32, dec_smem_bytes(FMT, kDecStagesSmallBatch, c.kv.page_tokens));
       break;
     case kDecOneShot3:
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStages>, kDecWarps * 32, (size_t)kDecStages * c.kv.page_tokens * 128 * 2 * 2);
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, attn_decode_kernel<kDecStages, kDecPlain, FMT>, kDecWarps * 32, dec_smem_bytes(FMT, kDecStages, c.kv.page_tokens));
       break;
   }
   if (e != cudaSuccess) { set_error("attention_decode_ctas_per_sm: %s", cudaGetErrorString(e)); (void)cudaGetLastError(); return -1; }
   return n;
+}
+
+int attention_decode_ctas_per_sm(const DecodeAttnCall& c, KvFormat fmt) {
+  if (attention_init()) return -1;
+  return fmt == KV_INT8 ? decode_ctas_per_sm<KV_INT8>(c) : decode_ctas_per_sm<KV_BF16>(c);
 }
 
 }  // namespace vcla

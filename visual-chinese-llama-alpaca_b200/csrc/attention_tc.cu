@@ -78,11 +78,18 @@ __device__ __forceinline__ void wgmma_pv(float (&o)[HD / 2], const uint32_t (&a)
   else wgmma_bf16_rs_tb_n128(o, a, bdesc, 1);
 }
 
-template <int HD, bool PAGED>
+// FMT = KV_INT8 (PAGED only): the pool holds int8 rows + fp32 row scales (kernels.h).  TMA brings each page's int8 rows (a UINT8 map
+// over the 128-byte rows) into the upper half of the stage's K / V tiles and a bulk copy its scales; the warpgroup converts the rows
+// to bf16 in the 128 B-swizzled image the descriptors read (exact: |q| <= 127), multiplies S by s_k, scales P's columns by s_v before
+// P is rounded to bf16, and keeps the row sum on the unscaled p.
+constexpr int kAtQ8ScaleBytes = 2 * kAtBKV * 4;   // per stage: K scales, V scales of the tile's 64 keys
+template <int HD, bool PAGED, int FMT = KV_BF16>
 __global__ void __launch_bounds__(kAtThreads, 2)
 attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0, const __grid_constant__ CUtensorMap tmV0,
                        const __grid_constant__ CUtensorMap tmK1, const __grid_constant__ CUtensorMap tmV1, const AttnTcParams p) {
   using C = AttnTcCfg<HD>;
+  constexpr bool Q8 = FMT == KV_INT8;
+  static_assert(!Q8 || (PAGED && HD == 128), "the int8 pool is read by the paged kernel only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar0 = base + C::BAR_OFF;
@@ -134,8 +141,23 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       for (int i = 0; i < n_tiles; ++i) {
         const int j = jt0 + i, stage = i % kAtStages;
         mbar_wait_mma(kv_empty(stage), (((uint32_t)(i / kAtStages)) & 1u) ^ 1u);
-        mbar_arrive_expect_tx(kv_full(stage), C::K_BYTES + C::V_BYTES);
         const uint32_t sk = base + C::KV_OFF + stage * (C::K_BYTES + C::V_BYTES), sv = sk + C::K_BYTES;
+        if constexpr (Q8) {
+          // int8 rows into the second k-block of the K / V tiles (the warpgroup expands them in place), scales after the barriers
+          mbar_arrive_expect_tx(kv_full(stage), 2 * kAtBKV * 128 + kAtQ8ScaleBytes);
+          const uint32_t ssc = base + C::BAR_OFF + 256 + stage * kAtQ8ScaleBytes;
+          const int pt = p.kv.page_tokens, last_page = (n0 - 1) / pt;
+          const int32_t* prow = p.kv.seq_pages(b);
+          for (int r = 0; r < kAtBKV; r += pt) {
+            const int page = prow[min((j * kAtBKV + r) / pt, last_page)];
+            tma_load_2d(sk + kAtBKV * 128 + r * 128, &tmK0, 0, p.kv.row<int>(page, 0, h), kv_full(stage), kEvictNormal);
+            tma_load_2d(sv + kAtBKV * 128 + r * 128, &tmK0, 0, p.kv.row<int>(page, 1, h), kv_full(stage), kEvictNormal);
+            bulk_load_1d(ssc + r * 4, p.kv.q8_scale(page, 0, h, 0), (uint32_t)pt * 4, kv_full(stage));
+            bulk_load_1d(ssc + kAtBKV * 4 + r * 4, p.kv.q8_scale(page, 1, h, 0), (uint32_t)pt * 4, kv_full(stage));
+          }
+          continue;
+        }
+        mbar_arrive_expect_tx(kv_full(stage), C::K_BYTES + C::V_BYTES);
         if constexpr (PAGED) {
           // one box of page_tokens rows per page and 64-column half; boxes past the sequence's last page re-read that page
           // (only pages the sequence owns are touched; those rows are masked)
@@ -182,6 +204,45 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       const int lo = max(kv0 - kbase, 0);
       const uint32_t sk = base + C::KV_OFF + stage * (C::K_BYTES + C::V_BYTES), sv = sk + C::K_BYTES;
       mbar_wait_mma(kv_full(stage), ((uint32_t)(i / kAtStages)) & 1u);
+      const float* ksc = nullptr;
+      const float* vsc = nullptr;
+      if constexpr (Q8) {
+        // expand the int8 rows (upper k-block of each tile) to the bf16 swizzled image: thread t owns row t / 2, k-block t % 2.  All
+        // reads finish before any write, since the bf16 image overwrites the int8 rows.
+        const int r = threadIdx.x >> 1, kb = threadIdx.x & 1;
+        uint4 kr[4], vr[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(kr[c].x), "=r"(kr[c].y), "=r"(kr[c].z), "=r"(kr[c].w)
+                       : "r"(sk + kAtBKV * 128 + r * 128 + kb * 64 + c * 16));
+          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(vr[c].x), "=r"(vr[c].y), "=r"(vr[c].z), "=r"(vr[c].w)
+                       : "r"(sv + kAtBKV * 128 + r * 128 + kb * 64 + c * 16));
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const uint32_t kw[4] = {kr[c].x, kr[c].y, kr[c].z, kr[c].w}, vw[4] = {vr[c].x, vr[c].y, vr[c].z, vr[c].w};
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {             // 16 int8 -> two 16 B chunks of 8 bf16
+            const int chunk = 2 * c + half;
+            const uint32_t off = kb * kAtBKV * 128 + r * 128 + ((chunk ^ (r & 7)) << 4);
+            uint32_t ko[4], vo[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const uint32_t kword = kw[2 * half + (e >> 1)], vword = vw[2 * half + (e >> 1)];
+              const int lo = 2 * (e & 1);
+              ko[e] = pack_bf16x2(q8_lane(kword, lo), q8_lane(kword, lo + 1));
+              vo[e] = pack_bf16x2(q8_lane(vword, lo), q8_lane(vword, lo + 1));
+            }
+            asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(sk + off), "r"(ko[0]), "r"(ko[1]), "r"(ko[2]), "r"(ko[3]) : "memory");
+            asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(sv + off), "r"(vo[0]), "r"(vo[1]), "r"(vo[2]), "r"(vo[3]) : "memory");
+          }
+        }
+        fence_proxy_async();
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        ksc = reinterpret_cast<const float*>(smem_raw + (base - smem_u32(smem_raw)) + C::BAR_OFF + 256 + stage * kAtQ8ScaleBytes);
+        vsc = ksc + kAtBKV;
+      }
       if constexpr (PAGED) {
         // V rows past the sequence end are cache slots nobody wrote (any bits, NaN included) and P = 0 does not cancel a NaN
         // in the PV product: zero them (whole 128 B rows, so the swizzle does not matter) before the tensor core reads them
@@ -206,6 +267,12 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(s);
+      if constexpr (Q8) {
+#pragma unroll
+        for (int jj = 0; jj < kAtBKV / 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) s[4 * jj + e] *= ksc[8 * jj + fc + (e & 1)];   // NaN scales of unwritten slots stay masked
+      }
       uint32_t pa[kAtBKV / 16][4];                             // P as the A fragments of the 4 k-steps of P V
 #pragma unroll
       for (int h2 = 0; h2 < 2; ++h2) {
@@ -232,8 +299,14 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
           const int col = 8 * jj + fc;
           const float p0 = (col >= lo && col < hi) ? exp2f(s[4 * jj + 2 * h2] * p.sl2 - m_safe) : 0.f;
           const float p1 = (col + 1 >= lo && col + 1 < hi) ? exp2f(s[4 * jj + 2 * h2 + 1] * p.sl2 - m_safe) : 0.f;
-          const __nv_bfloat162 pb = __floats2bfloat162_rn(p0, p1);
+          __nv_bfloat162 pb;
+          if constexpr (Q8) {
+            pb = __floats2bfloat162_rn(p0 > 0.f ? p0 * vsc[col] : 0.f, p1 > 0.f ? p1 * vsc[col + 1] : 0.f);
+            ls += p0 + p1;                                        // the row sum of the unscaled p
+          } else {
+          pb = __floats2bfloat162_rn(p0, p1);
           ls += __bfloat162float(pb.x) + __bfloat162float(pb.y);   // the sum of what the tensor core will actually multiply
+          }
           // k-step jj / 2: registers {row, cols 0-7 | row + 8, cols 0-7 | row, cols 8-15 | row + 8, cols 8-15}
           pa[jj >> 1][(jj & 1) * 2 + h2] = *reinterpret_cast<const uint32_t*>(&pb);
         }
@@ -339,7 +412,9 @@ static int attn_tc_init() {
     g_at_encode = reinterpret_cast<PFN_encodeTiled>(fn);
     if (cudaFuncSetAttribute(attn_prefill_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnTcCfg<64>::SMEM_BYTES) != cudaSuccess ||
         cudaFuncSetAttribute(attn_prefill_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnTcCfg<128>::SMEM_BYTES) != cudaSuccess ||
-        cudaFuncSetAttribute(attn_prefill_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnTcCfg<128>::SMEM_BYTES) != cudaSuccess) {
+        cudaFuncSetAttribute(attn_prefill_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnTcCfg<128>::SMEM_BYTES) != cudaSuccess ||
+        cudaFuncSetAttribute(attn_prefill_tc_kernel<128, true, KV_INT8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             AttnTcCfg<128>::SMEM_BYTES + kAtStages * kAtQ8ScaleBytes) != cudaSuccess) {
       set_error("attention_tc: cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError())); g_at_rc = -1;
     }
   });
@@ -356,6 +431,19 @@ static int attn_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t co
   CUresult r = g_at_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("attention_tc: cuTensorMapEncodeTiled failed (%d)", (int)r); return -1; }
+  return 0;
+}
+
+// the int8 pool's rows as a [rows][128] uint8 tensor: boxes of box_rows whole rows, no swizzle (the kernel expands them)
+static int attn_tmap_q8(CUtensorMap* m, const void* ptr, uint64_t rows, int box_rows) {
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0) { set_error("attention_tc: the int8 pool must be 16 B aligned"); return -1; }
+  cuuint64_t dims[2] = {128, rows};
+  cuuint64_t strides[1] = {128};
+  cuuint32_t box[2] = {128, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = g_at_encode(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                           CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("attention_tc: cuTensorMapEncodeTiled (uint8) failed (%d)", (int)r); return -1; }
   return 0;
 }
 
@@ -406,14 +494,19 @@ static int paged_kv_splits(int ctas, int max_kv) {
   return std::max(1, std::min(s, kAtMaxKvSplits));
 }
 
-int attention_paged(const AttnPagedCall& c, cudaStream_t st) {
+int attention_paged(const AttnPagedCall& c, cudaStream_t st, KvFormat fmt) {
   if (attn_tc_init()) return -1;
   if (c.kv.page_tokens < 8 || c.kv.page_tokens > 64 || c.kv.page_tokens % 8 != 0) { set_error("attention_paged: page_tokens %d must be a multiple of 8 <= 64", c.kv.page_tokens); return -1; }
   if (c.B < 1 || c.kv.heads < 1 || c.T < 1 || c.kv.total_pages < 1) { set_error("attention_paged: empty launch"); return -1; }
   if ((c.o_stride % 8) != 0) { set_error("attention_paged: output pitch must keep 16 B alignment"); return -1; }
+  if (fmt != KV_BF16 && fmt != KV_INT8) { set_error("attention_paged: KV cache format %d unsupported", (int)fmt); return -1; }
   CUtensorMap tq, tkv;
   if (attn_tmap(&tq, c.q, (uint64_t)c.B * c.T, (uint64_t)c.kv.heads * 128, c.q_stride)) return -1;
-  if (attn_tmap(&tkv, c.kv.pages, c.kv.row<uint64_t>(c.kv.total_pages, 0, 0), 128, 128, c.kv.page_tokens)) return -1;
+  if (fmt == KV_INT8) {
+    if (attn_tmap_q8(&tkv, c.kv.pages, c.kv.row<uint64_t>(c.kv.total_pages, 0, 0), c.kv.page_tokens)) return -1;
+  } else {
+    if (attn_tmap(&tkv, c.kv.pages, c.kv.row<uint64_t>(c.kv.total_pages, 0, 0), 128, 128, c.kv.page_tokens)) return -1;
+  }
   const int qt = (c.T + kAtBQ - 1) / kAtBQ, ctas = qt * c.kv.heads * c.B;
   const int splits = paged_kv_splits(ctas, c.max_kv);
   if (splits > 1 && (c.part == nullptr || c.counters == nullptr || (int64_t)ctas * splits > attention_paged_partials())) {
@@ -432,6 +525,11 @@ int attention_paged(const AttnPagedCall& c, cudaStream_t st) {
   int na = 0;
   if (pdl_enabled()) { attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[na].val.programmaticStreamSerializationAllowed = 1; ++na; }
   cfg.attrs = attr; cfg.numAttrs = na;
+  if (fmt == KV_INT8) {
+    cfg.dynamicSmemBytes = AttnTcCfg<128>::SMEM_BYTES + kAtStages * kAtQ8ScaleBytes;
+    VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_prefill_tc_kernel<128, true, KV_INT8>, tq, tkv, tkv, tkv, tkv, p));
+    return 0;
+  }
   VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, attn_prefill_tc_kernel<128, true>, tq, tkv, tkv, tkv, tkv, p));
   return 0;
 }

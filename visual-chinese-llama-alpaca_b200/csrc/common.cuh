@@ -36,6 +36,12 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+// int8 KV rows (KV_INT8): the load_in_8bit row quantiser (quant.cu) given the row's absmax a.  q8_inv(0) = 0 gives q = 0.
+__device__ __forceinline__ float q8_inv(float a) { return a > 0.f ? __fdiv_rn(127.f, a) : 0.f; }
+__device__ __forceinline__ float q8_step(float a) { return __fdiv_rn(a, 127.f); }
+__device__ __forceinline__ int q8_quant(float x, float inv) { return (int)fminf(fmaxf(rintf(__fmul_rn(x, inv)), -127.f), 127.f); }
+// 4 int8 lanes of a word -> fp32 (exact)
+__device__ __forceinline__ float q8_lane(uint32_t w, int i) { return (float)(int)(int8_t)(w >> (8 * i)); }
 
 // ------------------------------------------------------------------------------------------------
 // mbarrier

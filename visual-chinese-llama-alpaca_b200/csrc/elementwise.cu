@@ -734,6 +734,7 @@ int lookup_accept(const LookupCall& c, int prime, cudaStream_t st) {
 // index i of every row that references it.  Rows that share page i also share every page before it (a fork copies the parent's row;
 // only pages created after it differ), so an old row's pages that no new row keeps are a suffix of its row.
 constexpr int kReorderThreads = 1024;
+template <int FMT = KV_BF16>   // the cache format sets the bytes a copied row counts
 __global__ void __launch_bounds__(kReorderThreads, 1)
 kv_beam_reorder_kernel(int rows_old, int rows_new, const int32_t* __restrict__ parent_row, const int32_t* __restrict__ new_tok, int32_t* seq_len,
                        const KvCache kv, int32_t* table_tmp, int32_t* history, const int32_t* __restrict__ step_idx, int32_t* copy_list,
@@ -797,7 +798,7 @@ kv_beam_reorder_kernel(int rows_old, int rows_new, const int32_t* __restrict__ p
     }
     copy_list[0] = n;
     kv.state[0] = top;
-    if (cow_bytes) *cow_bytes += (unsigned long long)(rows_copied * kv.layers * kv.planes() * 128 * (long long)sizeof(bf16));
+    if (cow_bytes) *cow_bytes += (unsigned long long)(rows_copied * kv.layers * kv.planes() * (FMT == KV_INT8 ? (long long)kKvQ8RowBytes : 128 * (long long)sizeof(bf16)));
   }
   // token history: columns gathered by parent, then this step's tokens as row t (one thread per history row: in place)
   const int t = *step_idx - 1;
@@ -811,17 +812,22 @@ kv_beam_reorder_kernel(int rows_old, int rows_new, const int32_t* __restrict__ p
 }
 int kv_beam_reorder(int rows_old, int rows_new, const int32_t* parent_row, const int32_t* new_tok, int32_t* seq_len, const KvCache& kv,
                     int32_t* table_tmp, int32_t* history, const int32_t* step_idx, int32_t* copy_list, unsigned long long* cow_bytes,
-                    cudaStream_t st) {
+                    cudaStream_t st, KvFormat fmt) {
   if (rows_old < 1 || rows_new < rows_old || rows_new > 64) { set_error("kv_beam_reorder: rows %d -> %d", rows_old, rows_new); return -1; }
   const size_t smem = (size_t)((kv.total_pages + 31) / 32) * 4;
   if (smem > 200u * 1024u) { set_error("kv_beam_reorder: %d pages exceed the page bitmap", kv.total_pages); return -1; }
   static bool opted_in = false;        // the first call is vcla_prefill's fork, outside any graph capture
   if (smem > 48u * 1024u && !opted_in) {
-    VCLA_CUDA_OK(cudaFuncSetAttribute(kv_beam_reorder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    VCLA_CUDA_OK(cudaFuncSetAttribute(kv_beam_reorder_kernel<KV_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    VCLA_CUDA_OK(cudaFuncSetAttribute(kv_beam_reorder_kernel<KV_INT8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     opted_in = true;
   }
-  kv_beam_reorder_kernel<<<1, kReorderThreads, smem, st>>>(rows_old, rows_new, parent_row, new_tok, seq_len, kv, table_tmp, history, step_idx,
-                                                            copy_list, cow_bytes);
+  if (fmt == KV_INT8)
+    kv_beam_reorder_kernel<KV_INT8><<<1, kReorderThreads, smem, st>>>(rows_old, rows_new, parent_row, new_tok, seq_len, kv, table_tmp, history,
+                                                                      step_idx, copy_list, cow_bytes);
+  else
+    kv_beam_reorder_kernel<<<1, kReorderThreads, smem, st>>>(rows_old, rows_new, parent_row, new_tok, seq_len, kv, table_tmp, history, step_idx,
+                                                              copy_list, cow_bytes);
   VCLA_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -842,8 +848,32 @@ __global__ void kv_page_copy_kernel(const KvCache kv, const int32_t* __restrict_
   }
   trace.done();
 }
-int kv_page_copy(const KvCache& kv, const int32_t* copy_list, int max_entries, cudaStream_t st) {
-  kv_page_copy_kernel<<<dim3(max_entries, kv.layers), 256, 0, st>>>(kv, copy_list);
+// KV_INT8: the int8 rows (8 uint4 each) and their fp32 scales, plane by plane
+__global__ void kv_page_copy_q8_kernel(const KvCache kv, const int32_t* __restrict__ copy_list) {
+  TraceScope trace(18);
+  trace.dep();
+  const int e = blockIdx.x;
+  if (e >= copy_list[0]) return;
+  const int src = copy_list[1 + 3 * e], dst = copy_list[2 + 3 * e], n = copy_list[3 + 3 * e];
+  const KvPool layer = kv.layer(blockIdx.y);
+  const uint4* s = reinterpret_cast<const uint4*>(layer.q8_at(src, 0, 0, 0));
+  uint4* d = reinterpret_cast<uint4*>(layer.q8_at(dst, 0, 0, 0));
+  const int per_plane = n * 8, plane_stride = kv.page_tokens * 8;
+  for (int i = threadIdx.x; i < kv.planes() * per_plane; i += blockDim.x) {
+    const int plane = i / per_plane, off = i % per_plane;
+    d[(size_t)plane * plane_stride + off] = s[(size_t)plane * plane_stride + off];
+  }
+  const float* ss = layer.q8_scale(src, 0, 0, 0);
+  float* ds = layer.q8_scale(dst, 0, 0, 0);
+  for (int i = threadIdx.x; i < kv.planes() * n; i += blockDim.x) {
+    const int plane = i / n, off = i % n;
+    ds[(size_t)plane * kv.page_tokens + off] = ss[(size_t)plane * kv.page_tokens + off];
+  }
+  trace.done();
+}
+int kv_page_copy(const KvCache& kv, const int32_t* copy_list, int max_entries, cudaStream_t st, KvFormat fmt) {
+  if (fmt == KV_INT8) kv_page_copy_q8_kernel<<<dim3(max_entries, kv.layers), 256, 0, st>>>(kv, copy_list);
+  else kv_page_copy_kernel<<<dim3(max_entries, kv.layers), 256, 0, st>>>(kv, copy_list);
   VCLA_CUDA_OK(cudaGetLastError());
   return 0;
 }

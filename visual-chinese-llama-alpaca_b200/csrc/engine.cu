@@ -83,6 +83,7 @@ struct vcla_ctx {
   uint8_t* w_arena = nullptr; size_t w_bytes = 0, w_off = 0;
   uint8_t* a_arena = nullptr; size_t a_bytes = 0, a_off = 0;
   size_t kv_bytes = 0;
+  KvFormat kv_format() const { return (KvFormat)cfg.kv_format; }
   std::vector<Slot> slots;
   std::map<std::string, int> slot_index;
   // vision weights
@@ -524,6 +525,7 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   if (g.page_tokens > 64 || g.page_tokens % 8) return bad("page_tokens must be a multiple of 8 and <= 64");
   if (g.weight_format != 0 && g.weight_format != 1) return bad("weight_format must be 0 (bf16) or 1 (int8 LLaMA projections)");
   if (g.weight_format == 1 && (g.t_hidden % 64 || g.t_ffn % 64)) return bad("int8 projections need LLaMA hidden and ffn sizes that are multiples of 64");
+  if (g.kv_format != KV_BF16 && g.kv_format != KV_INT8) return bad("kv_format must be 0 (bf16) or 1 (int8 rows + fp32 row scales)");
   c->v_tokens = (g.v_image / g.v_patch) * (g.v_image / g.v_patch) + 1;
   c->kpatch = 3 * g.v_patch * g.v_patch;
   c->kpad = (c->kpatch + 63) / 64 * 64;
@@ -531,7 +533,7 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   c->kv.heads = g.t_heads; c->kv.page_tokens = g.page_tokens; c->kv.layers = g.t_layers;
   c->kv.pages_per_seq = (g.max_seq + g.page_tokens - 1) / g.page_tokens;
   c->kv.total_pages = c->kv.pages_per_seq * g.max_batch;
-  c->kv.layer_elems = c->kv.row(c->kv.total_pages, 0, 0) * 128;
+  c->kv.layer_elems = g.kv_format == KV_INT8 ? c->kv.row(c->kv.total_pages, 0, 0) * (kKvQ8RowBytes / 2) : c->kv.row(c->kv.total_pages, 0, 0) * 128;
   c->sp_qkv = pick_splits(3 * g.t_hidden, g.t_hidden);
   c->sp_o = pick_splits(g.t_hidden, g.t_hidden);
   c->sp_gu = pick_splits(2 * g.t_ffn, g.t_hidden);
@@ -549,6 +551,7 @@ int vcla_create(const vcla_config* cfg, vcla_ctx** out) {
   cudaError_t e;
   if ((e = cudaMalloc(&c->w_arena, c->w_bytes)) != cudaSuccess || (e = cudaMalloc(&c->a_arena, c->a_bytes)) != cudaSuccess ||
       (e = cudaMalloc(&c->kv.pages, c->kv_bytes)) != cudaSuccess) {
+    (void)cudaGetLastError();   // a failed allocation must not surface as the error of the next context's first launch
     set_error("vcla_create: cudaMalloc failed (%s): weights %.2f GB, activations %.2f GB, kv %.2f GB", cudaGetErrorString(e),
               c->w_bytes / 1e9, c->a_bytes / 1e9, c->kv_bytes / 1e9);
     vcla_destroy(c);
@@ -807,6 +810,12 @@ int vcla_kv_read_pages(vcla_ctx* c, int32_t* table_host, int32_t* npages_host, i
   if (state_host) VCLA_CUDA_OK(cudaMemcpy(state_host, c->kv.state, 8, cudaMemcpyDeviceToHost));
   return 0;
 }
+int vcla_kv_read_layer(vcla_ctx* c, int layer, void* host) {
+  if (!c || !host || layer < 0 || layer >= c->kv.layers) { set_error("vcla_kv_read_layer: bad arguments"); return -1; }
+  VCLA_CUDA_OK(cudaDeviceSynchronize());
+  VCLA_CUDA_OK(cudaMemcpy(host, c->kv.layer(layer).pages, c->kv_bytes / c->kv.layers, cudaMemcpyDeviceToHost));
+  return 0;
+}
 int vcla_kv_geometry(const vcla_ctx* c, int* pages_per_seq, int* total_pages, int* page_tokens) {
   if (!c) return -1;
   if (pages_per_seq) *pages_per_seq = c->kv.pages_per_seq;
@@ -1062,6 +1071,7 @@ static int prefill_layers(vcla_ctx* c, int B, int S, const int32_t* left_pad, in
       gc.rope.cos = c->rope_cos; gc.rope.sin = c->rope_sin; gc.rope.kv = c->kv.layer(i);
       gc.rope.S = S; gc.rope.T = TH; gc.rope.left_pad = left_pad; gc.rope.pos_from_mask = pos_from_mask;
       gc.rope.base_len = base_len;
+      gc.kv_format = c->kv_format();
       count(c); if (gemm_tc(gc, st)) return -1;
     }
     if (base_len == nullptr) {
@@ -1071,7 +1081,7 @@ static int prefill_layers(vcla_ctx* c, int B, int S, const int32_t* left_pad, in
     } else {
       AttnPagedCall a; a.q = c->qkv; a.q_stride = 3 * TH; a.kv = c->kv.layer(i); a.base_len = base_len; a.max_kv = (int)c->len_bound + S;
       a.out = c->attn; a.o_stride = TH; a.B = B; a.T = S; a.scale = scale; a.part = c->pa_part; a.counters = c->pa_counters;
-      count(c); if (attention_paged(a, st)) return -1;
+      count(c); if (attention_paged(a, st, c->kv_format())) return -1;
     }
     {
       GemmCall gc; if (weight(L.wo, L.qo, TH, TH, gc, L.so)) return -1;
@@ -1200,9 +1210,9 @@ int vcla_prefill_extend(vcla_ctx* c, const int64_t* ids, int B, int T, float* lo
 static int beam_reorder(vcla_ctx* c, int rows_old, int rows_new, const int32_t* tok, cudaStream_t st) {
   count(c, 2);
   if (kv_beam_reorder(rows_old, rows_new, c->beam_parent, tok, c->seq_len, c->kv, c->beam_table_tmp, c->tok_hist, c->step_idx, c->beam_copy,
-                      c->beam_cow_bytes, st))
+                      c->beam_cow_bytes, st, c->kv_format()))
     return -1;
-  return kv_page_copy(c->kv, c->beam_copy, rows_new, st);
+  return kv_page_copy(c->kv, c->beam_copy, rows_new, st, c->kv_format());
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1253,7 +1263,7 @@ static int ws_stack(vcla_ctx* c, const int32_t* tok_in, int B, cudaStream_t st) 
     const TextLayer& L = c->tl[i];
     count(c); if (dec_resid_norm(i == 0 ? nullptr : c->ws_d, c->sp_d, B, c->d_resid, B, TH, L.ln1, g.t_eps, c->d_xn, st)) return -1;
     if (ws_gemm(c, DG_QKV, i, B, st)) return -1;
-    count(c); if (attention_decode(decode_attn_call(c, i, B, c->sp_qkv), st)) return -1;
+    count(c); if (attention_decode(decode_attn_call(c, i, B, c->sp_qkv), st, c->kv_format())) return -1;
     if (ws_gemm(c, DG_O, i, B, st)) return -1;
     count(c); if (dec_resid_norm(c->ws_o, c->sp_o, B, c->d_resid, B, TH, L.ln2, g.t_eps, c->d_xn, st)) return -1;
     if (ws_gemm(c, DG_GATE_UP, i, B, st)) return -1;
@@ -1277,9 +1287,9 @@ static int csk_stack(vcla_ctx* c, const int32_t* tok_in, int B, bool lookup, cud
     if (lookup) {
       DecodeAttnCall a = decode_attn_call(c, i, 1, 1);
       a.B = B; a.ws_rows = B;
-      count(c, 2); if (attention_decode_lookup(a, st)) return -1;
+      count(c, 2); if (attention_decode_lookup(a, st, c->kv_format())) return -1;
     } else {
-      count(c); if (attention_decode(decode_attn_call(c, i, B, 1), st)) return -1;
+      count(c); if (attention_decode(decode_attn_call(c, i, B, 1), st, c->kv_format())) return -1;
     }
     if (csk_gemm(c, DG_O, i, B, st) || csk_gemm(c, DG_GATE_UP, i, B, st) || csk_gemm(c, DG_DOWN, i, B, st)) return -1;
   }
@@ -1961,7 +1971,7 @@ int vcla_debug_get_csk_splits(vcla_ctx* c, int B, int* out5) {
 int vcla_debug_decode_ctas_per_sm(vcla_ctx* c, int B, int* out2) {
   if (!c || !out2 || B < 1 || B > csk_max_batch(c)) { set_error("vcla_debug_decode_ctas_per_sm: bad arguments"); return -1; }
   out2[0] = gemm_csk_ctas_per_sm(B, c->cfg.weight_format == 1);
-  out2[1] = attention_decode_ctas_per_sm(decode_attn_call(c, 0, B, 1));
+  out2[1] = attention_decode_ctas_per_sm(decode_attn_call(c, 0, B, 1), c->kv_format());
   return out2[0] > 0 && out2[1] > 0 ? 0 : -1;
 }
 int vcla_op_gemm_csk_clusters(int B, int splits) { return gemm_csk_clusters(B, splits); }
@@ -2020,35 +2030,56 @@ static KvPool op_pool(const void* pages, const int32_t* table, int pages_per_seq
   return kv;
 }
 
-int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, const int32_t* page_table, int pages_per_seq, int page_tokens,
-                            const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T, float scale, vcla_stream stream) {
-  // operator entry for tests: the pool extent and the longest sequence are read back from the caller's table and lengths, the
+// int8 pools: the caller's total_pages places the scale region, so every page the call reads must lie below it
+static int op_check_q8_extent(const char* who, KvFormat fmt, const KvPool& kv, int total_pages) {
+  if (fmt == KV_INT8 && kv.total_pages > total_pages) {
+    set_error("%s: page %d is outside the %d-page int8 pool", who, kv.total_pages - 1, total_pages); return -1;
+  }
+  return 0;
+}
+static int op_attention_paged(KvFormat fmt, const void* q, int q_stride, const void* kv_pages, int total_pages, const int32_t* page_table,
+                              int pages_per_seq, int page_tokens, const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T,
+                              float scale, vcla_stream stream) {
+  // operator entry for tests: the pool extent (bf16) and the longest sequence are read back from the caller's table and lengths, the
   // split-KV scratch is allocated for the call.  Synchronises.
-  if (!q || !kv_pages || !page_table || !base_len_dev || !out || B < 1 || B > 64 || H < 1 || T < 1 || pages_per_seq < 1) {
+  if (!q || !kv_pages || !page_table || !base_len_dev || !out || B < 1 || B > 64 || H < 1 || T < 1 || pages_per_seq < 1 ||
+      (fmt == KV_INT8 && total_pages < 1)) {
     set_error("vcla_op_attention_paged: bad arguments"); return -1;
   }
   cudaStream_t st = (cudaStream_t)stream;
   KvPool kv = op_pool(kv_pages, page_table, pages_per_seq, page_tokens, H);
   const int longest = op_check_pages("vcla_op_attention_paged", kv, base_len_dev, B, T, st);
-  if (longest < 0) return -1;
+  if (longest < 0 || op_check_q8_extent("vcla_op_attention_paged", fmt, kv, total_pages)) return -1;
+  if (fmt == KV_INT8) kv.total_pages = total_pages;
   const int n = attention_paged_partials();
   void* scratch = nullptr;
   VCLA_CUDA_OK(cudaMalloc(&scratch, (size_t)n * kAttnPartialFloats * 4 + (size_t)n * 4));
   int32_t* counters = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(scratch) + (size_t)n * kAttnPartialFloats);
   AttnPagedCall a; a.q = (const bf16*)q; a.q_stride = q_stride; a.kv = kv; a.base_len = base_len_dev; a.max_kv = longest + T;
   a.out = (bf16*)out; a.o_stride = o_stride; a.B = B; a.T = T; a.scale = scale; a.part = reinterpret_cast<float*>(scratch); a.counters = counters;
-  int rc = cudaMemsetAsync(counters, 0, (size_t)n * 4, st) == cudaSuccess ? attention_paged(a, st) : -1;
+  int rc = cudaMemsetAsync(counters, 0, (size_t)n * 4, st) == cudaSuccess ? attention_paged(a, st, fmt) : -1;
   if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_attention_paged: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
   cudaFree(scratch);
   return rc;
 }
-int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq, int page_tokens,
-                             const int32_t* seq_len_dev, void* out, int B, int H, int kv_splits, float scale, float rope_theta, int persistent,
-                             int persistent_grid, int launches, vcla_stream stream) {
+int vcla_op_attention_paged(const void* q, int q_stride, const void* kv_pages, const int32_t* page_table, int pages_per_seq, int page_tokens,
+                            const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T, float scale, vcla_stream stream) {
+  return op_attention_paged(KV_BF16, q, q_stride, kv_pages, 0, page_table, pages_per_seq, page_tokens, base_len_dev, out, o_stride, B, H, T,
+                            scale, stream);
+}
+int vcla_op_attention_paged_q8(const void* q, int q_stride, const void* kv_pool, int total_pages, const int32_t* page_table, int pages_per_seq,
+                               int page_tokens, const int32_t* base_len_dev, void* out, int o_stride, int B, int H, int T, float scale,
+                               vcla_stream stream) {
+  return op_attention_paged(KV_INT8, q, q_stride, kv_pool, total_pages, page_table, pages_per_seq, page_tokens, base_len_dev, out, o_stride, B,
+                            H, T, scale, stream);
+}
+static int op_attention_decode(KvFormat fmt, const float* qkv_partial, int splits, void* kv_pages, int total_pages, const int32_t* page_table,
+                               int pages_per_seq, int page_tokens, const int32_t* seq_len_dev, void* out, int B, int H, int kv_splits, float scale,
+                               float rope_theta, int persistent, int persistent_grid, int launches, vcla_stream stream) {
   // operator entry for tests: goes through attention_decode() (the dispatch is under test too); the RoPE tables, the combine scratch
   // and the arrival counters are made for the call.  Everything a kernel would index with is checked here first.  Synchronises.
   if (!qkv_partial || !kv_pages || !page_table || !seq_len_dev || !out || splits < 1 || B < 1 || B > 64 || H < 1 || pages_per_seq < 1 ||
-      page_tokens < 1 || launches < 1 || persistent_grid < 0 || !(rope_theta > 0.f)) {
+      page_tokens < 1 || launches < 1 || persistent_grid < 0 || !(rope_theta > 0.f) || (fmt == KV_INT8 && total_pages < 1)) {
     set_error("vcla_op_attention_decode: bad arguments"); return -1;
   }
   if (kv_splits < 1 || kv_splits > 8) { set_error("vcla_op_attention_decode: kv_splits %d outside 1..8", kv_splits); return -1; }
@@ -2057,7 +2088,8 @@ int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_page
   cudaStream_t st = (cudaStream_t)stream;
   KvPool kv = op_pool(kv_pages, page_table, pages_per_seq, page_tokens, H);
   const int max_len = op_check_pages("vcla_op_attention_decode", kv, seq_len_dev, B, 1, st);
-  if (max_len < 0) return -1;
+  if (max_len < 0 || op_check_q8_extent("vcla_op_attention_decode", fmt, kv, total_pages)) return -1;
+  if (fmt == KV_INT8) kv.total_pages = total_pages;
   const size_t rope_floats = (size_t)(max_len + 1) * 64, scratch_floats = (size_t)B * H * kv_splits * (128 + 2);
   float* buf = nullptr;
   VCLA_CUDA_OK(cudaMalloc(&buf, (2 * rope_floats + scratch_floats + (size_t)B * H) * 4));
@@ -2072,25 +2104,38 @@ int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_page
   // element the last launch did not write cannot pass for one an earlier launch wrote
   for (int i = 0; i < launches && rc == 0; ++i) {
     if (cudaMemsetAsync(out, 0xff, (size_t)B * H * 128 * 2, st) != cudaSuccess) { set_error("vcla_op_attention_decode: memset failed"); rc = -1; break; }
-    rc = attention_decode(a, st);
+    rc = attention_decode(a, st, fmt);
   }
   if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_attention_decode: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
   cudaFree(buf);
   return rc;
 }
-int vcla_op_attention_decode_lookup(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq,
-                                    int page_tokens, const int32_t* seq_len_dev, void* out, int rows, int H, int kv_splits, float scale,
-                                    float rope_theta, vcla_stream stream) {
+int vcla_op_attention_decode(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq, int page_tokens,
+                             const int32_t* seq_len_dev, void* out, int B, int H, int kv_splits, float scale, float rope_theta, int persistent,
+                             int persistent_grid, int launches, vcla_stream stream) {
+  return op_attention_decode(KV_BF16, qkv_partial, splits, kv_pages, 0, page_table, pages_per_seq, page_tokens, seq_len_dev, out, B, H, kv_splits,
+                             scale, rope_theta, persistent, persistent_grid, launches, stream);
+}
+int vcla_op_attention_decode_q8(const float* qkv_partial, int splits, void* kv_pool, int total_pages, const int32_t* page_table, int pages_per_seq,
+                                int page_tokens, const int32_t* seq_len_dev, void* out, int B, int H, int kv_splits, float scale, float rope_theta,
+                                int persistent, int persistent_grid, int launches, vcla_stream stream) {
+  return op_attention_decode(KV_INT8, qkv_partial, splits, kv_pool, total_pages, page_table, pages_per_seq, page_tokens, seq_len_dev, out, B, H,
+                             kv_splits, scale, rope_theta, persistent, persistent_grid, launches, stream);
+}
+static int op_attention_decode_lookup(KvFormat fmt, const float* qkv_partial, int splits, void* kv_pages, int total_pages, const int32_t* page_table,
+                                      int pages_per_seq, int page_tokens, const int32_t* seq_len_dev, void* out, int rows, int H, int kv_splits,
+                                      float scale, float rope_theta, vcla_stream stream) {
   // operator entry for tests: attention_decode_lookup on caller buffers; the RoPE tables, scratch and counters are made for the call.
   if (!qkv_partial || !kv_pages || !page_table || !seq_len_dev || !out || splits < 1 || rows < 2 || rows > 16 || H < 1 || pages_per_seq < 1 ||
-      page_tokens < 1 || !(rope_theta > 0.f)) {
+      page_tokens < 1 || !(rope_theta > 0.f) || (fmt == KV_INT8 && total_pages < 1)) {
     set_error("vcla_op_attention_decode_lookup: bad arguments"); return -1;
   }
   if (kv_splits < 1 || kv_splits > 8) { set_error("vcla_op_attention_decode_lookup: kv_splits %d outside 1..8", kv_splits); return -1; }
   cudaStream_t st = (cudaStream_t)stream;
   KvPool kv = op_pool(kv_pages, page_table, pages_per_seq, page_tokens, H);
   const int len = op_check_pages("vcla_op_attention_decode_lookup", kv, seq_len_dev, 1, rows, st);
-  if (len < 0) return -1;
+  if (len < 0 || op_check_q8_extent("vcla_op_attention_decode_lookup", fmt, kv, total_pages)) return -1;
+  if (fmt == KV_INT8) kv.total_pages = total_pages;
   const size_t rope_floats = (size_t)(len + rows) * 64, scratch_floats = (size_t)rows * H * kv_splits * (128 + 2);
   float* buf = nullptr;
   VCLA_CUDA_OK(cudaMalloc(&buf, (2 * rope_floats + scratch_floats + (size_t)rows * H) * 4));
@@ -2100,10 +2145,22 @@ int vcla_op_attention_decode_lookup(const float* qkv_partial, int splits, void* 
   a.scratch = buf + 2 * rope_floats; a.counters = reinterpret_cast<int32_t*>(a.scratch + scratch_floats);
   int rc = rope_fill_tables(len + rows, 128, rope_theta, buf, buf + rope_floats);
   if (rc == 0 && cudaMemsetAsync(a.scratch, 0, (scratch_floats + (size_t)rows * H) * 4, st) != cudaSuccess) { set_error("vcla_op_attention_decode_lookup: memset failed"); rc = -1; }
-  if (rc == 0) rc = attention_decode_lookup(a, st);
+  if (rc == 0) rc = attention_decode_lookup(a, st, fmt);
   if (cudaStreamSynchronize(st) != cudaSuccess && rc == 0) { set_error("vcla_op_attention_decode_lookup: %s", cudaGetErrorString(cudaGetLastError())); rc = -1; }
   cudaFree(buf);
   return rc;
+}
+int vcla_op_attention_decode_lookup(const float* qkv_partial, int splits, void* kv_pages, const int32_t* page_table, int pages_per_seq,
+                                    int page_tokens, const int32_t* seq_len_dev, void* out, int rows, int H, int kv_splits, float scale,
+                                    float rope_theta, vcla_stream stream) {
+  return op_attention_decode_lookup(KV_BF16, qkv_partial, splits, kv_pages, 0, page_table, pages_per_seq, page_tokens, seq_len_dev, out, rows, H,
+                                    kv_splits, scale, rope_theta, stream);
+}
+int vcla_op_attention_decode_lookup_q8(const float* qkv_partial, int splits, void* kv_pool, int total_pages, const int32_t* page_table,
+                                       int pages_per_seq, int page_tokens, const int32_t* seq_len_dev, void* out, int rows, int H, int kv_splits,
+                                       float scale, float rope_theta, vcla_stream stream) {
+  return op_attention_decode_lookup(KV_INT8, qkv_partial, splits, kv_pool, total_pages, page_table, pages_per_seq, page_tokens, seq_len_dev, out,
+                                    rows, H, kv_splits, scale, rope_theta, stream);
 }
 int vcla_op_logits_argmax(const float* partial, int splits, int ldp, int B, int V, float* logits_out, int32_t* tok_out, vcla_stream stream) {
   // operator entry for tests: dec_logits_argmax without token history or data-parallel send buffer.  Synchronises.

@@ -95,7 +95,9 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   return x;
 }
 
-template <int BM, int BN, int STAGES, bool SWAP>
+// KVF = KV_INT8 (the fused QKV epilogue of an int8 KV cache only): every k / v head row is quantised (kernels.h: KvPool), its q and
+// s go to the cache and bf16(q * s) to the k / v columns of the output, so the prefill attention reads what the cache holds.
+template <int BM, int BN, int STAGES, bool SWAP, int KVF = KV_BF16>
 __global__ void __launch_bounds__(kGemmThreads, SWAP ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using C = GemmCfg<BM, BN, STAGES>;
@@ -313,6 +315,48 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     const int hcol = col_tile + hh * 128;                  // first column of this head inside [q | k | v]
                     if (hcol < p.N) {
                       const int region = hcol / R.T, head = (hcol % R.T) / 128;
+                      if constexpr (KVF == KV_INT8) {
+                        if (region >= 1) {
+                          // the 4 lanes of a quad hold the row's 128 dims: 32 values each, absmax in two quad shuffles
+                          float x[32];
+#pragma unroll
+                          for (int jj = 0; jj < 8; ++jj) {
+                            const int d = 8 * jj + fc;
+                            float lo0 = ACC(hh * 16 + jj, 0) * rs, lo1 = ACC(hh * 16 + jj, 1) * rs;
+                            float hi0 = ACC(hh * 16 + jj + 8, 0) * rs, hi1 = ACC(hh * 16 + jj + 8, 1) * rs;
+                            if (region < 2 && cached) {
+                              const float2 c2 = __ldg(reinterpret_cast<const float2*>(ct + d));
+                              const float2 s2 = __ldg(reinterpret_cast<const float2*>(stb + d));
+                              const float a0 = lo0, b0 = hi0, a1 = lo1, b1 = hi1;
+                              lo0 = a0 * c2.x - b0 * s2.x; hi0 = b0 * c2.x + a0 * s2.x;
+                              lo1 = a1 * c2.y - b1 * s2.y; hi1 = b1 * c2.y + a1 * s2.y;
+                            }
+                            x[4 * jj] = lo0; x[4 * jj + 1] = lo1; x[4 * jj + 2] = hi0; x[4 * jj + 3] = hi1;
+                          }
+                          float a = 0.f;
+#pragma unroll
+                          for (int i = 0; i < 32; ++i) a = fmaxf(a, fabsf(x[i]));
+                          const unsigned qmask = 0xfu << (lane & 28);
+                          a = fmaxf(a, __shfl_xor_sync(qmask, a, 1));
+                          a = fmaxf(a, __shfl_xor_sync(qmask, a, 2));
+                          const float inv = q8_inv(a), sc = q8_step(a);
+                          int8_t* qdst = cached ? R.kv.q8_at(page, region - 1, head, slot) : nullptr;
+#pragma unroll
+                          for (int jj = 0; jj < 8; ++jj) {
+                            const int d = 8 * jj + fc;
+                            const int q0 = q8_quant(x[4 * jj], inv), q1 = q8_quant(x[4 * jj + 1], inv);
+                            const int q2 = q8_quant(x[4 * jj + 2], inv), q3 = q8_quant(x[4 * jj + 3], inv);
+                            *reinterpret_cast<uint32_t*>(orow_ptr + hcol + d) = pack_bf16x2(__fmul_rn((float)q0, sc), __fmul_rn((float)q1, sc));
+                            *reinterpret_cast<uint32_t*>(orow_ptr + hcol + 64 + d) = pack_bf16x2(__fmul_rn((float)q2, sc), __fmul_rn((float)q3, sc));
+                            if (qdst != nullptr) {
+                              *reinterpret_cast<uint16_t*>(qdst + d) = (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8));
+                              *reinterpret_cast<uint16_t*>(qdst + 64 + d) = (uint16_t)((q2 & 0xff) | ((q3 & 0xff) << 8));
+                            }
+                          }
+                          if (qdst != nullptr && (lane & 3) == 0) *R.kv.q8_scale(page, region - 1, head, slot) = sc;
+                          continue;
+                        }
+                      }
                       bf16* cdst = (region >= 1 && cached) ? R.kv.at(page, region - 1, head, slot) : nullptr;
 #pragma unroll
                       for (int jj = 0; jj < 8; ++jj) {                     // dims d = 8 jj + fc (+1) pair with d + 64 (HF rotate_half)
@@ -436,10 +480,10 @@ static PFN_encodeTiled g_encode = nullptr;
 static std::once_flag g_gemm_once;
 static int g_gemm_init_rc = 0;
 
-template <int BM, int BN, int STAGES, bool SWAP>
+template <int BM, int BN, int STAGES, bool SWAP, int KVF = KV_BF16>
 static int set_attr() {
   using C = GemmCfg<BM, BN, STAGES>;
-  VCLA_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BM, BN, STAGES, SWAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+  VCLA_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BM, BN, STAGES, SWAP, KVF>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
   return 0;
 }
 
@@ -455,6 +499,7 @@ static int gemm_init_impl() {
   }
   g_encode = reinterpret_cast<PFN_encodeTiled>(fn);
   if (set_attr<64, 256, 5, false>()) return -1;
+  if (set_attr<64, 256, 5, false, KV_INT8>()) return -1;
   if (set_attr<128, 128, 6, false>()) return -1;
   if (set_attr<128, 64, 8, false>()) return -1;
   if (set_attr<128, 16, 5, true>()) return -1;
@@ -487,7 +532,7 @@ static int make_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t co
   return 0;
 }
 
-template <int BM, int BN, int STAGES, bool SWAP>
+template <int BM, int BN, int STAGES, bool SWAP, int KVF = KV_BF16>
 static int launch(const GemmCall& c, GemmParams p, cudaStream_t st) {
   using C = GemmCfg<BM, BN, STAGES>;
   CUtensorMap ta, tb;
@@ -518,11 +563,11 @@ static int launch(const GemmCall& c, GemmParams p, cudaStream_t st) {
     if (!once) {
       once = true;
       int per_sm = -1;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_tc_kernel<BM, BN, STAGES, SWAP>, kGemmThreads, C::SMEM_BYTES);
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gemm_tc_kernel<BM, BN, STAGES, SWAP, KVF>, kGemmThreads, C::SMEM_BYTES);
       fprintf(stderr, "[vcla] gemm_tc<%d,%d,%d,%d>: smem %d, occupancy query %d blocks/SM, grid %d\n", BM, BN, STAGES, (int)SWAP, C::SMEM_BYTES, per_sm, grid);
     }
   }
-  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BM, BN, STAGES, SWAP>, ta, tb, p));
+  VCLA_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BM, BN, STAGES, SWAP, KVF>, ta, tb, p));
   return 0;
 }
 
@@ -574,6 +619,8 @@ int gemm_tc(const GemmCall& c, cudaStream_t st) {
   if (c.rope.cos != nullptr && !(c.mode == GEMM_STORE_BF16 && c.N == 3 * c.rope.T && c.rope.T % 128 == 0 && c.bias == nullptr && c.act == ACT_NONE && c.rows_per_group == 0 && (c.ldo % 8) == 0)) {
     set_error("gemm: the RoPE + KV-append epilogue needs the plain fused QKV projection (N = 3T, T %% 128 == 0)"); return -1;
   }
+  if (c.kv_format != KV_BF16 && (c.rope.cos == nullptr || c.kv_format != KV_INT8)) { set_error("gemm: KV cache format %d needs the fused QKV epilogue", c.kv_format); return -1; }
+  if (c.kv_format == KV_INT8) return launch<64, 256, 5, false, KV_INT8>(c, p, st);
   int bn = c.bn;
   if (c.rope.cos != nullptr) bn = 256;    // two whole heads per tile
   if (bn == 0) bn = gemm_pick_bn(c.M, c.N);

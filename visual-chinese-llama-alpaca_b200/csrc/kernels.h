@@ -42,6 +42,15 @@ enum Act { ACT_NONE = 0, ACT_QUICK_GELU = 1, ACT_GELU_ERF = 2 };
 // every (page, K|V, head) plane is page_tokens contiguous 128-wide rows.  Sequence b's i-th page is table[b][i]: its token t sits in
 // slot t % page_tokens of page table[b][t / page_tokens].  This struct is the only place that knows the layout.  It is a field of the
 // decode and prefill attention parameter blocks: keep it at 32 bytes, larger blocks change how those kernels are compiled.
+//
+// The int8 format (KV_INT8, kv_cache_dtype="int8") keeps the same page geometry: `pages` points at the layer's int8 rows
+// [total_pages][K|V][heads][page_tokens][128] (row(...) * 128 bytes in), followed by one fp32 scale per row in the same order, so a
+// (page, K|V, head) plane is page_tokens x 128 contiguous bytes and its scales page_tokens x 4 contiguous bytes (16 B aligned for
+// page_tokens % 8 == 0).  A row holds q = clamp(rint(x * (127 / a)), -127, 127) and s = a / 127 with a = max |x| (the load_in_8bit
+// quantiser); attention reads q * s.  The format is a template parameter of the kernels that read the pool, never a field: the
+// scale region is derived from total_pages, and a bf16 kernel compiles exactly as it does without the int8 format.
+enum KvFormat { KV_BF16 = 0, KV_INT8 = 1 };
+constexpr int kKvQ8RowBytes = 128 + 4;   // int8 row + its fp32 scale
 struct KvPool {
   bf16* pages = nullptr;
   int32_t* table = nullptr;          // [sequences][pages_per_seq]
@@ -53,6 +62,13 @@ struct KvPool {
     return (((I)page * 2 + kv) * heads + head) * page_tokens + slot;
   }
   __host__ __device__ __forceinline__ bf16* at(int page, int kv, int head, int slot) const { return pages + row(page, kv, head, slot) * 128; }
+  // KV_INT8: the int8 row and its scale
+  __host__ __device__ __forceinline__ int8_t* q8_at(int page, int kv, int head, int slot) const {
+    return reinterpret_cast<int8_t*>(pages) + row(page, kv, head, slot) * 128;
+  }
+  __host__ __device__ __forceinline__ float* q8_scale(int page, int kv, int head, int slot) const {
+    return reinterpret_cast<float*>(reinterpret_cast<int8_t*>(pages) + row(total_pages, 0, 0) * 128) + row(page, kv, head, slot);
+  }
   __host__ __device__ __forceinline__ int planes() const { return 2 * heads; }   // (K|V, head) planes of a page
   __host__ __device__ __forceinline__ int32_t* seq_pages(int b) const { return table + (size_t)b * pages_per_seq; }
   // pages that hold n tokens, clamped to a table row
@@ -68,7 +84,7 @@ struct KvCache : KvPool {
   int32_t* state = nullptr;          // {free pages, exhausted flag}
   int32_t* npages = nullptr;         // [sequences] pages owned: table[b][0 .. npages[b])
   int layers = 1;
-  size_t layer_elems = 0;            // = row(total_pages, 0, 0) * 128, set with the geometry
+  size_t layer_elems = 0;            // layer stride in bf16 units: row(total_pages, 0, 0) * 128, or * 132 / 2 for KV_INT8
   __host__ __device__ __forceinline__ KvPool layer(int i) const { KvPool v = *this; v.pages += i * layer_elems; return v; }
 };
 
@@ -124,6 +140,7 @@ struct GemmCall {
   GemmEmitNorm emit;         // ADD_F32 + accumulate: also write the next operand + row statistics
   GemmRope rope;             // STORE_BF16: RoPE + KV-cache append (runs on the 64 x 256 tile, N = 3T)
   const float* colscale = nullptr;   // [N] or null: acc[row, col] *= colscale[col] before every epilogue (per-row scales of int8 weights)
+  int kv_format = KV_BF16;           // rope.kv's format: KV_INT8 quantises each k / v head row, caches q and s, and stores bf16(q * s)
 };
 int gemm_tc(const GemmCall& c, cudaStream_t st);
 int gemm_pick_bn(int M, int N);   // tile width gemm_tc picks for a non-swap GEMM (= the number of ssq slots per row it emits: ceil(N / bn))
@@ -193,7 +210,7 @@ struct AttnPagedCall {
   float scale = 1.f;
   float* part = nullptr; int32_t* counters = nullptr;
 };
-int attention_paged(const AttnPagedCall& c, cudaStream_t st);
+int attention_paged(const AttnPagedCall& c, cudaStream_t st, KvFormat fmt = KV_BF16);   // fmt: c.kv's format
 int attention_paged_partials();   // (query tile, head, sequence, split) partials a split launch may need at most
 constexpr int kAttnPartialFloats = 64 * 132;
 
@@ -212,12 +229,12 @@ struct DecodeAttnCall {
   int persistent_grid = 0;             // VCLA_ATTN_PERSISTENT_GRID
   KvPool kv;                           // this layer's view (kv.heads heads of HD = 128)
 };
-int attention_decode(const DecodeAttnCall& c, cudaStream_t st);
+int attention_decode(const DecodeAttnCall& c, cudaStream_t st, KvFormat fmt = KV_BF16);   // fmt: c.kv's format
 // Prompt lookup verification over c.B <= 16 query rows of sequence 0 (row r at position seq_len[0] + r, qkv / out row r): two launches,
 // the K/V append of every row, then each row's attention over keys [0, seq_len[0] + r] with the one-token kernel's arithmetic at that
 // length (c.kv_splits must be the split count the one-token call of sequence 0 uses).  scratch / counters are indexed by row.
-int attention_decode_lookup(const DecodeAttnCall& c, cudaStream_t st);
-int attention_decode_ctas_per_sm(const DecodeAttnCall& c);     // resident CTAs per SM of the kernel attention_decode picks for c
+int attention_decode_lookup(const DecodeAttnCall& c, cudaStream_t st, KvFormat fmt = KV_BF16);
+int attention_decode_ctas_per_sm(const DecodeAttnCall& c, KvFormat fmt = KV_BF16);     // resident CTAs per SM of the kernel attention_decode picks for c
 int attention_init();          // sets the dynamic-smem attributes and reads the VCLA_ATTN_* switches once (call outside graph capture)
 
 // ------------------------------------------------------------------------------------------
@@ -374,9 +391,9 @@ int lookup_accept(const LookupCall& c, int prime, cudaStream_t st);
 // of dynamic shared memory).  cow_bytes (nullable) accumulates the bytes of the copied rows over every layer.
 int kv_beam_reorder(int rows_old, int rows_new, const int32_t* parent_row, const int32_t* new_tok, int32_t* seq_len, const KvCache& kv,
                     int32_t* table_tmp, int32_t* history, const int32_t* step_idx, int32_t* copy_list, unsigned long long* cow_bytes,
-                    cudaStream_t st);
+                    cudaStream_t st, KvFormat fmt = KV_BF16);
 // copies the copy list's rows of every layer (K and V, every head) from src to dst page; fixed grid (max_entries x layers)
-int kv_page_copy(const KvCache& kv, const int32_t* copy_list, int max_entries, cudaStream_t st);
+int kv_page_copy(const KvCache& kv, const int32_t* copy_list, int max_entries, cudaStream_t st, KvFormat fmt = KV_BF16);
 // fp32 RoPE tables [max_pos][head_dim/2], computed on the host the way HF does and uploaded to cos_dev / sin_dev
 int rope_fill_tables(int max_pos, int head_dim, float theta, float* cos_dev, float* sin_dev);
 

@@ -19,7 +19,7 @@ class VclaConfig(C.Structure):
         ("t_hidden", C.c_int), ("t_layers", C.c_int), ("t_heads", C.c_int), ("t_ffn", C.c_int),
         ("t_vocab", C.c_int), ("t_eps", C.c_float), ("rope_theta", C.c_float),
         ("max_batch", C.c_int), ("max_seq", C.c_int), ("max_prefill_tokens", C.c_int), ("page_tokens", C.c_int),
-        ("weight_format", C.c_int),
+        ("weight_format", C.c_int), ("kv_format", C.c_int),
     ]
 
 
@@ -63,6 +63,7 @@ _SIGNATURES = [
     ("vcla_load_weight_q8", C.c_int, [_P, C.c_char_p, _P, _P, C.c_int, _P]),
     ("vcla_reset", C.c_int, [_P, _P]),
     ("vcla_kv_geometry", C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    ("vcla_kv_read_layer", C.c_int, [_P, C.c_int, _P]),
     ("vcla_kv_read_pages", C.c_int, [_P, _P, _P, _P]),
     ("vcla_kv_debug_shuffle", C.c_int, [_P, C.c_uint32]),
     ("vcla_kv_truncate", C.c_int, [_P, _P, C.c_int, _P]),
@@ -113,6 +114,12 @@ _SIGNATURES = [
                                            C.c_float, C.c_int, C.c_int, C.c_int, _P]),
     ("vcla_op_attention_decode_lookup", C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float,
                                                   C.c_float, _P]),
+    ("vcla_op_attention_paged_q8", C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int,
+                                             C.c_float, _P]),
+    ("vcla_op_attention_decode_q8", C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float,
+                                              C.c_float, C.c_int, C.c_int, C.c_int, _P]),
+    ("vcla_op_attention_decode_lookup_q8", C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int,
+                                                     C.c_float, C.c_float, _P]),
     ("vcla_op_logits_argmax", C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     ("vcla_op_layernorm", C.c_int, [_P, C.c_int, C.c_int, _P, _P, C.c_float, _P, _P, _P]),
     ("vcla_op_rmsnorm", C.c_int, [_P, C.c_int, C.c_int, _P, C.c_float, _P, _P]),

@@ -22,11 +22,22 @@ def path_config_7b() -> Dict:
                 t_hidden=4096, t_layers=32, t_heads=32, t_ffn=11008, t_vocab=49958, t_eps=1e-6, rope_theta=10000.0)
 
 
+def kv_format_of(kv_cache_dtype) -> int:
+    """kv_cache_dtype of the model constructors -> Engine kv_format: "int8" / torch.int8 select the int8 KV cache; None, "bfloat16"
+    and torch.bfloat16 the bf16 one.  The cache format is fixed when the engine is built."""
+    if kv_cache_dtype is None or kv_cache_dtype in ("bfloat16", torch.bfloat16):
+        return Engine.KV_BF16
+    if kv_cache_dtype in ("int8", torch.int8):
+        return Engine.KV_INT8
+    raise ValueError(f"kv_cache_dtype must be None, 'bfloat16', torch.bfloat16, 'int8' or torch.int8 (got {kv_cache_dtype!r})")
+
+
 class Engine:
     WEIGHT_BF16, WEIGHT_INT8 = 0, 1      # weight_format: storage of the LLaMA projections (int8 = load_in_8bit, include/vcla.h)
+    KV_BF16, KV_INT8 = 0, 1              # kv_format: storage of the paged KV cache (int8 = kv_cache_dtype="int8", include/vcla.h)
 
     def __init__(self, path_cfg: Dict, max_batch: int = 8, max_seq: int = 512, max_prefill_tokens: Optional[int] = None,
-                 device: Optional[torch.device] = None, page_tokens: int = 64, weight_format: int = 0):
+                 device: Optional[torch.device] = None, page_tokens: int = 64, weight_format: int = 0, kv_format: int = 0):
         if not torch.cuda.is_available():
             raise N.NativeError("visualcla (H100) needs a CUDA device: there is no CPU fallback")
         self.lib = N.load()
@@ -37,8 +48,10 @@ class Engine:
         self.max_batch, self.max_seq = int(max_batch), int(max_seq)
         self.max_prefill_tokens = int(max_prefill_tokens or max_batch * max_seq)
         cfg = N.VclaConfig(**self.path_cfg, max_batch=self.max_batch, max_seq=self.max_seq,
-                           max_prefill_tokens=self.max_prefill_tokens, page_tokens=page_tokens, weight_format=int(weight_format))
+                           max_prefill_tokens=self.max_prefill_tokens, page_tokens=page_tokens, weight_format=int(weight_format),
+                           kv_format=int(kv_format))
         self.weight_format = int(weight_format)
+        self.kv_format = int(kv_format)
         self._ctx = C.c_void_p()
         with torch.cuda.device(self.device):
             N.check(self.lib.vcla_create(C.byref(cfg), C.byref(self._ctx)), "vcla_create")
@@ -457,6 +470,13 @@ class Engine:
         a, b, c = C.c_int(), C.c_int(), C.c_int()
         N.check(self.lib.vcla_kv_geometry(self._ctx, C.byref(a), C.byref(b), C.byref(c)), "vcla_kv_geometry")
         return a.value, b.value, c.value
+
+    def kv_read_layer(self, layer: int) -> torch.Tensor:
+        """One layer's pool bytes (uint8, host): bf16 rows [pages][K|V][heads][page_tokens][128], or with the int8 cache the int8 rows in
+        that order followed by their fp32 scales (include/vcla.h).  Synchronises the device."""
+        out = torch.empty(self.memory_bytes()[1] // self.path_cfg["t_layers"], dtype=torch.uint8)
+        N.check(self.lib.vcla_kv_read_layer(self._ctx, int(layer), N.ptr(out)), "vcla_kv_read_layer")
+        return out
 
     def kv_pages(self):
         """-> (page_table (max_batch, pages_per_seq) int32, pages owned per sequence (max_batch,), free pages, exhausted flag)."""

@@ -23,7 +23,7 @@ import torch
 
 from . import _native as N
 from .configuration_visualcla import VisualCLAConfig
-from .engine import Engine, path_config_7b
+from .engine import Engine, kv_format_of, path_config_7b
 
 
 # --------------------------------------------------------------------------------------------------
@@ -113,7 +113,7 @@ class VisualCLAModel:
 
     def __init__(self, config: VisualCLAConfig = None, vision_model=None, text_model=None, device=None,
                  max_batch: int = 8, max_seq: int = 1024, max_prefill_tokens: Optional[int] = None,
-                 torch_dtype=torch.bfloat16, load_in_8bit: bool = False):
+                 torch_dtype=torch.bfloat16, load_in_8bit: bool = False, kv_cache_dtype=None):
         if config is None:
             raise ValueError("VisualCLAModel needs a VisualCLAConfig")
         if vision_model is not None or text_model is not None:
@@ -123,7 +123,8 @@ class VisualCLAModel:
         # load_in_8bit: the seven LLaMA projections of every layer become weight-only int8 with per-row scales (what bitsandbytes
         # converts in the reference, modeling_visualcla.py:151-156); everything else stays as it is
         self._engine = Engine(config.to_path_config(), max_batch=max_batch, max_seq=max_seq, max_prefill_tokens=max_prefill_tokens,
-                              device=device, weight_format=Engine.WEIGHT_INT8 if load_in_8bit else Engine.WEIGHT_BF16)
+                              device=device, weight_format=Engine.WEIGHT_INT8 if load_in_8bit else Engine.WEIGHT_BF16,
+                              kv_format=kv_format_of(kv_cache_dtype))
         self.dtype = torch.bfloat16      # compute dtype of the path (bf16 operands, fp32 accumulate / residual stream)
         self.requested_dtype = torch_dtype
         self.image_at_head = True        # constructor default of the reference (:108); the loader flips it (:134)
@@ -194,7 +195,7 @@ class VisualCLAModel:
         cfg = copy.deepcopy(self.config)
         cfg.text_config["vocab_size"] = int(new_num_tokens)
         new = Engine(cfg.to_path_config(), max_batch=e.max_batch, max_seq=e.max_seq, max_prefill_tokens=e.max_prefill_tokens, device=e.device,
-                     weight_format=e.weight_format)
+                     weight_format=e.weight_format, kv_format=e.kv_format)
         for n in q8:                        # int8 tensors move as stored (quantising q * s again could change them)
             new.load_weight_q8(n, *e.read_weight_q8(n))
         for k in ("text_model.model.embed_tokens.weight", "text_model.lm_head.weight"):
@@ -211,6 +212,11 @@ class VisualCLAModel:
         self.text_model.config = SimpleNamespace(**cfg.text_config)
         self._tok_buf = {}
         return self.get_input_embeddings()
+
+    @property
+    def kv_cache_dtype(self) -> torch.dtype:
+        """Storage of the KV cache: torch.int8 (int8 rows + one fp32 scale per token and head, kv_cache_dtype="int8") or torch.bfloat16."""
+        return torch.int8 if self._engine.kv_format == Engine.KV_INT8 else torch.bfloat16
 
     # ---- constructors -----------------------------------------------------------------------------
     @classmethod
